@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — scenes/sec (256×256×32 voxels @10 % occupancy) forward+backward, the BASELINE.json metric.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision fp32|bf16]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision fp32|bf16] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -15,6 +15,8 @@ Two timed regions, both bracketed by barrier + cuda.synchronize and CUDA events:
   e2e   : same K steps through the same public call with the step's inputs coming from pinned host
           memory (H2D inside the region, issued one step ahead on a copy stream) and the loss read back
           (asynchronous D2H into pinned memory) every step.
+`--dump-outputs DIR` writes what the last timed step returned (network outputs and loss) as DIR/<name>.npy, so that
+two builds can be compared output for output on identical seeded inputs.
 `--impl reference` times the CPU restatement of the MinkowskiEngine algorithm (oracle/) on the host
 cores on a bounded crop of the same workload (ME 0.5.4 itself is not installable offline, BASELINE.md §2).
 """
@@ -54,15 +56,8 @@ METRIC = "scenes/sec (256x256x32 voxels @10% occ) fwd+bwd"
 SHAPES = {"semkitti": dict(occ=0.10, in_ch=283, n_classes=20), "kitti360": dict(occ=0.08, in_ch=8, n_classes=19)}
 
 
-def _peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)), "measured"
-    return 6650.0, 1400.0, "fallback"
-
-
-NCU_FILE = "r02_ncu_conv_planes.json"
+# NVIDIA H100 SXM data sheet (dense, 700 W card): the denominators of the roofline fractions, not reached rates
+H100_HBM_GBS, H100_BF16_TFLOPS = 3350.0, 989.0
 
 
 def _kernel_name(kind, meta):
@@ -74,25 +69,62 @@ def _kernel_name(kind, meta):
     return "k_wgrad_tc" if kind == "wgrad" else "k_conv_tc"
 
 
-def _ncu_traffic(kind, meta):
-    """dram__bytes_read.sum + dram__bytes_write.sum (bytes) per launch of the dominant kernel from the committed
-    ncu --set full capture of the same layer shape (profiles/r02_ncu_conv_planes.json: N=1.05 M rows, C=64, bf16x3);
-    None if the dominant group is another shape or the capture is absent."""
-    if not (meta["Cin"] == 64 and meta["Cout"] == 64 and meta["K"] == 27 and 0.9e6 < meta["n_out"] < 1.2e6 and meta["precision"] == 3):
-        return None
+def _gpu_info(index: int):
+    """Name, power limit and max SM clock of the card: a measured rate is only meaningful with these beside it."""
     try:
-        d = json.load(open(os.path.join(ROOT, "profiles", NCU_FILE)))
-        want = _kernel_name(kind, meta)
-        for k in d["kernels"]:
-            if want in k["kernel"]:
-                return float(k["dram_bytes_per_launch"])
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                            "-i", str(index)], capture_output=True, text=True, timeout=10)
+        name, watts, mhz = [x.strip() for x in r.stdout.strip().split(",")]
+        return {"name": name, "power_limit_w": float(watts), "sm_max_mhz": int(float(mhz))}
     except Exception:
-        pass
-    return None
+        return {"name": torch.cuda.get_device_name(index)}
+
+
+def dump_outputs(out, loss, d, limit=1 << 20, budget=64 << 20):
+    """Writes the arrays one step returned (the network outputs and the loss) as d/<name>.npy in float32 / float64.
+    Sparse outputs are put in coordinate order (their row order depends on hashing); an array of more than `limit`
+    values is replaced by a fixed seeded sample of its rows; the files stop at `budget` bytes in all."""
+    import numpy as np
+    arrays = {}
+
+    def walk(x, name):
+        if isinstance(x, torch.Tensor):
+            arrays[name] = x.detach()
+        elif hasattr(x, "F") and hasattr(x, "C"):
+            C, F = x.C.detach().long(), x.F.detach()
+            order = torch.arange(C.shape[0], device=C.device)
+            for col in reversed(range(C.shape[1])):
+                order = order[torch.argsort(C[order, col], stable=True)]
+            arrays[name + ".C"], arrays[name + ".F"] = C[order], F[order]
+        elif isinstance(x, dict):
+            for k, v in x.items():
+                walk(v, f"{name}.{k}")
+        elif isinstance(x, (list, tuple)):
+            for i, v in enumerate(x):
+                walk(v, f"{name}.{i}")
+
+    walk(out, "out")
+    arrays["loss"] = loss.detach()
+    os.makedirs(d, exist_ok=True)
+    total = 0
+    for name, t in sorted(arrays.items()):
+        t = t if t.dtype == torch.float64 else t.float()
+        if t.dim() >= 1 and t.numel() > limit:
+            rows = max(1, limit // max(1, t[0].numel()))
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(t.shape[0], generator=g)[:rows].sort().values
+            t = t[idx.to(t.device)]
+        arr = t.cpu().numpy()
+        if total + arr.nbytes > budget:
+            log(f"dump-outputs: {budget >> 20} MB reached, {name} and later arrays not written")
+            break
+        np.save(os.path.join(d, name + ".npy"), arr)
+        total += arr.nbytes
+    log(f"dump-outputs: {total / 2**20:.1f} MB written to {d}")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         super().__init__(daemon=True)
@@ -173,8 +205,8 @@ def h2d_bytes(scene):
 
 # ------------------------------------------------------------------------------------------------------------
 def run_ours(a):
-    from pasco_b200 import build
-    build.build()
+    from pasco_b200 import _lib
+    _lib.load()                  # the library build() left in the tree (bench.py compiles nothing)
     from pasco_b200 import ops
     from pasco_b200.net3d import PascoNet
     from pasco_b200.losses import total_loss
@@ -212,6 +244,7 @@ def run_ours(a):
     torch.cuda.synchronize()
     # the reference's DDP gradient averaging (scripts/train.py:213): 64 MB buckets all-reduced while backward continues
     reducer = parallel.GradReducer(params, bucket_mb=a.bucket_mb) if world > 1 else None
+    last_out = {}
 
     def step(scene, micro=0):
         """One micro-step (one MIMO group of M scenes); the optimiser step closes on the last of ACC micro-steps
@@ -219,6 +252,8 @@ def run_ours(a):
         out = net(scene["in_feats"], scene["in_coords"], scene["global_min_Cs"], scene["global_max_Cs"],
                   scene["min_Cs"], scene["max_Cs"])
         loss = total_loss(out, scene, N_CLASSES, net.class_frequencies)
+        if a.dump_outputs:
+            last_out["out"], last_out["loss"] = out, loss
         if ACC > 1:
             loss = loss / ACC
         last = micro == ACC - 1
@@ -331,6 +366,9 @@ def run_ours(a):
     ms_e2e, _ = timed(a.steps, from_host=True)
     log(f"e2e region: {ms_e2e / a.steps:.1f} ms/step")
     clocks = sampler.stop() if sampler else None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(last_out["out"], last_out["loss"], a.dump_outputs)
+    last_out.clear()
     # per-launch CUDA events of the conv kernels (the roofline block) come from ONE extra step of the same workload run
     # right after the timed regions (same clocks, same allocator state): recording ~260 event pairs and the pair counts
     # inside a timed region cost 5-20 ms/step of host time in round 1 and made `value` slower than `e2e`
@@ -357,7 +395,7 @@ def run_ours(a):
         for key, g in sorted(groups.items(), key=lambda kv: -kv[1]["ms"])[:40]:
             log(f"  conv group {g['kind']:5s} n_out~{g['meta']['n_out']:8d} K={g['meta']['K']:3d} {g['meta']['Cin']:4d}->{g['meta']['Cout']:4d}: "
                 f"{g['n']:3d} launches, {g['ms'] / prof_steps:7.2f} ms/step, {g['flops'] / g['ms'] / 1e9:6.1f} useful TFLOP/s")
-    hbm_peak, tf_peak, peak_src = _peaks()
+    hbm_peak, tf_peak, peak_src = H100_HBM_GBS, H100_BF16_TFLOPS, "NVIDIA H100 SXM data sheet (dense BF16, HBM3)"
     roof = None
     if groups:
         top = max(groups.values(), key=lambda g: g["ms"])
@@ -367,8 +405,7 @@ def run_ours(a):
         m = top["meta"]
         roof = {"kernel": f"{_kernel_name(top['kind'], m)}<{m['precision']}> {top['kind']} K={m['K']} {m['Cin']}->{m['Cout']} n_out~{m['n_out']}",
                 "bound": "tensor", "achieved": round(ach_tf, 2), "peak": tf_peak, "unit": "TFLOP/s",
-                "frac": round(ach_tf / tf_peak, 4), "traffic": _ncu_traffic(top["kind"], m),
-                "traffic_source": f"dram__bytes_read.sum + dram__bytes_write.sum per launch, profiles/{NCU_FILE} (same layer shape)",
+                "frac": round(ach_tf / tf_peak, 4),
                 "algorithmic_bytes_per_launch": round(top["bytes"] / top["n"]), "peak_source": peak_src,
                 "launch_ms": round(per_launch_ms, 4), "launches": top["n"],
                 "algorithmic": "flops = 2*pairs*Cin*Cout per launch (useful MACs; bf16x3 issues 3x that on the tensor pipe)",
@@ -393,12 +430,12 @@ def run_ours(a):
                 if a.precision == "fp32" else "bf16 operands, fp32 accumulate", "data": "synthetic",
                 "config": {"workload": workload, "global_batch": scenes_per_step, "accum": ACC, "n_infers": M, "shape": a.shape,
                            "loss": "CE+Lovasz completion @3 scales + Hungarian set loss (class CE, focal, dice, 3 aux levels)",
-                           "parallelism": f"dp{world}", "l2": "inputs larger than L2: per-step working set (>4 GB of activations) >> 126 MB",
+                           "parallelism": f"dp{world}", "l2": "inputs larger than L2: per-step working set (>4 GB of activations) >> 50 MB",
                            "scene_pool": n_pool, "random_init_weights": True, "settle_steps": SETTLE},
                 "e2e": {"value": round(scenes_per_step * a.steps / (ms_e2e / 1e3), 4), "unit": "scenes/s",
                         "h2d_bytes_per_step": h2d_bytes(host_scenes[0]) * ACC, "d2h_bytes_per_step": 4,
                         "ms_per_step": round(ms_e2e / a.steps, 3)},
-                "gpu_launches": launches, "clocks": clocks, "roofline": roof}
+                "gpu_launches": launches, "gpu": _gpu_info(local), "clocks": clocks, "roofline": roof}
         if world == 1 and not a.no_cpu_baseline:
             line["cpu_baseline"] = cpu_baseline(a.cpu_seconds)
         print(json.dumps(line), flush=True)
@@ -477,6 +514,8 @@ if __name__ == "__main__":
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--bucket-mb", type=float, default=64.0, help="gradient all-reduce bucket size (N > 1)")
     ap.add_argument("--ref-full-scene", action="store_true", help="--impl reference: also time one unscaled full scene")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the network outputs and loss of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* pasco_sm100.h — C ABI of libpasco_sm100.so, the sm_100a sparse-voxel engine that sits
+/* pasco_sm100.h — C ABI of libpasco_sm100.so, the sm_90a sparse-voxel engine that sits
  * underneath PaSCo's operator surface.
  *
  * Every entry point replaces one granule of the MinkowskiEngine 0.5.4 pybind backend
@@ -121,11 +121,11 @@ int pasco_dense_occupancy(const float* dense, int32_t B, int32_t C, int64_t cell
 /* ---- sparse convolution (ME ConvolutionForward/Backward: every conv on the path) -------------
  * out[o,:] = sum_k in[nbr[k,o],:] @ W[k]        W: float32 [K, Cin, Cout]
  *
- * Tensor-core path (tcgen05, bf16 split operands, fp32 accumulate in TMEM):
+ * Tensor-core path (wgmma, bf16 split operands, fp32 accumulate in registers):
  *   precision 1 = bf16 operands (1 MMA / k-step), 3 = bf16x3 split (hi·hi + lo·hi + hi·lo,
  *   ~2^-16 relative: the "fp32" mode of BASELINE.json configs[1]).
  *   Requires Cin % 64 == 0, Cout % 16 == 0, 16 <= Cout <= 256.
- * Weights are first packed into the UMMA shared-memory image:
+ * Weights are first packed into the swizzled shared-memory operand image:
  *   transpose=0: B[n=co][k=ci] = W[k][ci][co]      (forward)
  *   transpose=1: B[n=ci][k=co] = W[k][ci][co]      (input gradient; swap Cin/Cout in the conv call)
  * packed size in bytes = pasco_conv_packed_bytes(K, Cin, Cout).                                 */
@@ -145,7 +145,7 @@ int pasco_conv_forward_tc(const float* in, int64_t n_in, const int32_t* nbr, int
                           double* stats, float* out, int32_t precision, int64_t in_pitch, int64_t out_pitch,
                           pasco_stream_t s);
 /* Split-K form of the same convolution for shapes with few output tiles and many offsets (the dense bottleneck of
- * layers.py:646-726 runs as 32 tiles x 245 offsets: one CTA per tile would leave 116 of 148 SMs idle).  The offsets are
+ * layers.py:646-726 runs as 32 tiles x 245 offsets: one CTA per tile would leave most SMs idle).  The offsets are
  * cut into ranges, every (tile, range) pair is a work item whose partial result goes to the caller's workspace, and a
  * second kernel adds the partials in a fixed order (+ bias) — still deterministic, no atomics.
  * pasco_conv_splitk_workspace_bytes returns 0 when the shape is not worth splitting (then call pasco_conv_forward_tc). */
@@ -159,7 +159,7 @@ int pasco_conv_forward_splitk(const float* in, int64_t n_in, const int32_t* nbr,
 /* Plane-gather path (the default for every gathered convolution): the activations are split ONCE per tensor into bf16
  * planes x = hi + lo (lo = NULL for precision 1) by pasco_split_planes — optionally fused with y = act(x*scale + shift),
  * the BatchNorm + activation of the producing layer — and the convolution / weight-gradient producers move plane rows
- * with 16-byte cp.async copies straight into the swizzled UMMA tiles (missing neighbours are zero-fill copies that touch
+ * with 16-byte cp.async copies straight into the swizzled operand tiles (missing neighbours are zero-fill copies that touch
  * no memory).  Planes are bf16 [N, C] with a row pitch in ELEMENTS (0 = C); C % 8 == 0.
  * pasco_conv_forward_planes: forward and input gradient (same contract as pasco_conv_forward_tc: koff_map, bias, fused
  * BatchNorm statistics of `out` in `stats`);  pasco_conv_wgrad_planes: dW (zeroed by the caller) from the planes of the
@@ -174,7 +174,7 @@ int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int64_t n_in, 
                             int64_t n_out, int32_t Cin, int32_t Cout, const void* g_hi, const void* g_lo, float* dW,
                             int32_t precision, int64_t in_pitch, int64_t gout_pitch, pasco_stream_t s);
 
-/* dW[k] = sum_o in[nbr[k,o],:]^T @ gout[o,:]   (tcgen05, MN-major operands); dW float32 [K,Cin,Cout] zeroed by caller */
+/* dW[k] = sum_o in[nbr[k,o],:]^T @ gout[o,:]   (wgmma, MN-major operands); dW float32 [K,Cin,Cout] zeroed by caller */
 int pasco_conv_wgrad_tc(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out, int32_t Cin,
                         int32_t Cout, const float* gout, const float* in_scale, const float* in_shift,
                         int32_t in_act, float* dW, int32_t precision, int64_t in_pitch, int64_t gout_pitch,
@@ -221,14 +221,14 @@ int pasco_bn_bwd_apply(const float* dy, const float* x, int64_t n, int32_t C, co
 /* ---- MaskPLS masked cross-attention (pasco/models/transformer/blocks.py:73-92 with the attention mask of
  *      transformer_predictor_v2.py:220-289): Q <= 128 queries against all P voxels, H heads of width D <= 64 ------
  * q [Q, H*D], k / v [P, H*D] float32 (already projected); logits = scale * q.k; mask = bit rows
- * uint32 [Q, 2*ceil(P/64)] (bit j of word 2t + j/32 set = key 64t + j masked) or NULL; out [Q, H*D] ZEROED by the
- * caller; lse [H, Q] receives log-sum-exp per row (needed by the backward).  Two streaming passes over K (row
- * statistics, then output), tcgen05 for both GEMMs, bf16x3 split operands.                                        */
+ * uint32 [Q, 2*ceil(P/64)] (bit j of word 2t + j/32 set = key 64t + j masked) or NULL; out [Q, H*D] is overwritten
+ * (the key chunks' shares are summed in a fixed order); lse [H, Q] receives log-sum-exp per row (needed by the backward).  Two streaming passes over K (row
+ * statistics, then output), wgmma for both GEMMs, bf16x3 split operands.                                          */
 int64_t pasco_xattn_workspace_bytes(int32_t Q, int64_t P, int32_t H, int32_t D);
 int pasco_xattn_forward(const float* q, const float* k, const float* v, const uint32_t* mask, int32_t Q, int64_t P,
                         int32_t H, int32_t D, float scale, float* out, float* lse, float* workspace,
                         int64_t workspace_bytes, pasco_stream_t s);
-/* backward of the above: recomputes the probabilities from lse; dq [Q, H*D] ZEROED by the caller (fp32 red.add),
+/* backward of the above: recomputes the probabilities from lse; dq [Q, H*D] is overwritten (chunk shares, fixed order),
  * dk / dv [P, H*D] are fully overwritten (every row written exactly once, no atomics).                            */
 int pasco_xattn_backward(const float* q, const float* k, const float* v, const uint32_t* mask, const float* lse,
                          const float* out, const float* dout, int32_t Q, int64_t P, int32_t H, int32_t D, float scale,

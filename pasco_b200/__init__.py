@@ -1,4 +1,4 @@
-"""pasco_b200 — B200-native (sm_100a) sparse-voxel engine behind PaSCo's operator surface.
+"""pasco_b200 — H100-native (sm_90a) sparse-voxel engine behind PaSCo's operator surface.
 
     pasco_b200.me       MinkowskiEngine-compatible API (the drop-in boundary; compat/MinkowskiEngine re-exports it)
     pasco_b200.ops      tensor-level wrappers / autograd Functions over the C-ABI

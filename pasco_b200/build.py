@@ -1,4 +1,4 @@
-"""Builds libpasco_sm100.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libpasco_sm100.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m pasco_b200.build [--force]
 """
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libpasco_sm100.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-DPASCO_NO_FAST_MATH"] + os.environ.get("PASCO_NVCC_FLAGS", "").split()
 
 
@@ -48,7 +48,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(run, jobs))
     if force or jobs or _stale(LIB, objs):
-        run([NVCC, "-shared", "-o", LIB, *objs, "-lcudart"])
+        run([NVCC, *FLAGS[:2], "-shared", "-o", LIB, *objs, "-lcudart"])
     return LIB
 
 

@@ -1,8 +1,9 @@
-// Shared helpers for libpasco_sm100 (sm_100a only).
+// Shared helpers for libpasco_sm100 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <mutex>
 #include "../../include/pasco_sm100.h"
 
 namespace pasco {
@@ -65,9 +66,41 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
+}
+
+// stream-ordered workspace of a call (freed with cudaFreeAsync on the same stream), from a memory pool of the library's
+// own per device.  The pool keeps freed blocks (release threshold = unlimited) instead of returning them to the driver
+// at every synchronisation, so a per-call workspace costs no re-mapping from one training step to the next; it holds
+// at most the largest workspace in flight and lives as long as the process.  The default pool is left untouched.
+inline cudaError_t ws_alloc(void** p, size_t bytes, cudaStream_t st) {
+  static std::mutex mu;
+  static cudaMemPool_t pools[64] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  cudaMemPool_t pool;
+  {
+    std::lock_guard<std::mutex> lock(mu);
+    if (!pools[dev]) {
+      cudaMemPoolProps props = {};
+      props.allocType = cudaMemAllocationTypePinned;
+      props.location.type = cudaMemLocationTypeDevice;
+      props.location.id = dev;
+      e = cudaMemPoolCreate(&pools[dev], &props);
+      if (e != cudaSuccess) {
+        pools[dev] = nullptr;
+        return e;
+      }
+      uint64_t keep = ~0ull;
+      cudaMemPoolSetAttribute(pools[dev], cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+    pool = pools[dev];
+  }
+  return cudaMallocFromPoolAsync(p, bytes, pool, st);
 }
 
 inline int grid_for(int64_t work, int block, int waves = 8) {

@@ -1,14 +1,14 @@
-// Pre-split bf16 planes of an activation tensor (sm_100a): x = hi + lo with hi = bf16(x), lo = bf16(x - hi).
+// Pre-split bf16 planes of an activation tensor (sm_90a): x = hi + lo with hi = bf16(x), lo = bf16(x - hi).
 //
 // The plane-gather convolution kernels (k_conv_pl in conv_tc.cu, k_wgrad_pl in wgrad_tc.cu) read their gathered
 // operand from these planes with 16-byte cp.async copies, so the split (and, optionally, the BatchNorm affine +
 // activation of the layer that produced x) is done ONCE per tensor here instead of once per kernel offset inside the
 // gather.  HBM-bound: reads 4 B and writes 4 B (2 B in bf16 mode) per element.
 #include "common.cuh"
-#include "umma.cuh"
+#include "gmma.cuh"
 
 using namespace pasco;
-using namespace umma;
+using namespace gmma;
 
 namespace {
 

@@ -1,5 +1,5 @@
 // CUDA-core fp32 path of the sparse-conv contraction  out[o,:] = Σ_k in[nbr[k,o],:] @ W[k].
-// Any Cin/Cout.  This is the in-library cross-check for the tcgen05 path (conv_tc.cu) and serves the
+// Any Cin/Cout.  This is the in-library cross-check for the tensor-core path (conv_tc.cu) and serves the
 // shapes the tensor-core kernel does not take (channel counts that are not multiples of 64/16).
 #include "common.cuh"
 
@@ -90,20 +90,22 @@ extern "C" int pasco_conv_forward_simt(const float* in, const int32_t* nbr, int3
   return 0;
 }
 
-// dW[k][ci][co] = Σ_o in[nbr[k,o]][ci] * gout[o][co];  grid = (row chunks, K); fp32 atomics into dW
-constexpr int WG_ROWS = 2048;  // rows per block
+// dW[k][ci][co] = Σ_o in[nbr[k,o]][ci] * gout[o][co];  grid = (row blocks, K); each block stores its partial sums
+constexpr int WG_ROWS = 2048;  // minimum rows per block
 constexpr int WG_TILE = 16;    // rows staged per iteration
+constexpr int WG_MAX_BLOCKS = 128;
+constexpr int64_t WG_MAX_WS_FLOATS = 16 << 20;   // workspace bound: 64 MB of per-block partials
 
 __global__ void __launch_bounds__(256)
-k_wgrad_simt(const float* __restrict__ in, const int32_t* __restrict__ nbr, int64_t n_out, int Cin, int Cout,
-             const float* __restrict__ gout, float* __restrict__ dW) {
+k_wgrad_simt(const float* __restrict__ in, const int32_t* __restrict__ nbr, int64_t n_out, int64_t rows, int Cin, int Cout,
+             const float* __restrict__ gout, float* __restrict__ part) {
   extern __shared__ float sm[];  // sA[WG_TILE][Cin], sG[WG_TILE][Cout]
   float* sA = sm;
   float* sG = sm + WG_TILE * Cin;
   __shared__ int sIdx[WG_TILE];
   int k = blockIdx.y;
-  int64_t r0 = (int64_t)blockIdx.x * WG_ROWS;
-  int64_t r1 = r0 + WG_ROWS < n_out ? r0 + WG_ROWS : n_out;
+  int64_t r0 = (int64_t)blockIdx.x * rows;
+  int64_t r1 = r0 + rows < n_out ? r0 + rows : n_out;
   int total = Cin * Cout;
   // each thread owns outputs e = threadIdx.x + j*256 (ci = e / Cout, co = e % Cout)
   constexpr int MAXE = 16;  // up to 4096 outputs per pass
@@ -146,8 +148,17 @@ k_wgrad_simt(const float* __restrict__ in, const int32_t* __restrict__ nbr, int6
 #pragma unroll
     for (int j = 0; j < MAXE; ++j) {
       int e = e0 + threadIdx.x + j * 256;
-      if (e < total && acc[j] != 0.f) atomicAdd(dW + (int64_t)k * total + e, acc[j]);
+      if (e < total) part[((int64_t)blockIdx.x * gridDim.y + k) * total + e] = acc[j];
     }
+  }
+}
+
+// dW[i] += Σ_b part[b][i] in block order (deterministic, no atomics)
+__global__ void k_wgrad_simt_sum(const float* __restrict__ part, int nb, int64_t n, float* __restrict__ dW) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float acc = 0.f;
+    for (int b = 0; b < nb; ++b) acc += __ldg(part + b * n + i);
+    dW[i] += acc;
   }
 }
 
@@ -157,8 +168,26 @@ extern "C" int pasco_conv_wgrad_simt(const float* in, const int32_t* nbr, int32_
   size_t smem = (size_t)WG_TILE * (Cin + Cout) * sizeof(float);
   PASCO_CHECK_ARG(smem <= 200 * 1024, "pasco_conv_wgrad_simt: channels too large");
   if (smem > 48 * 1024) cudaFuncSetAttribute(k_wgrad_simt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  dim3 grid((unsigned)((n_out + WG_ROWS - 1) / WG_ROWS), K);
-  k_wgrad_simt<<<grid, 256, smem, (cudaStream_t)s>>>(in, nbr, n_out, Cin, Cout, gout, dW);
+  // at most WG_MAX_BLOCKS row blocks (fewer when K*Cin*Cout is large, so that the workspace stays within 64 MB), whose
+  // partials go to a stream-ordered workspace and are summed in block order
+  const int64_t n = (int64_t)K * Cin * Cout;
+  int64_t max_blocks = WG_MAX_WS_FLOATS / n;
+  if (max_blocks > WG_MAX_BLOCKS) max_blocks = WG_MAX_BLOCKS;
+  if (max_blocks < 1) max_blocks = 1;
+  int64_t rows = (n_out + max_blocks - 1) / max_blocks;
+  if (rows < WG_ROWS) rows = WG_ROWS;
+  rows = (rows + WG_TILE - 1) / WG_TILE * WG_TILE;
+  const int nb = (int)((n_out + rows - 1) / rows);
+  cudaStream_t st = (cudaStream_t)s;
+  float* part = nullptr;
+  cudaError_t e = ws_alloc((void**)&part, (size_t)nb * n * sizeof(float), st);
+  if (e != cudaSuccess) {
+    ::pasco::set_error("pasco_conv_wgrad_simt: workspace of %lld bytes: %s", (long long)nb * n * 4, cudaGetErrorString(e));
+    return -1;
+  }
+  k_wgrad_simt<<<dim3((unsigned)nb, K), 256, smem, st>>>(in, nbr, n_out, rows, Cin, Cout, gout, part);
+  k_wgrad_simt_sum<<<grid_for(n, 256), 256, 0, st>>>(part, nb, n, dW);
+  cudaFreeAsync(part, st);
   PASCO_CHECK_LAUNCH("pasco_conv_wgrad_simt");
   return 0;
 }

@@ -1,49 +1,51 @@
-// Sparse convolution on the 5th-gen tensor cores (tcgen05 + TMEM), sm_100a.
+// Sparse convolution on the Hopper tensor cores (wgmma), sm_90a.
 //
 //   out[o, :] = Σ_k  in[nbr[k, o], :] @ W[k]           (output-stationary implicit GEMM)
 //
-// One persistent CTA per SM walks 128-row output tiles.  Warp roles:
-// A CTA owns a GROUP of T = 256/Cout consecutive tiles whose accumulators live side by side in TMEM, and walks
-// group → offset k → 64-channel block → tile, so every weight slice W[k] is fetched from L2 once per group
-// instead of once per tile.
-//   warps 0-3  gather: load the neighbour rows of a tile (coalesced 16-byte loads, 16 lanes per 256-byte row
-//              segment; neighbour indices arrive through a cp.async ring one offset ahead), optionally apply
-//              the fused BatchNorm affine + activation of the producing layer, split fp32 → bf16 hi (+ lo), and
-//              store the 128x64 tile into shared memory in the 128-byte-swizzled K-major UMMA layout.  Loads of
-//              slot s+1 are in flight in registers while slot s is converted and stored.
-//   warp  9    streams the pre-swizzled weight slices with bulk async copies (UBLKCP) into their own ring.
-//   warp  8    one elected thread issues tcgen05.mma (M=128, N=Cout, K=16) into the tile's TMEM accumulator
-//              and commits to the A / B "empty" mbarriers; accumulator sets are double-buffered in TMEM so
-//              the epilogue of group g overlaps the main loop of group g+1.
-//   warps 4-7  epilogue: tcgen05.ld the accumulators (lane = output row), add bias, store fp32 rows.
+// One persistent CTA per SM walks work items of 128-row output tiles.  A work item is a GROUP of T consecutive tiles
+// (T x the item's columns <= 128 accumulator columns) and walks offset k → 64-channel block → tile, so every weight
+// slice W[k] is fetched from L2 once per group instead of once per tile.  Outputs wider than 128 channels are cut into
+// column ranges, one work item each.  Warp roles:
+//   warps 0-7   gather: load the neighbour rows of a tile (coalesced 16-byte loads, 16 lanes per 256-byte row
+//               segment; neighbour indices arrive through a cp.async ring one offset ahead), optionally apply
+//               the fused BatchNorm affine + activation of the producing layer, split fp32 → bf16 hi (+ lo), and
+//               store the 128x64 tile into shared memory in the 128-byte-swizzled K-major layout.  Loads of
+//               slot s+1 are in flight in registers while slot s is converted and stored.
+//   warps 8-15  two consumer warpgroups: warpgroup g issues wgmma (M=64 rows [64 g, 64 g + 64), N=64 or 16, K=16)
+//               into register accumulators, then adds the bias and stores its fp32 rows.
+//   warp  16    streams the pre-swizzled weight slices with bulk async copies into their own ring (warps 17-19 only
+//               complete its warpgroup, whose registers go to the gather and consumer warpgroups).
 // No atomics: every output row is written exactly once, results are run-to-run deterministic.
 //
 // precision 3 (the "fp32" mode): operands split as x = hi + lo (bf16 each) and three MMAs
 // hi·hi + lo·hi + hi·lo accumulate in fp32 — ~2^-16 relative error, well inside the 1e-3 parity bound.
 #include "common.cuh"
-#include "umma.cuh"
+#include "gmma.cuh"
 #include <cstdlib>
 
 using namespace pasco;
-using namespace umma;
+using namespace gmma;
 
 namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int KBLK = 64;                    // channels per K-block (= one 128-byte swizzle row of bf16)
 constexpr int A_TILE_BYTES = BLOCK_M * 128; // 16 KB
-#ifndef PASCO_GATHER_WARPS
-#define PASCO_GATHER_WARPS 8
-#endif
-constexpr int NUM_GATHER_WARPS = PASCO_GATHER_WARPS;            // 8 (16 tile rows each) or 16 (8 rows each)
-constexpr int NUM_EPI_WARPS = 4;                                // next 4 warps: warp % 4 = TMEM lane quadrant
-constexpr int MMA_WARP = NUM_GATHER_WARPS + NUM_EPI_WARPS;
-constexpr int LOAD_WARP = MMA_WARP + 1;
-constexpr int NUM_THREADS = (LOAD_WARP + 1) * 32;              // 448 / 704
-constexpr int ROWS_PER_WARP = BLOCK_M / NUM_GATHER_WARPS;       // 16 / 8
+constexpr int NUM_GATHER_WARPS = 8;                             // 16 tile rows each
+constexpr int NUM_CONS_WARPS = 8;                               // two consumer warpgroups
+constexpr int CONS_WARP0 = NUM_GATHER_WARPS;                    // warpgroup-aligned (a multiple of 4)
+constexpr int LOAD_WARP = CONS_WARP0 + NUM_CONS_WARPS;          // first warp of the last warpgroup; its 3 others idle
+constexpr int NUM_THREADS = (LOAD_WARP + 4) * 32;              // 640 = 5 warpgroups (96 registers each at launch)
+// setmaxnreg budgets (640 x 96 at launch): the loader warpgroup keeps 24 and the registers it releases go to the gather
+// and consumer warpgroups, 2 x 128 x (GATHER_REGS - 96) + 2 x 128 x (CONS_REGS - 96) <= 128 x (96 - 24).  With these
+// budgets ptxas reports no spills in any variant (at 96 the register-gather producers spilled).
+constexpr int GATHER_REGS = 112, CONS_REGS = 112, LOAD_REGS = 24;
+static_assert(2 * 128 * (GATHER_REGS - 96) + 2 * 128 * (CONS_REGS - 96) <= 128 * (96 - LOAD_REGS), "setmaxnreg budget");
+constexpr int ROWS_PER_WARP = BLOCK_M / NUM_GATHER_WARPS;       // 16
 constexpr int LOADS_PER_SLOT = ROWS_PER_WARP / 2;               // float4 per lane per slot
 constexpr int TILES_PER_IDX_STEP = 32 / ROWS_PER_WARP;          // tiles whose indices one warp-wide cp.async covers
 constexpr int MAX_STAGES = 8;
+constexpr int ACC_COLS = 128;               // accumulator columns per consumer warpgroup (64 fp32 registers per thread)
 
 struct ConvParams {
   const float* in;
@@ -58,15 +60,15 @@ struct ConvParams {
   int64_t out_pitch;   // row stride of out (floats)
   int64_t in_pitch;    // row stride of in (floats)
   int K, Cin, Cout, in_act;
-  int sa, sb, tiles_per_group, tmem_cols;
+  int sa, sb, tiles_per_group;
+  int nsplit, ncols;          // output columns in ranges of ncols (the last one may be narrower), one work item each
   int koff_base, koff_step;   // weight slice of table row k = koff_base + koff_step * k
-  int ksplit, kchunk;         // split-K: work item v = (tile group v / ksplit, offsets [ks*kchunk, (ks+1)*kchunk)), partial
-                              // results go to out + ks * n_out * out_pitch (summed by k_splitk_reduce)
+  int ksplit, kchunk;         // split-K: offset range ks covers [ks*kchunk, (ks+1)*kchunk); partial results go to
+                              // out + ks * n_out * out_pitch (summed by k_splitk_reduce)
   // k_conv_pl only: the input as pre-split bf16 planes x = hi + lo, [n_in, Cin] each with row pitch pl_pitch (elements)
   const uint16_t* pl_hi;
   const uint16_t* pl_lo;
   int64_t pl_pitch;
-  int pl_depth;               // slots whose copies are in flight per producer thread before the oldest is published
 };
 
 // ------------------------------------------------------------------------------------------------------------
@@ -127,8 +129,8 @@ constexpr int IDX_RING = 6;  // neighbour-index ring depth (entries of T*128 int
 
 // position of a gather warp inside the flat slot sequence  group → k → kb → t
 struct SlotIt {
-  int64_t v;       // work item handled by this CTA: tile group v / ksplit, offset range number v % ksplit
-  int64_t group;   // = v / ksplit
+  int64_t v;       // work item handled by this CTA
+  int64_t group;   // = item_group(v)
   int gk;          // running (work item, k) counter → index ring slot
   int k, k1, kb, t;  // k walks [k0(v), k1(v))
   int t_eff;       // tiles in this group
@@ -141,27 +143,39 @@ struct SlotIt {
 struct Pipe {
   uint8_t* a_smem;          // [sa][A_hi | A_lo]
   uint8_t* b_smem;          // [sb][B_hi | B_lo]
-  uint64_t *afull, *aempty, *bfull, *bempty, *tfull, *tempty;
-  uint32_t tmem_base;
+  uint64_t *afull, *aempty, *bfull, *bempty;
   double* stat_acc;         // [2*Cout] per-CTA accumulators in shared memory (nullptr: no fused statistics)
-  int a_stage_bytes, b_stage_bytes, b_tile;
-  int KB, T, acc_cols;
-  int64_t num_tiles, num_groups;
+  int a_stage_bytes, b_tile;
+  int KB, T;
+  int64_t num_tiles, num_groups, num_items;
 };
 
-// one thread: streams the pre-swizzled weight slices with bulk async copies (UBLKCP) into the B ring
-__device__ __forceinline__ void role_weight_loader(const ConvParams& p, const Pipe& pl) {
+// work item v = (tile group, offset range, column range): columns vary fastest, then offset ranges
+__device__ __forceinline__ int64_t item_group(const ConvParams& p, int64_t v) { return v / ((int64_t)p.ksplit * p.nsplit); }
+__device__ __forceinline__ int item_ks(const ConvParams& p, int64_t v) { return (int)((v / p.nsplit) % p.ksplit); }
+__device__ __forceinline__ int item_n0(const ConvParams& p, int64_t v) { return (int)(v % p.nsplit) * p.ncols; }
+__device__ __forceinline__ int item_ncols(const ConvParams& p, int64_t v) {
+  const int n0 = item_n0(p, v);
+  return p.Cout - n0 < p.ncols ? p.Cout - n0 : p.ncols;
+}
+
+// one thread: streams the pre-swizzled weight slices (the item's column range of the hi [and lo] image) with bulk async
+// copies into the B ring
+__device__ __forceinline__ void role_weight_loader(const ConvParams& p, const Pipe& pl, int n_op) {
   int stage = 0;
   uint32_t phase = 0;
-  const uint32_t bytes = (uint32_t)pl.b_stage_bytes;
-  for (int64_t v = blockIdx.x; v < pl.num_groups * p.ksplit; v += gridDim.x) {
-    const int k0 = (int)(v % p.ksplit) * p.kchunk, k1 = k0 + p.kchunk < p.K ? k0 + p.kchunk : p.K;
+  for (int64_t v = blockIdx.x; v < pl.num_items; v += gridDim.x) {
+    const int k0 = item_ks(p, v) * p.kchunk, k1 = k0 + p.kchunk < p.K ? k0 + p.kchunk : p.K;
+    const int n0 = item_n0(p, v);
+    const uint32_t bytes = (uint32_t)item_ncols(p, v) * 128u;
     for (int k = k0; k < k1; ++k) {
       for (int kb = 0; kb < pl.KB; ++kb) {
         mbar_wait(smem_u32(pl.bempty + stage), phase ^ 1);
-        mbar_arrive_expect_tx(smem_u32(pl.bfull + stage), bytes);
-        const uint8_t* src = p.wpk + ((int64_t)(p.koff_base + p.koff_step * k) * pl.KB + kb) * (int64_t)p.Cout * 256;
-        bulk_g2s(smem_u32(pl.b_smem + (size_t)stage * pl.b_stage_bytes), src, bytes, smem_u32(pl.bfull + stage));
+        mbar_arrive_expect_tx(smem_u32(pl.bfull + stage), bytes * n_op);
+        const uint8_t* src = p.wpk + ((int64_t)(p.koff_base + p.koff_step * k) * pl.KB + kb) * (int64_t)p.Cout * 256 + n0 * 128;
+        const uint32_t dst = smem_u32(pl.b_smem + (size_t)stage * n_op * pl.b_tile);
+        bulk_g2s(dst, src, bytes, smem_u32(pl.bfull + stage));
+        if (n_op == 2) bulk_g2s(dst + pl.b_tile, src + (int64_t)p.Cout * 128, bytes, smem_u32(pl.bfull + stage));
         if (++stage == p.sb) {
           stage = 0;
           phase ^= 1;
@@ -171,166 +185,136 @@ __device__ __forceinline__ void role_weight_loader(const ConvParams& p, const Pi
   }
 }
 
-// one thread: tcgen05.mma (M=128, N=Cout, K=16) into the tile's TMEM accumulator; commits free the A / B ring slots
-// `nm` issuer threads (one per warp) share the work: issuer `mid` owns the tiles t ≡ mid (mod nm) of every group — tiles
-// of a group accumulate into different TMEM columns, so their MMAs are independent.  One issuer needs ~100 cycles of
-// descriptor / uniform-register work per tcgen05.mma while an M=128, N=64 MMA executes in 32: with a single issuer the
-// tensor pipe idled at 30 % (ncu: the issuer thread busy on every instruction of its loop, producers waiting for stages).
-// The "B stage free" and "accumulators ready" barriers expect one commit per issuer.
-template <int NSPLIT, bool CPASYNC_A = false>
-__device__ __forceinline__ void role_mma(const ConvParams& p, const Pipe& pl, int mid = 0, int nm = 1) {
-  // Called by a WHOLE warp: waits, counters and descriptor arithmetic are warp-uniform (the compiler keeps them in uniform
-  // registers), only tcgen05.mma / tcgen05.commit are issued by the elected lane.  (With the loop inside `if (lane == 0)`
-  // every descriptor went through ELECT + R2UR moves: ~13 instructions and ~100 cycles per 32-cycle MMA.)
-  const bool lead = elect_one();
-  const uint32_t idesc = make_idesc_bf16(BLOCK_M, p.Cout, 0, 0);
+// Consumer warpgroup g (0 or 1) owns rows [64 g, 64 g + 64) of every tile of a group: it issues wgmma
+// (M = 64, N = CH per instruction, K = 16) over the A and B rings into register accumulators, then stores the finished
+// rows itself.  acc[c] holds accumulator columns [c CH, c CH + CH); the group's T tiles sit side by side, tile t in
+// columns [t ncols, (t + 1) ncols).  Every consumer warp arrives on the ring "empty" barriers (expected count 8), so a
+// stage is refilled only after both warpgroups' MMAs on it have completed.
+// The epilogue adds the bias, stores fp32 rows and optionally accumulates the per-channel sum and sum of squares of
+// what was stored (the BatchNorm statistics of the next layer): per warp over its rows with shuffles, then in fp64 in
+// shared memory, one global fp64 atomic per channel and CTA.
+template <int NSPLIT, bool CPASYNC_A, int CH>
+__device__ __forceinline__ void role_consumer(const ConvParams& p, const Pipe& pl, int g, int wq, int lane) {
+  constexpr int NCH = ACC_COLS / CH;
+  float acc[NCH][CH / 2];
+  const bool want_stats = pl.stat_acc != nullptr;
   int sa = 0, sb = 0;
   uint32_t pa = 0, pb = 0;
-  int it = 0;
-  for (int64_t v = blockIdx.x; v < pl.num_groups * p.ksplit; v += gridDim.x, ++it) {
-    const int buf = it & 1;
-    const int64_t group = v / p.ksplit;
-    const int k0 = (int)(v % p.ksplit) * p.kchunk, k1 = k0 + p.kchunk < p.K ? k0 + p.kchunk : p.K;
-    const int64_t rem = pl.num_tiles - group * pl.T;
-    const int t_eff = pl.T;        // the last group is padded to T tiles (rows >= n_out: never gathered, never stored)
-    (void)rem;
-    mbar_wait(smem_u32(pl.tempty + buf), ((it >> 1) & 1) ^ 1);
-    tc_fence_after();
+  for (int64_t v = blockIdx.x; v < pl.num_items; v += gridDim.x) {
+    const int64_t group = item_group(p, v);
+    const int k0 = item_ks(p, v) * p.kchunk, k1 = k0 + p.kchunk < p.K ? k0 + p.kchunk : p.K;
+    const int ncols = item_ncols(p, v);
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int i = 0; i < CH / 2; ++i) acc[c][i] = 0.f;
     for (int k = k0; k < k1; ++k) {
       for (int kb = 0; kb < pl.KB; ++kb) {
         mbar_wait(smem_u32(pl.bfull + sb), pb);
-        const uint32_t b_hi = smem_u32(pl.b_smem + (size_t)sb * pl.b_stage_bytes), b_lo = b_hi + pl.b_tile;
-        for (int t = 0; t < t_eff; ++t) {
-          if (t % nm == mid) {
+        const uint32_t b_hi = smem_u32(pl.b_smem + (size_t)sb * (NSPLIT == 3 ? 2 : 1) * pl.b_tile), b_lo = b_hi + pl.b_tile;
+        for (int t = 0; t < pl.T; ++t) {     // the last group is padded to T tiles (rows >= n_out: never gathered, never stored)
           mbar_wait(smem_u32(pl.afull + sa), pa);
           if (CPASYNC_A) fence_proxy_async_smem();   // the A stage was written by cp.async copies (generic proxy)
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(pl.a_smem + (size_t)sa * pl.a_stage_bytes), a_lo = a_hi + A_TILE_BYTES;
-          const uint32_t d_tmem = pl.tmem_base + (uint32_t)(buf * pl.acc_cols + t * p.Cout);
-          // descriptors of the k-step j: the start-address field (bits 0-13, 16-byte units) advances by 2 per 32 bytes
-          const uint64_t da_hi0 = make_desc_sw128(a_hi, 16, 1024), db_hi0 = make_desc_sw128(b_hi, 16, 1024);
-          const uint64_t da_lo0 = make_desc_sw128(a_lo, 16, 1024), db_lo0 = make_desc_sw128(b_lo, 16, 1024);
-          if (lead) {
+          const uint32_t a_hi = smem_u32(pl.a_smem + (size_t)sa * pl.a_stage_bytes) + (uint32_t)g * (64 * 128), a_lo = a_hi + A_TILE_BYTES;
+          const uint64_t da_hi = make_desc_sw128(a_hi, 16, 1024), da_lo = make_desc_sw128(a_lo, 16, 1024);
+          wg_fence();
 #pragma unroll
-            for (int j = 0; j < KBLK / 16; ++j) {
-              const uint32_t accum = (k > k0 || kb > 0 || j > 0) ? 1u : 0u;
-              mma_bf16(d_tmem, da_hi0 + 2 * j, db_hi0 + 2 * j, idesc, accum);
-              if (NSPLIT == 3) {
-                mma_bf16(d_tmem, da_lo0 + 2 * j, db_hi0 + 2 * j, idesc, 1);
-                mma_bf16(d_tmem, da_hi0 + 2 * j, db_lo0 + 2 * j, idesc, 1);
+          for (int c = 0; c < NCH; ++c) {
+            const int col = c * CH - t * p.ncols;     // chunk column inside tile t
+            if (col >= 0 && col < ncols) {
+              const uint64_t db_hi = make_desc_sw128(b_hi + (uint32_t)col * 128u, 16, 1024);
+              const uint64_t db_lo = make_desc_sw128(b_lo + (uint32_t)col * 128u, 16, 1024);
+#pragma unroll
+              for (int j = 0; j < KBLK / 16; ++j) {   // the start-address field (16-byte units) advances by 2 per 32 bytes
+                if constexpr (CH == 64) {
+                  wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(acc[c]), da_hi + 2 * j, db_hi + 2 * j);
+                  if (NSPLIT == 3) {
+                    wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(acc[c]), da_lo + 2 * j, db_hi + 2 * j);
+                    wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(acc[c]), da_hi + 2 * j, db_lo + 2 * j);
+                  }
+                } else {
+                  wgmma_n16(*reinterpret_cast<float(*)[8]>(acc[c]), da_hi + 2 * j, db_hi + 2 * j);
+                  if (NSPLIT == 3) {
+                    wgmma_n16(*reinterpret_cast<float(*)[8]>(acc[c]), da_lo + 2 * j, db_hi + 2 * j);
+                    wgmma_n16(*reinterpret_cast<float(*)[8]>(acc[c]), da_hi + 2 * j, db_lo + 2 * j);
+                  }
+                }
               }
             }
-            mma_commit(smem_u32(pl.aempty + sa));
           }
+          wg_commit();
+          wg_wait<0>();
           __syncwarp();
-          }
+          if (lane == 0) mbar_arrive(smem_u32(pl.aempty + sa));
           if (++sa == p.sa) {
             sa = 0;
             pa ^= 1;
           }
         }
-        if (lead) mma_commit(smem_u32(pl.bempty + sb));
-        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(pl.bempty + sb));
         if (++sb == p.sb) {
           sb = 0;
           pb ^= 1;
         }
       }
     }
-    if (lead) mma_commit(smem_u32(pl.tfull + buf));
-    __syncwarp();
-  }
-}
-
-// Column sums over the 32 rows held by a warp (lane = row, v[j] = column j): butterfly transpose-reduce, 31 shuffles;
-// lane j returns Σ_rows v[j].  Destroys v.
-__device__ __forceinline__ float warp_col_sums32(float (&v)[32], int lane) {
+    // ---- epilogue ----
+    float* out_part = p.out + item_ks(p, v) * p.n_out * p.out_pitch;    // this split's partial output
+    const int n0 = item_n0(p, v);
 #pragma unroll
-  for (int w = 16; w >= 1; w >>= 1) {
-    const bool up = (lane & w) != 0;
+    for (int c = 0; c < NCH; ++c) {
+      const int t = (c * CH) / p.ncols, col0 = c * CH - t * p.ncols;
+      if (t >= pl.T || col0 >= ncols) continue;
+      const int64_t rbase = (group * pl.T + t) * BLOCK_M + g * 64;
 #pragma unroll
-    for (int i = 0; i < w; ++i) {
-      const float send = up ? v[i] : v[i + w];
-      const float keep = up ? v[i + w] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, w);
-    }
-  }
-  return v[0];
-}
-
-// one warp per TMEM lane quadrant q: tcgen05.ld the accumulators (lane = output row), add bias, store fp32 rows;
-// optionally accumulate the per-channel sum and sum of squares of what was stored (the BatchNorm statistics of the
-// next layer) — per warp in fp32 over its 32 rows, then in fp64 in shared memory, one global fp64 atomic per CTA.
-__device__ __forceinline__ void role_epilogue(const ConvParams& p, const Pipe& pl, int q, int lane) {
-  int it = 0;
-  const bool want_stats = pl.stat_acc != nullptr;
-  for (int64_t v = blockIdx.x; v < pl.num_groups * p.ksplit; v += gridDim.x, ++it) {
-    const int buf = it & 1;
-    const int64_t group = v / p.ksplit;
-    float* out_part = p.out + (v % p.ksplit) * p.n_out * p.out_pitch;    // this split's partial output
-    const int64_t rem = pl.num_tiles - group * pl.T;
-    const int t_eff = pl.T;        // the last group is padded to T tiles (rows >= n_out: never gathered, never stored)
-    (void)rem;
-    mbar_wait(smem_u32(pl.tfull + buf), (it >> 1) & 1);
-    tc_fence_after();
-    for (int t = 0; t < t_eff; ++t) {
-      const int64_t row = (group * pl.T + t) * BLOCK_M + q * 32 + lane;
-      const uint32_t taddr = pl.tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * pl.acc_cols + t * p.Cout);
-      float* orow = out_part + row * p.out_pitch;
-      const bool live = row < p.n_out;
-      for (int c0 = 0; c0 < p.Cout; c0 += 32) {
-        const bool full = c0 + 32 <= p.Cout;          // else a 16-column tail (Cout % 32 == 16)
-        float v[32];
-        if (full) {
-          tmem_ld32(taddr + c0, v);
-        } else {
-          float u[16];
-          tmem_ld16(taddr + c0, u);
+      for (int i4 = 0; i4 < CH / 8; ++i4) {
+        const int col = n0 + col0 + frag_col(i4 * 4, lane);
+        float2 b = make_float2(0.f, 0.f);
+        if (p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+        float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            v[j] = u[j];
-            v[j + 16] = 0.f;
+        for (int h = 0; h < 2; ++h) {              // rows r and r + 8
+          const int64_t row = rbase + frag_row(i4 * 4 + 2 * h, wq, lane);
+          const float v0 = acc[c][i4 * 4 + 2 * h] + b.x, v1 = acc[c][i4 * 4 + 2 * h + 1] + b.y;
+          if (row < p.n_out) {
+            *reinterpret_cast<float2*>(out_part + row * p.out_pitch + col) = make_float2(v0, v1);
+            s1[0] += v0; s1[1] += v1;
+            s2[0] += v0 * v0; s2[1] += v1 * v1;
           }
-        }
-        tmem_ld_wait();
-        if (p.bias) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            if (full || j < 16) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + c0 + j));
-              v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
-            }
-          }
-        }
-        if (live) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            if (full || j < 16) *reinterpret_cast<float4*>(orow + c0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
         }
         if (want_stats) {
-          float sq[32];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            v[j] = live ? v[j] : 0.f;
-            sq[j] = v[j] * v[j];
+          for (int w = 4; w < 32; w <<= 1) {        // lanes with the same (lane & 3) hold the same columns
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], w);
+              s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], w);
+            }
           }
-          const float s1 = warp_col_sums32(v, lane);
-          const float s2 = warp_col_sums32(sq, lane);
-          if (c0 + lane < p.Cout) {
-            atomicAdd(pl.stat_acc + c0 + lane, (double)s1);
-            atomicAdd(pl.stat_acc + p.Cout + c0 + lane, (double)s2);
+          if (lane < 4) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              atomicAdd(pl.stat_acc + col + e, (double)s1[e]);
+              atomicAdd(pl.stat_acc + p.Cout + col + e, (double)s2[e]);
+            }
           }
         }
       }
     }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(pl.tempty + buf));
   }
   if (want_stats) {
-    asm volatile("bar.sync 1, 128;" ::: "memory");   // the 4 epilogue warps
-    for (int i = q * 32 + lane; i < 2 * p.Cout; i += NUM_EPI_WARPS * 32) atomicAdd(p.stats + i, pl.stat_acc[i]);
+    named_sync(1, NUM_CONS_WARPS * 32);   // the consumer warps
+    const int ct = g * 128 + wq * 32 + lane;
+    for (int i = ct; i < 2 * p.Cout; i += NUM_CONS_WARPS * 32) atomicAdd(p.stats + i, pl.stat_acc[i]);
   }
+}
+
+// the consumer role of warp `warp` (CONS_WARP0 <= warp < LOAD_WARP), dispatched on the chunk width
+template <int NSPLIT, bool CPASYNC_A>
+__device__ __forceinline__ void run_consumer(const ConvParams& p, const Pipe& pl, int warp, int lane) {
+  const int g = (warp - CONS_WARP0) >> 2, wq = (warp - CONS_WARP0) & 3;
+  if (p.Cout % 64 == 0) role_consumer<NSPLIT, CPASYNC_A, 64>(p, pl, g, wq, lane);
+  else role_consumer<NSPLIT, CPASYNC_A, 16>(p, pl, g, wq, lane);
 }
 
 template <int NSPLIT, bool PROLOGUE>
@@ -338,7 +322,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr int n_op = (NSPLIT == 3) ? 2 : 1;
-  const int b_tile = p.Cout * 128;
+  const int b_tile = p.ncols * 128;
   const int a_stage_bytes = n_op * A_TILE_BYTES;
   const int b_stage_bytes = n_op * b_tile;
   const int T = p.tiles_per_group;
@@ -350,46 +334,35 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
   uint64_t* aempty = bars + MAX_STAGES;           // [MAX_STAGES]
   uint64_t* bfull = bars + 2 * MAX_STAGES;        // [MAX_STAGES]
   uint64_t* bempty = bars + 3 * MAX_STAGES;       // [MAX_STAGES]
-  uint64_t* tfull = bars + 4 * MAX_STAGES;        // [2]
-  uint64_t* tempty = bars + 4 * MAX_STAGES + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4 * MAX_STAGES + 4);
-  double* stat_acc = p.stats ? reinterpret_cast<double*>(tmem_slot + 4) : nullptr;   // [2*Cout]
+  double* stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;   // [2*Cout]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KB = p.Cin / KBLK;
   const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
   const int64_t num_groups = (num_tiles + T - 1) / T;
-  const int acc_cols = T * p.Cout;                // TMEM columns of one accumulator set
 
   if (stat_acc)
     for (int i = threadIdx.x; i < 2 * p.Cout; i += NUM_THREADS) stat_acc[i] = 0.0;
   if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_STAGES; ++s) {
       mbar_init(smem_u32(afull + s), NUM_GATHER_WARPS);
-      mbar_init(smem_u32(aempty + s), 1);
+      mbar_init(smem_u32(aempty + s), NUM_CONS_WARPS);
       mbar_init(smem_u32(bfull + s), 1);
-      mbar_init(smem_u32(bempty + s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(tfull + b), 1);
-      mbar_init(smem_u32(tempty + b), NUM_EPI_WARPS);
+      mbar_init(smem_u32(bempty + s), NUM_CONS_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == MMA_WARP) tmem_alloc(smem_u32(tmem_slot), (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   Pipe pl;
   pl.a_smem = a_smem; pl.b_smem = b_smem;
-  pl.afull = afull; pl.aempty = aempty; pl.bfull = bfull; pl.bempty = bempty; pl.tfull = tfull; pl.tempty = tempty;
-  pl.tmem_base = tmem_base;
+  pl.afull = afull; pl.aempty = aempty; pl.bfull = bfull; pl.bempty = bempty;
   pl.stat_acc = stat_acc;
-  pl.a_stage_bytes = a_stage_bytes; pl.b_stage_bytes = b_stage_bytes; pl.b_tile = b_tile;
-  pl.KB = KB; pl.T = T; pl.acc_cols = acc_cols; pl.num_tiles = num_tiles; pl.num_groups = num_groups;
+  pl.a_stage_bytes = a_stage_bytes; pl.b_tile = b_tile;
+  pl.KB = KB; pl.T = T; pl.num_tiles = num_tiles; pl.num_groups = num_groups;
+  pl.num_items = num_groups * p.ksplit * p.nsplit;
 
   if (warp < NUM_GATHER_WARPS) {
+    reg_alloc<GATHER_REGS>();
     // ===================================== gather producers =====================================
     const int chunk = lane & 15;  // 16-byte fp32 chunk inside the 64-channel block
     const int rsub = lane >> 4;   // which of the 2 rows this half-warp handles per step
@@ -412,18 +385,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
       }
       cp_async_commit();
     };
-    const int64_t num_items = num_groups * p.ksplit;
+    const int64_t num_items = pl.num_items;
     // position `it` at the first offset of work item v
     auto enter = [&](SlotIt& it, int64_t v) {
       it.v = v;
       it.valid = v < num_items;
       if (it.valid) {
-        it.group = v / p.ksplit;
-        it.k = (int)(v % p.ksplit) * p.kchunk;
+        it.group = item_group(p, v);
+        it.k = item_ks(p, v) * p.kchunk;
         it.k1 = it.k + p.kchunk < p.K ? it.k + p.kchunk : p.K;
-        const int64_t rem = num_tiles - it.group * T;
-        it.t_eff = T;              // padded to T tiles (see role_mma)
-        (void)rem;
+        it.t_eff = T;              // padded to T tiles (see role_consumer)
       }
     };
     auto advance = [&](SlotIt& it) {
@@ -444,12 +415,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
         const int over = k - k1;
         v += gridDim.x;
         if (v >= num_items) break;
-        const int k0 = (int)(v % p.ksplit) * p.kchunk;
+        const int k0 = item_ks(p, v) * p.kchunk;
         k1 = k0 + p.kchunk < p.K ? k0 + p.kchunk : p.K;
         k = k0 + over;
       }
       if (v < num_items) {
-        const int64_t g = v / p.ksplit;
+        const int64_t g = item_group(p, v);
         prefetch_idx(g, k, gk, T);
       } else {
         cp_async_commit();  // keep the group count uniform
@@ -555,38 +526,29 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
       }
     }
     cp_async_wait<0>();
-  } else if (warp == LOAD_WARP) {
-    if (lane == 0) role_weight_loader(p, pl);
-  } else if (warp == MMA_WARP) {
-    role_mma<NSPLIT>(p, pl);
+  } else if (warp >= LOAD_WARP) {
+    reg_dealloc<LOAD_REGS>();
+    if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, n_op);
   } else {
-    role_epilogue(p, pl, warp - NUM_GATHER_WARPS, lane);   // == warp % 4: the TMEM lane quadrant this warp may read
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+    reg_alloc<CONS_REGS>();
+    run_consumer<NSPLIT, false>(p, pl, warp, lane);
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // Plane-gather variant: the input arrives PRE-SPLIT as bf16 planes (hi [+ lo]) and the producers only move bytes
 // ------------------------------------------------------------------------------------------------------------
-// ncu of k_conv_tc (round 1): 3.5 long-scoreboard stall cycles per issued instruction, L2 at 15 % — every gathered
-// fp32 value crosses the register file and is converted 27x (once per kernel offset).  Here the split x = hi + lo is
-// done ONCE per tensor by the producing pass (k_split_planes / the BatchNorm apply), and a gather warp issues
-// 16-byte cp.async (LDGSTS) copies straight from the plane rows into the 128-byte-swizzled UMMA tile:
-//   * no registers on the data path, so `pl_depth` whole A stages (32 KB each in fp32 mode) are in flight per SM;
-//   * a missing neighbour is a ZERO-FILL copy (src-size 0): no global or L2 traffic at all for the ~38 % of
-//     (row, offset) pairs that have no neighbour — the TMA gather4 variant of round 1 had to fetch a zero row for each;
+// In k_conv_tc every gathered fp32 value crosses the register file and is converted once per kernel offset.  Here the
+// split x = hi + lo is done ONCE per tensor by the producing pass (k_split_planes / the BatchNorm apply), and a gather
+// warp issues 16-byte cp.async (LDGSTS) copies straight from the plane rows into the 128-byte-swizzled operand tile:
+//   * no registers on the data path, so whole A stages (32 KB each in fp32 mode) are in flight per SM;
+//   * a missing neighbour is a ZERO-FILL copy (src-size 0): no global or L2 traffic for (row, offset) pairs that have
+//     no neighbour;
 //   * 8 copies per lane per slot instead of ~600 gather/convert/store instructions.
-// Completion is tracked by the hardware: after issuing the copies of a slot every producer thread executes
-// cp.async.mbarrier.arrive.noinc on the slot's "full" barrier (expected count = 256 producer threads), so the barrier
-// completes when the last copy has landed — no wait_group, no software publish step, and the producers run up to `sa`
-// slots ahead of the MMA (a first version published slot n-D in software after issuing slot n: ncu showed the MMA
-// thread and the producers waiting on each other's hand-off, 1.43 ms).  The MMA thread adds a generic→async proxy
-// fence after its barrier wait (CUTLASS's sm100 cp.async collective issues none; it costs one instruction per slot).
+// Completion is tracked by the hardware: after issuing the copies of a slot every lane of the filling warp executes
+// cp.async.mbarrier.arrive.noinc on the slot's "full" barrier (expected count = 32), so the barrier completes when the
+// last copy has landed — no wait_group, no software publish step, and the producers run up to `sa` slots ahead of the
+// MMA.  The consumers add a generic→async proxy fence after their barrier wait.
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
 }
@@ -595,16 +557,12 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
 
-constexpr int PL_MMA_WARPS = 4;                                      // tcgen05.mma issuers (one thread each), see role_mma
-constexpr int PL_MMA_WARP0 = LOAD_WARP + 1;                          // issuer 0 = MMA_WARP, issuers 1..3 = warps 14..16
-constexpr int NUM_THREADS_PL = (PL_MMA_WARP0 + PL_MMA_WARPS - 1) * 32;   // 544
-
 template <int NSPLIT>
-__global__ void __launch_bounds__(NUM_THREADS_PL, 1) k_conv_pl(const __grid_constant__ ConvParams p) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr int n_op = (NSPLIT == 3) ? 2 : 1;
-  const int b_tile = p.Cout * 128;
+  const int b_tile = p.ncols * 128;
   const int a_stage_bytes = n_op * A_TILE_BYTES;
   const int b_stage_bytes = n_op * b_tile;
   const int T = p.tiles_per_group;
@@ -615,53 +573,35 @@ __global__ void __launch_bounds__(NUM_THREADS_PL, 1) k_conv_pl(const __grid_cons
   uint64_t* aempty = bars + MAX_STAGES;           // [MAX_STAGES]
   uint64_t* bfull = bars + 2 * MAX_STAGES;        // [MAX_STAGES]
   uint64_t* bempty = bars + 3 * MAX_STAGES;       // [MAX_STAGES]
-  uint64_t* tfull = bars + 4 * MAX_STAGES;        // [2]
-  uint64_t* tempty = bars + 4 * MAX_STAGES + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4 * MAX_STAGES + 4);
-  double* stat_acc = p.stats ? reinterpret_cast<double*>(tmem_slot + 4) : nullptr;   // [2*Cout]
+  double* stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;   // [2*Cout]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KB = p.Cin / KBLK;
   const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
   const int64_t num_groups = (num_tiles + T - 1) / T;
-  const int acc_cols = T * p.Cout;
 
-  // active issuers.  A parity wait is only sound for a waiter that sees EVERY phase of the barrier, so a stage of the A ring
-  // must always be consumed by the same issuer: slot n holds tile n % T (groups are padded to T tiles) and sits in stage
-  // n % sa, hence n_mma must divide both T and sa.  (4 issuers on a 6-stage ring gave rare wrong tiles: an issuer came
-  // back to a stage two fills later and its parity wait passed one fill early.)
-  int n_mma = 1;
-  for (int c = 2; c <= PL_MMA_WARPS && c <= p.pl_depth; c <<= 1)
-    if (T % c == 0 && p.sa % c == 0) n_mma = c;
   if (stat_acc)
-    for (int i = threadIdx.x; i < 2 * p.Cout; i += NUM_THREADS_PL) stat_acc[i] = 0.0;
+    for (int i = threadIdx.x; i < 2 * p.Cout; i += NUM_THREADS) stat_acc[i] = 0.0;
   if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_STAGES; ++s) {
       mbar_init(smem_u32(afull + s), 32);   // one cp.async arrival per lane of the warp that fills the slot
-      mbar_init(smem_u32(aempty + s), 1);
+      mbar_init(smem_u32(aempty + s), NUM_CONS_WARPS);
       mbar_init(smem_u32(bfull + s), 1);
-      mbar_init(smem_u32(bempty + s), n_mma);   // one commit per issuer
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(tfull + b), n_mma);
-      mbar_init(smem_u32(tempty + b), NUM_EPI_WARPS);
+      mbar_init(smem_u32(bempty + s), NUM_CONS_WARPS);
     }
     fence_barrier_init();
   }
-  if (warp == MMA_WARP) tmem_alloc(smem_u32(tmem_slot), (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   Pipe pl;
   pl.a_smem = a_smem; pl.b_smem = b_smem;
-  pl.afull = afull; pl.aempty = aempty; pl.bfull = bfull; pl.bempty = bempty; pl.tfull = tfull; pl.tempty = tempty;
-  pl.tmem_base = tmem_base;
+  pl.afull = afull; pl.aempty = aempty; pl.bfull = bfull; pl.bempty = bempty;
   pl.stat_acc = stat_acc;
-  pl.a_stage_bytes = a_stage_bytes; pl.b_stage_bytes = b_stage_bytes; pl.b_tile = b_tile;
-  pl.KB = KB; pl.T = T; pl.acc_cols = acc_cols; pl.num_tiles = num_tiles; pl.num_groups = num_groups;
+  pl.a_stage_bytes = a_stage_bytes; pl.b_tile = b_tile;
+  pl.KB = KB; pl.T = T; pl.num_tiles = num_tiles; pl.num_groups = num_groups;
+  pl.num_items = num_groups * p.ksplit * p.nsplit;
 
   if (warp < NUM_GATHER_WARPS) {
+    reg_alloc<GATHER_REGS>();
     // ===================================== plane-gather producers =====================================
     // ONE WARP PER SLOT: warp w fills the slots n ≡ w (mod 8) of the CTA's slot sequence (work item → k → kb → tile),
     // all 128 rows of the tile.  (A first version let every warp fill 16 rows of EVERY slot: ncu showed ~300
@@ -670,7 +610,7 @@ __global__ void __launch_bounds__(NUM_THREADS_PL, 1) k_conv_pl(const __grid_cons
     // instructions per plane per slot.  Lane l holds the neighbour indices of rows l, l+32, l+64, l+96 (four coalesced
     // 128-byte loads, fetched two of the warp's slots = 16 CTA slots ahead), distributed by one shuffle per instruction.
     const int ch = lane & 7, sub = lane >> 3;
-    const int64_t num_items = num_groups * p.ksplit;
+    const int64_t num_items = pl.num_items;
     struct It {
       int64_t v, group;
       int k, k1, kb, t, t_eff;
@@ -681,12 +621,10 @@ __global__ void __launch_bounds__(NUM_THREADS_PL, 1) k_conv_pl(const __grid_cons
       it.valid = v < num_items;
       it.kb = 0; it.t = 0;
       if (it.valid) {
-        it.group = v / p.ksplit;
-        it.k = (int)(v % p.ksplit) * p.kchunk;
+        it.group = item_group(p, v);
+        it.k = item_ks(p, v) * p.kchunk;
         it.k1 = it.k + p.kchunk < p.K ? it.k + p.kchunk : p.K;
-        const int64_t rem = num_tiles - it.group * T;
-        it.t_eff = T;              // padded to T tiles (see role_mma)
-        (void)rem;
+        it.t_eff = T;              // padded to T tiles (see role_consumer)
       }
     };
     auto advance = [&](It& it) {
@@ -769,28 +707,13 @@ __global__ void __launch_bounds__(NUM_THREADS_PL, 1) k_conv_pl(const __grid_cons
     }
     cp_async_commit();
     cp_async_wait<0>();
-  } else if (warp == LOAD_WARP) {
-    if (lane == 0) role_weight_loader(p, pl);
-  } else if (warp == MMA_WARP) {
-    role_mma<NSPLIT, true>(p, pl, 0, n_mma);
-  } else if (warp >= PL_MMA_WARP0) {
-    const int mid = warp - PL_MMA_WARP0 + 1;
-    if (mid < n_mma) role_mma<NSPLIT, true>(p, pl, mid, n_mma);
+  } else if (warp >= LOAD_WARP) {
+    reg_dealloc<LOAD_REGS>();
+    if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, n_op);
   } else {
-    role_epilogue(p, pl, warp - NUM_GATHER_WARPS, lane);
+    reg_alloc<CONS_REGS>();
+    run_consumer<NSPLIT, true>(p, pl, warp, lane);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-  }
-}
-
-int pow2_cols(int c) {
-  int v = 32;
-  while (v < c) v <<= 1;
-  return v;
 }
 
 }  // namespace
@@ -811,6 +734,16 @@ extern "C" int pasco_conv_pack_weights(const float* W, int32_t K, int32_t Cin, i
 }
 
 namespace {
+
+// output column ranges: up to 128 columns (the register accumulators of a consumer warpgroup) per work item, and
+// the tiles per group whose accumulators fit beside each other; small inputs spread tiles over more SMs instead
+void column_plan(int Cout, int64_t tiles, int& nsplit, int& ncols, int& T) {
+  nsplit = (Cout + ACC_COLS - 1) / ACC_COLS;
+  ncols = nsplit > 1 ? ACC_COLS : Cout;
+  T = ACC_COLS / ncols;
+  if (T > 4) T = 4;
+  while (T > 1 && tiles < (int64_t)T * num_sms()) T >>= 1;
+}
 
 // split-K plan: few output tiles and many offsets (the dense bottleneck: 32 tiles x 245 offsets) leave most SMs idle with
 // one CTA per tile; cut the offsets into `ksplit` ranges so that ~2 x #SM work items exist.  1 = no split.
@@ -854,15 +787,13 @@ int conv_forward_impl(const float* in, int64_t n_in, const int32_t* nbr, int32_t
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   const int n_op = precision == 3 ? 2 : 1;
-  const int a_stage = n_op * A_TILE_BYTES, b_stage = n_op * Cout * 128;
   int64_t tiles = (n_out + BLOCK_M - 1) / BLOCK_M;
-  int T = 256 / Cout;
-  if (T < 1) T = 1;
-  if (T > 4) T = 4;
-  while (T > 1 && tiles < (int64_t)T * num_sms()) T >>= 1;   // small inputs: spread tiles over more SMs instead
+  int nsplit, ncols, T;
+  column_plan(Cout, tiles, nsplit, ncols, T);
   if (ksplit > 1) T = 1;
+  const int a_stage = n_op * A_TILE_BYTES, b_stage = n_op * ncols * 128;
   const int idx_bytes = IDX_RING * T * BLOCK_M * 4;
-  const int fixed = 1024 /*align slack*/ + idx_bytes + (4 * MAX_STAGES + 4) * 8 + 16 + (stats ? 2 * Cout * 8 : 0);
+  const int fixed = 1024 /*align slack*/ + idx_bytes + 4 * MAX_STAGES * 8 + (stats ? 2 * Cout * 8 : 0);
   int sb = 2;
   int sa = (smem_optin - fixed - sb * b_stage) / a_stage;
   if (sa > 5) {  // room to spare: deepen the weight ring first
@@ -885,8 +816,8 @@ int conv_forward_impl(const float* in, int64_t n_in, const int32_t* nbr, int32_t
   p.in_pitch = in_pitch > 0 ? in_pitch : Cin;
   PASCO_CHECK_ARG(p.out_pitch % 4 == 0 && p.in_pitch % 4 == 0, "pasco_conv_forward_tc: pitches must be multiples of 4 floats");
   p.K = K; p.Cin = Cin; p.Cout = Cout; p.in_act = in_act;
-  p.pl_hi = nullptr; p.pl_lo = nullptr; p.pl_pitch = 0; p.pl_depth = 0;
-  p.sa = sa; p.sb = sb; p.tiles_per_group = T; p.tmem_cols = pow2_cols(2 * T * Cout);
+  p.pl_hi = nullptr; p.pl_lo = nullptr; p.pl_pitch = 0;
+  p.sa = sa; p.sb = sb; p.tiles_per_group = T; p.nsplit = nsplit; p.ncols = ncols;
   p.koff_base = 0; p.koff_step = 1;
   if (koff_map) {
     bool ident = true, rev = true;
@@ -898,8 +829,8 @@ int conv_forward_impl(const float* in, int64_t n_in, const int32_t* nbr, int32_t
     if (!ident) { p.koff_base = K - 1; p.koff_step = -1; }
   }
   const size_t smem = (size_t)sa * a_stage + (size_t)sb * b_stage + fixed;
-  int64_t groups = (tiles + T - 1) / T * p.ksplit;
-  int grid = (int)(groups < num_sms() ? groups : num_sms());
+  const int64_t items = (tiles + T - 1) / T * p.ksplit * nsplit;
+  const int grid = (int)(items < num_sms() ? items : num_sms());
   cudaError_t e;
   const bool prologue = in_scale != nullptr || in_act != 0;
   auto launch = [&](auto kern) {
@@ -951,19 +882,14 @@ extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   const int n_op = precision == 3 ? 2 : 1;
-  const int a_stage = n_op * A_TILE_BYTES, b_stage = n_op * Cout * 128;
   const int64_t tiles = (n_out + BLOCK_M - 1) / BLOCK_M;
-  int T = 256 / Cout;
-  if (T < 1) T = 1;
-  if (T > 4) T = 4;
-  while (T > 1 && tiles < (int64_t)T * num_sms()) T >>= 1;
-  const int fixed = 1024 + (4 * MAX_STAGES + 4) * 8 + 16 + (stats ? 2 * Cout * 8 : 0);
+  int nsplit, ncols, T;
+  column_plan(Cout, tiles, nsplit, ncols, T);
+  const int a_stage = n_op * A_TILE_BYTES, b_stage = n_op * ncols * 128;
+  const int fixed = 1024 + 4 * MAX_STAGES * 8 + (stats ? 2 * Cout * 8 : 0);
   int sb = 2;
   int sa = (smem_optin - fixed - sb * b_stage) / a_stage;
   if (sa > MAX_STAGES) sa = MAX_STAGES;
-  // an even ring lets two MMA issuers share the tile groups (n_mma must divide T and sa, see k_conv_pl): at C = 128 in
-  // fp32 mode 4 stages + 2 issuers beat 5 stages + 1 issuer
-  if (T >= 2 && (sa & 1) && sa > 2) sa -= 1;
   static const int sa_env = [] { const char* e = getenv("PASCO_PL_SA"); return e ? atoi(e) : 0; }();
   if (sa_env >= 2 && sa_env < sa) sa = sa_env;
   PASCO_CHECK_ARG(sa >= 2, "pasco_conv_forward_planes: not enough shared memory (Cout=%d)", Cout);
@@ -975,7 +901,7 @@ extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t
   p.in_pitch = Cin;
   PASCO_CHECK_ARG(p.out_pitch % 4 == 0, "pasco_conv_forward_planes: out_pitch must be a multiple of 4 floats");
   p.K = K; p.Cin = Cin; p.Cout = Cout; p.in_act = 0;
-  p.sa = sa; p.sb = sb; p.tiles_per_group = T; p.tmem_cols = pow2_cols(2 * T * Cout);
+  p.sa = sa; p.sb = sb; p.tiles_per_group = T; p.nsplit = nsplit; p.ncols = ncols;
   p.ksplit = 1; p.kchunk = K;
   p.koff_base = 0; p.koff_step = 1;
   if (koff_map) {
@@ -988,15 +914,12 @@ extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t
     if (!ident) { p.koff_base = K - 1; p.koff_step = -1; }
   }
   p.pl_hi = (const uint16_t*)hi; p.pl_lo = (const uint16_t*)lo; p.pl_pitch = pitch;
-  static const int depth_env = [] { const char* e = getenv("PASCO_PL_DEPTH"); return e ? atoi(e) : 0; }();
-  p.pl_depth = PL_MMA_WARPS;                 // MMA issuer warps (PASCO_PL_DEPTH=1..4 overrides: debugging)
-  if (depth_env >= 1 && depth_env <= PL_MMA_WARPS) p.pl_depth = depth_env;
   const size_t smem = (size_t)sa * a_stage + (size_t)sb * b_stage + fixed;
-  const int64_t groups = (tiles + T - 1) / T;
-  const int grid = (int)(groups < num_sms() ? groups : num_sms());
+  const int64_t items = (tiles + T - 1) / T * nsplit;
+  const int grid = (int)(items < num_sms() ? items : num_sms());
   auto launch = [&](auto kern) {
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (err == cudaSuccess) kern<<<grid, NUM_THREADS_PL, smem, (cudaStream_t)s>>>(p);
+    if (err == cudaSuccess) kern<<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
     return err;
   };
   const cudaError_t e = precision == 3 ? launch(k_conv_pl<3>) : launch(k_conv_pl<1>);

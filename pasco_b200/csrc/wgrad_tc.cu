@@ -1,25 +1,27 @@
-// Weight gradient of the sparse convolution on tcgen05 (sm_100a).
+// Weight gradient of the sparse convolution on the Hopper tensor cores (wgmma), sm_90a.
 //
 //   dW[k] = Σ_o in[nbr[k,o], :]^T @ gout[o, :]
 //
-// UMMA view: D[M = 128 input channels][N = Cout] += A^T · G with the voxel rows as the contraction dimension, so
-// both operands are MN-major: the very same gathered [rows][64 ch] swizzled tiles the forward kernel builds serve as
-// A (LBO = distance between two 64-channel sub-tiles) and the gout tile as B (LBO = distance between 64-col blocks).
-// "sub-tile" s = (offset k, 64-channel block cb); a unit = two consecutive sub-tiles = one M=128 accumulator of
-// Cout TMEM columns; a CTA keeps 512/Cout units resident in TMEM, walks its share of 64-row tiles, and finally
-// adds its partial dW with fp32 reductions (red.global.add).
+// MMA view: D[M = 64 input channels][N = columns of gout] += A^T · G with the voxel rows as the contraction dimension,
+// so both operands are MN-major: the very same gathered [rows][64 ch] swizzled tiles the forward kernel builds serve
+// as A and the gout tile as B.  "sub-tile" s = (offset k, 64-channel block cb); a unit = two consecutive sub-tiles x
+// one range of UC output columns (UC = Cout up to 128); consumer warpgroup h accumulates sub-tile h of the CTA's units
+// in registers (at most 128 columns per thread set), walks its share of 64-row tiles, and finally stores its partial
+// dW into its own workspace slot; k_wgrad_sum adds the slots of a pass in CTA order (deterministic, no atomics).
 #include <stdlib.h>
 #include "common.cuh"
-#include "umma.cuh"
+#include "gmma.cuh"
 
 using namespace pasco;
-using namespace umma;
+using namespace gmma;
 
 namespace {
 
 constexpr int NUM_GATHER_WARPS = 8;                 // 8 tile rows each
-constexpr int MMA_WARP = NUM_GATHER_WARPS;           // 8 (gather warps 0-3 also run the epilogue: TMEM quadrant = warp % 4)
-constexpr int NUM_THREADS = (MMA_WARP + 1) * 32;     // 288
+constexpr int CONS_WARP0 = NUM_GATHER_WARPS;         // warps 8-15: consumer warpgroups 0 and 1 (sub-tile 0 / 1 of a unit)
+constexpr int NUM_CONS_WARPS = 8;
+constexpr int NUM_THREADS = (CONS_WARP0 + NUM_CONS_WARPS) * 32;   // 512
+constexpr int ACC_COLS = 128;                        // accumulator columns per consumer thread set (64 registers)
 constexpr int WROWS = 64 / NUM_GATHER_WARPS;         // rows of a 64-row tile per gather warp
 constexpr int WLOADS = WROWS / 2;                    // float4 loads per lane per sub-tile
 constexpr int MAX_STAGES = 8;
@@ -36,8 +38,11 @@ struct WgradParams {
   int64_t n_out;
   int64_t in_pitch, gout_pitch;   // row strides (floats)
   int K, Cin, Cout, in_act;
-  int stages, tmem_cols;
+  int stages;
   int units_per_pass, num_units, num_subs, passes, ctas_per_pass;
+  int uc, ncr;                    // columns per unit, column ranges (unit u = sub-tile pair u / ncr, columns of range u % ncr)
+  float* part;                    // [grid][slot]: partial dW of CTA b = cta_in_pass * passes + pass
+  int64_t slot;                   // units_per_pass * 128 * uc floats
 };
 
 constexpr int IDX_RING = 16;   // unit slots are short: fetch neighbour indices 15 slots ahead (HBM-latency bound otherwise)
@@ -109,6 +114,117 @@ __device__ __forceinline__ void sub_store(const SubRegs& r, uint8_t* dst_hi, uin
   }
 }
 
+// Consumer warpgroup hh (0 / 1) accumulates sub-tile hh of every unit of the CTA's pass: acc[q] holds columns
+// [64 q, 64 q + 64) of the pass's accumulator, i.e. column block q % (uc / 64) of unit q / (uc / 64).  Every consumer
+// warp arrives on the ring "empty" barriers (expected count 8).  After the CTA's last row tile it stores its partial dW
+// into its workspace slot: row (u * 128 + 64 hh + channel), column within the unit.
+template <int NSPLIT, bool CPASYNC, class P>
+__device__ __forceinline__ void wgrad_consumer(const P& p, const uint8_t* g_smem, const uint8_t* a_smem, int g_bytes, int a_bytes,
+                                               uint64_t* full_bar, uint64_t* empty_bar, uint64_t* gfull_bar, uint64_t* gempty_bar,
+                                               int unit0, int nunits, int cta_in_pass, int64_t num_rt, int hh, int wq, int lane) {
+  const int NB = p.Cout / 64, UNB = p.uc / 64, CB = p.Cin / 64;
+  float acc[2][32];
+#pragma unroll
+  for (int q = 0; q < 2; ++q)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  int git = 0;
+  for (int64_t rt = cta_in_pass; rt < num_rt; rt += p.ctas_per_pass, ++git) {
+    const int gb = git & 1;
+    mbar_wait(smem_u32(gfull_bar + gb), (git >> 1) & 1);
+    if (CPASYNC) fence_proxy_async_smem();     // tiles were written by cp.async copies (generic proxy)
+    const uint32_t g_hi = smem_u32(g_smem + (size_t)gb * g_bytes);
+    const uint32_t g_lo_off = NB * WG_SUB_BYTES;
+    for (int u = 0; u < nunits; ++u) {
+      mbar_wait(smem_u32(full_bar + stage), phase);
+      if (CPASYNC) fence_proxy_async_smem();
+      const uint32_t a_hi = smem_u32(a_smem + (size_t)stage * a_bytes) + (uint32_t)hh * WG_SUB_BYTES;
+      const uint32_t a_lo = a_hi + 2 * WG_SUB_BYTES;
+      const uint64_t da_hi = make_desc_sw128(a_hi, WG_SUB_BYTES, 1024), da_lo = make_desc_sw128(a_lo, WG_SUB_BYTES, 1024);
+      const int nb0 = ((unit0 + u) % p.ncr) * UNB;   // first 64-column block of gout that the unit covers
+      wg_fence();
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        if (q / UNB != u) continue;
+        const uint32_t b = g_hi + (uint32_t)(nb0 + q % UNB) * WG_SUB_BYTES;
+        const uint64_t db_hi = make_desc_sw128(b, WG_SUB_BYTES, 1024), db_lo = make_desc_sw128(b + g_lo_off, WG_SUB_BYTES, 1024);
+#pragma unroll
+        for (int j = 0; j < WG_R / 16; ++j) {          // 16 rows = 2048 bytes = 128 address units per k-step
+          wgmma_n64<1, 1>(acc[q], da_hi + 128 * j, db_hi + 128 * j);
+          if (NSPLIT == 3) {
+            wgmma_n64<1, 1>(acc[q], da_lo + 128 * j, db_hi + 128 * j);
+            wgmma_n64<1, 1>(acc[q], da_hi + 128 * j, db_lo + 128 * j);
+          }
+        }
+      }
+      wg_commit();
+      wg_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(empty_bar + stage));
+      if (++stage == p.stages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(gempty_bar + gb));
+  }
+  (void)CB;
+  float* slot = p.part + (int64_t)blockIdx.x * p.slot;
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    const int u = q / UNB;
+    if (u >= nunits) continue;
+    const int col0 = (q % UNB) * 64;
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int ch = frag_row(i, wq, lane), col = col0 + frag_col(i, lane);
+      *reinterpret_cast<float2*>(slot + (int64_t)(u * 128 + hh * 64 + ch) * p.uc + col) = make_float2(acc[q][i], acc[q][i + 1]);
+    }
+  }
+}
+
+// dW[k][ci][co] += Σ_c part[c * passes + pass][...] over the CTAs c of the pass that owns (k, ci, co), in CTA order
+template <class P>
+__global__ void k_wgrad_sum(const P p, float* __restrict__ dW) {
+  const int CB = p.Cin / 64;
+  const int64_t total = (int64_t)p.K * p.Cin * p.Cout;
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t kc = e / p.Cout;
+    const int col = (int)(e - kc * p.Cout);
+    const int k = (int)(kc / p.Cin), ci = (int)(kc - (int64_t)k * p.Cin);
+    const int sub = k * CB + ci / 64, hh = sub & 1;
+    const int unit = (sub >> 1) * p.ncr + col / p.uc;
+    const int pass = unit / p.units_per_pass, u = unit - pass * p.units_per_pass;
+    const float* src = p.part + (int64_t)pass * p.slot + (int64_t)(u * 128 + hh * 64 + (ci & 63)) * p.uc + col % p.uc;
+    float acc = 0.f;
+    for (int c = 0; c < p.ctas_per_pass; ++c) acc += __ldg(src + (int64_t)c * p.passes * p.slot);
+    dW[e] += acc;
+  }
+}
+
+// the per-CTA partials, summed in a fixed order into dW: stream-ordered workspace around the launch
+template <class P, class Launch>
+int wgrad_launch(P& p, float* dW, cudaStream_t st, const char* name, Launch launch) {
+  p.slot = (int64_t)p.units_per_pass * 128 * p.uc;
+  const int grid = p.passes * p.ctas_per_pass;
+  cudaError_t e = ws_alloc((void**)&p.part, (size_t)grid * p.slot * sizeof(float), st);
+  if (e != cudaSuccess) {
+    set_error("%s: workspace of %lld bytes: %s", name, (long long)grid * p.slot * 4, cudaGetErrorString(e));
+    return -1;
+  }
+  e = launch(grid);
+  if (e == cudaSuccess) k_wgrad_sum<P><<<grid_for((int64_t)p.K * p.Cin * p.Cout, 256), 256, 0, st>>>(p, dW);
+  cudaFreeAsync(p.part, st);
+  if (e != cudaSuccess) {
+    set_error("%s: cudaFuncSetAttribute failed: %s", name, cudaGetErrorString(e));
+    return -1;
+  }
+  return 0;
+}
+
 template <int NSPLIT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_constant__ WgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -124,8 +240,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
   uint64_t* empty_bar = bars + MAX_STAGES;
   uint64_t* gfull_bar = bars + 2 * MAX_STAGES;       // [2]
   uint64_t* gempty_bar = bars + 2 * MAX_STAGES + 2;  // [2]
-  uint64_t* done_bar = bars + 2 * MAX_STAGES + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 5);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int CB = p.Cin / 64;
@@ -138,18 +252,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(full_bar + s), NUM_GATHER_WARPS);
-      mbar_init(smem_u32(empty_bar + s), 1);
+      mbar_init(smem_u32(empty_bar + s), NUM_CONS_WARPS);
     }
     for (int b = 0; b < 2; ++b) {
       mbar_init(smem_u32(gfull_bar + b), NUM_GATHER_WARPS);
-      mbar_init(smem_u32(gempty_bar + b), 1);
+      mbar_init(smem_u32(gempty_bar + b), NUM_CONS_WARPS);
     }
-    mbar_init(smem_u32(done_bar), 1);
     fence_barrier_init();
   }
   // slot descriptor table: [j][0]=type (0 gout, 1 unit), [1],[2]=column bases of the two sub-tiles (-1 = none),
   // [3],[4]=kernel offset of the two sub-tiles (-1 = padding)
-  int* idx_ring = reinterpret_cast<int*>(tmem_slot + 4);            // [IDX_RING][2][WG_R]
+  int* idx_ring = reinterpret_cast<int*>(bars + 2 * MAX_STAGES + 4);   // [IDX_RING][2][WG_R]
   int* desc = idx_ring + IDX_RING * 2 * WG_R;                        // [<=16][8]
   {
     const int GSd = (NB + 1) / 2;
@@ -160,7 +273,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
       } else {
         dj[0] = 1;
         for (int h = 0; h < 2; ++h) {
-          const int sub = (unit0 + (j - GSd)) * 2 + h;
+          const int sub = ((unit0 + (j - GSd)) / p.ncr) * 2 + h;
           const bool ok = sub < p.num_subs;
           dj[1 + h] = ok ? (sub % CB) * 64 : 0;
           dj[3 + h] = ok ? sub / CB : -1;
@@ -168,11 +281,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
       }
     }
   }
-  if (warp == MMA_WARP) tmem_alloc(smem_u32(tmem_slot), (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int GS = (NB + 1) / 2;
   const int spr = GS + nunits;               // slots per row tile
 
@@ -288,93 +397,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
     }
 #undef WG_ADV
     cp_async_wait<0>();
-    // epilogue (gather warps 0-3, after their last slot): once the CTA's last MMA has retired, add the partial dW
-    if (warp < 4) {
-    const int q = warp;
-    const bool any_work = cta_in_pass < num_rt;
-    if (any_work) {
-      mbar_wait(smem_u32(done_bar), 0);
-      tc_fence_after();
-      const int L = q * 32 + lane;  // accumulator row = channel within the unit
-      for (int u = 0; u < nunits; ++u) {
-        const int sub = (unit0 + u) * 2 + (L >> 6);
-        const bool ok = sub < p.num_subs;
-        const int k = ok ? sub / CB : 0;
-        const int cb = ok ? sub - k * CB : 0;
-        float* drow = p.dW + ((int64_t)k * p.Cin + cb * 64 + (L & 63)) * p.Cout;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(u * p.Cout);
-        for (int c0 = 0; c0 < p.Cout; c0 += 32) {
-          float v[32];
-          tmem_ld32(taddr + c0, v);
-          tmem_ld_wait();
-          if (ok) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) atomicAdd(drow + c0 + j, v[j]);
-          }
-        }
-      }
-    }
-  }
-  } else if (warp == MMA_WARP) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(128, p.Cout, 1, 1);
-      int stage = 0;
-      uint32_t phase = 0;
-      int git = 0;
-      for (int64_t rt = cta_in_pass; rt < num_rt; rt += p.ctas_per_pass, ++git) {
-        const int gb = git & 1;
-        mbar_wait(smem_u32(gfull_bar + gb), (git >> 1) & 1);
-        tc_fence_after();
-        const uint32_t g_hi = smem_u32(g_smem + (size_t)gb * g_bytes);
-        const uint32_t g_lo = g_hi + NB * WG_SUB_BYTES;
-        for (int u = 0; u < nunits; ++u) {
-          mbar_wait(smem_u32(full_bar + stage), phase);
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(a_smem + (size_t)stage * a_bytes);
-          const uint32_t a_lo = a_hi + 2 * WG_SUB_BYTES;
-          const uint32_t d_tmem = tmem_base + (uint32_t)(u * p.Cout);
-#pragma unroll
-          for (int j = 0; j < WG_R / 16; ++j) {
-            const uint32_t acc = (git > 0 || j > 0) ? 1u : 0u;
-            const uint64_t da_hi = make_desc_sw128(a_hi + j * 2048, WG_SUB_BYTES, 1024);
-            const uint64_t db_hi = make_desc_sw128(g_hi + j * 2048, WG_SUB_BYTES, 1024);
-            mma_bf16(d_tmem, da_hi, db_hi, idesc, acc);
-            if (NSPLIT == 3) {
-              const uint64_t da_lo = make_desc_sw128(a_lo + j * 2048, WG_SUB_BYTES, 1024);
-              const uint64_t db_lo = make_desc_sw128(g_lo + j * 2048, WG_SUB_BYTES, 1024);
-              mma_bf16(d_tmem, da_lo, db_hi, idesc, 1);
-              mma_bf16(d_tmem, da_hi, db_lo, idesc, 1);
-            }
-          }
-          mma_commit(smem_u32(empty_bar + stage));
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        mma_commit(smem_u32(gempty_bar + gb));
-      }
-      mma_commit(smem_u32(done_bar));
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+  } else {
+    wgrad_consumer<NSPLIT, false>(p, g_smem, a_smem, g_bytes, a_bytes, full_bar, empty_bar, gfull_bar, gempty_bar, unit0, nunits,
+                                  cta_in_pass, num_rt, (warp - CONS_WARP0) >> 2, (warp - CONS_WARP0) & 3, lane);
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // Plane-gather variant of the weight gradient: both operands arrive as pre-split bf16 planes
 // ------------------------------------------------------------------------------------------------------------
-// Same UMMA view, TMEM residency, passes and epilogue as k_wgrad_tc; the producers only move bytes: 16-byte cp.async
+// Same MMA view, consumers, passes and epilogue as k_wgrad_tc; the producers only move bytes: 16-byte cp.async
 // copies from the `in` planes (gathered rows; a missing neighbour is a zero-fill copy that touches no memory) and from
 // the `gout` planes (contiguous rows) straight into the 128-byte-swizzled tiles.  Slot 0 of a row tile = the whole gout
 // tile, slots 1.. = one unit of two gathered sub-tiles each; every producer thread arrives on the slot's "full" barrier
-// with cp.async.mbarrier.arrive.noinc (count = 256 threads), so the hardware completes it when the last copy has landed
-// and the producers run a whole ring ahead of the MMA.  Round-1 k_wgrad_tc spent ~600 gather / convert / store
-// instructions per sub-tile and ran at 15 % tensor-pipe utilisation, 2.4x slower than the forward.
+// with cp.async.mbarrier.arrive.noinc (count = 32 lanes of the filling warp), so the hardware completes it when the last
+// copy has landed and the producers run a whole ring ahead of the MMA.
 struct WgradPlParams {
   const uint16_t* in_hi;
   const uint16_t* in_lo;
@@ -385,8 +422,11 @@ struct WgradPlParams {
   int64_t n_out;
   int64_t in_pitch, gout_pitch;   // row strides (bf16 elements)
   int K, Cin, Cout;
-  int stages, tmem_cols, depth;
+  int stages;
   int units_per_pass, num_units, num_subs, passes, ctas_per_pass;
+  int uc, ncr;
+  float* part;
+  int64_t slot;
 };
 
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
@@ -396,11 +436,8 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
 
-constexpr int WG_MMA_WARPS = 4;                                   // tcgen05.mma issuers of k_wgrad_pl (warps 8..11)
-constexpr int NUM_THREADS_WPL = (MMA_WARP + WG_MMA_WARPS) * 32;   // 384
-
 template <int NSPLIT>
-__global__ void __launch_bounds__(NUM_THREADS_WPL, 1) k_wgrad_pl(const __grid_constant__ WgradPlParams p) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_constant__ WgradPlParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int n_op = (NSPLIT == 3) ? 2 : 1;
@@ -414,8 +451,6 @@ __global__ void __launch_bounds__(NUM_THREADS_WPL, 1) k_wgrad_pl(const __grid_co
   uint64_t* empty_bar = bars + MAX_STAGES;
   uint64_t* gfull_bar = bars + 2 * MAX_STAGES;       // [2]
   uint64_t* gempty_bar = bars + 2 * MAX_STAGES + 2;  // [2]
-  uint64_t* done_bar = bars + 2 * MAX_STAGES + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 5);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int CB = p.Cin / 64;
@@ -425,32 +460,18 @@ __global__ void __launch_bounds__(NUM_THREADS_WPL, 1) k_wgrad_pl(const __grid_co
   const int nunits = min(p.units_per_pass, p.num_units - unit0);
   const int64_t num_rt = (p.n_out + WG_R - 1) / WG_R;
 
-  // MMA issuers: the units of a row tile accumulate into different TMEM columns, so issuer `mid` (one thread of warp
-  // 8 + mid) owns the units u ≡ mid (mod n_mma); one issuer alone needs ~100 cycles of descriptor work per tcgen05.mma
-  // that executes in 32 (N = 64) and left the tensor pipe at 33 %
-  // A parity wait is only sound for a waiter that sees every phase of the barrier, so a stage of the unit ring must
-  // always be consumed by the same issuer: unit slot `ord` holds unit ord % nunits and sits in stage ord % stages, hence
-  // n_mma must divide both nunits and stages (the host picks `stages` and the pass split accordingly).
-  int n_mma = 1;
-  for (int c = 2; c <= WG_MMA_WARPS && c <= p.depth; ++c)
-    if (nunits % c == 0 && p.stages % c == 0) n_mma = c;
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(full_bar + s), 32);    // one cp.async arrival per lane of the warp that fills the slot
-      mbar_init(smem_u32(empty_bar + s), 1);
+      mbar_init(smem_u32(empty_bar + s), NUM_CONS_WARPS);
     }
     for (int b = 0; b < 2; ++b) {
       mbar_init(smem_u32(gfull_bar + b), 32);
-      mbar_init(smem_u32(gempty_bar + b), n_mma);     // one commit per MMA issuer
+      mbar_init(smem_u32(gempty_bar + b), NUM_CONS_WARPS);
     }
-    mbar_init(smem_u32(done_bar), n_mma);
     fence_barrier_init();
   }
-  if (warp == MMA_WARP) tmem_alloc(smem_u32(tmem_slot), (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < NUM_GATHER_WARPS) {
     // ONE WARP PER SLOT, ownership split by resource:
@@ -472,8 +493,7 @@ __global__ void __launch_bounds__(NUM_THREADS_WPL, 1) k_wgrad_pl(const __grid_co
     const uint8_t* gp_hi = reinterpret_cast<const uint8_t*>(p.g_hi);
     const uint8_t* gp_lo = reinterpret_cast<const uint8_t*>(p.g_lo);
     // unit producers: Wu = the largest divisor of `stages` that is <= 7, so that warp w always fills the same stages
-    // (w, w + Wu, ...) and sees every phase of their "empty" barriers — with several MMA issuers stages are not freed in
-    // slot order, and a producer that skipped a revolution of a stage could pass its parity wait one use early
+    // (w, w + Wu, ...) and sees every phase of their "empty" barriers
     int Wu = 1;
     for (int c = 2; c <= NUM_GATHER_WARPS - 1; ++c)
       if (p.stages % c == 0) Wu = c;
@@ -509,7 +529,7 @@ __global__ void __launch_bounds__(NUM_THREADS_WPL, 1) k_wgrad_pl(const __grid_co
           const int u = (int)(ord % nunits);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int sbi = (unit0 + u) * 2 + h;
+            const int sbi = ((unit0 + u) / p.ncr) * 2 + h;
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
               const int64_t row = rt * WG_R + q * 32 + lane;
@@ -528,7 +548,7 @@ __global__ void __launch_bounds__(NUM_THREADS_WPL, 1) k_wgrad_pl(const __grid_co
         const int u = (int)(ord % nunits);
         mbar_wait(smem_u32(empty_bar + stage), phase ^ 1);
         const uint32_t a0 = smem_u32(a_smem + (size_t)stage * a_bytes) + (uint32_t)sub * 128u;
-        const int sb0 = (unit0 + u) * 2;
+        const int sb0 = ((unit0 + u) / p.ncr) * 2;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int sbi = sb0 + h;
@@ -554,97 +574,34 @@ __global__ void __launch_bounds__(NUM_THREADS_WPL, 1) k_wgrad_pl(const __grid_co
     }
     cp_async_commit();
     cp_async_wait<0>();
-    // epilogue (gather warps 0-3): once the CTA's last MMA has retired, add the partial dW
-    if (warp < 4) {
-      const int qd = warp;
-      if (cta_in_pass < num_rt) {
-        mbar_wait(smem_u32(done_bar), 0);
-        tc_fence_after();
-        const int L = qd * 32 + lane;  // accumulator row = channel within the unit
-        for (int u = 0; u < nunits; ++u) {
-          const int sbi = (unit0 + u) * 2 + (L >> 6);
-          const bool ok = sbi < p.num_subs;
-          const int k = ok ? sbi / CB : 0;
-          const int cb = ok ? sbi - k * CB : 0;
-          float* drow = p.dW + ((int64_t)k * p.Cin + cb * 64 + (L & 63)) * p.Cout;
-          const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(u * p.Cout);
-          for (int c0 = 0; c0 < p.Cout; c0 += 32) {
-            float v[32];
-            tmem_ld32(taddr + c0, v);
-            tmem_ld_wait();
-            if (ok) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) atomicAdd(drow + c0 + j, v[j]);
-            }
-          }
-        }
-      }
-    }
-  } else if (warp >= MMA_WARP && warp - MMA_WARP < n_mma) {
-    // whole warp, warp-uniform loop; the elected lane issues tcgen05.mma / tcgen05.commit (descriptors stay in uniform
-    // registers instead of ~13 ELECT / R2UR instructions per MMA)
-    const int mid = warp - MMA_WARP;
-    const bool lead = elect_one();
-    {
-      const uint32_t idesc = make_idesc_bf16(128, p.Cout, 1, 1);
-      int stage = 0;
-      uint32_t phase = 0;
-      int git = 0;
-      for (int64_t rt = cta_in_pass; rt < num_rt; rt += p.ctas_per_pass, ++git) {
-        const int gb = git & 1;
-        mbar_wait(smem_u32(gfull_bar + gb), (git >> 1) & 1);
-        fence_proxy_async_smem();                  // tiles were written by cp.async copies (generic proxy)
-        tc_fence_after();
-        const uint32_t g_hi = smem_u32(g_smem + (size_t)gb * g_bytes);
-        const uint32_t g_lo = g_hi + NB * WG_SUB_BYTES;
-        const uint64_t db_hi0 = make_desc_sw128(g_hi, WG_SUB_BYTES, 1024), db_lo0 = make_desc_sw128(g_lo, WG_SUB_BYTES, 1024);
-        for (int u = 0; u < nunits; ++u) {
-          if (u % n_mma == mid) {
-            mbar_wait(smem_u32(full_bar + stage), phase);
-            fence_proxy_async_smem();
-            tc_fence_after();
-            const uint32_t a_hi = smem_u32(a_smem + (size_t)stage * a_bytes);
-            const uint32_t a_lo = a_hi + 2 * WG_SUB_BYTES;
-            const uint32_t d_tmem = tmem_base + (uint32_t)(u * p.Cout);
-            const uint64_t da_hi0 = make_desc_sw128(a_hi, WG_SUB_BYTES, 1024), da_lo0 = make_desc_sw128(a_lo, WG_SUB_BYTES, 1024);
-            if (lead) {
-#pragma unroll
-              for (int j = 0; j < WG_R / 16; ++j) {             // 16 rows = 2048 bytes = 128 address units per k-step
-                const uint32_t acc = (git > 0 || j > 0) ? 1u : 0u;
-                mma_bf16(d_tmem, da_hi0 + 128 * j, db_hi0 + 128 * j, idesc, acc);
-                if (NSPLIT == 3) {
-                  mma_bf16(d_tmem, da_lo0 + 128 * j, db_hi0 + 128 * j, idesc, 1);
-                  mma_bf16(d_tmem, da_hi0 + 128 * j, db_lo0 + 128 * j, idesc, 1);
-                }
-              }
-              mma_commit(smem_u32(empty_bar + stage));
-            }
-            __syncwarp();
-          }
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (lead) mma_commit(smem_u32(gempty_bar + gb));
-        __syncwarp();
-      }
-      if (lead) mma_commit(smem_u32(done_bar));
-      __syncwarp();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+  } else {
+    wgrad_consumer<NSPLIT, true>(p, g_smem, a_smem, g_bytes, a_bytes, full_bar, empty_bar, gfull_bar, gempty_bar, unit0, nunits,
+                                 cta_in_pass, num_rt, (warp - CONS_WARP0) >> 2, (warp - CONS_WARP0) & 3, lane);
   }
 }
 
-int pow2_cols(int c) {
-  int v = 32;
-  while (v < c) v <<= 1;
-  return v;
+// CTAs per pass: at least one per SM, and enough that no CTA sums more than WG_MAX_RT row tiles in its fp32 register
+// accumulators before adding its partial dW (the rounding error of that sum grows with its length)
+constexpr int64_t WG_MAX_RT = 128;
+int ctas_per_pass(int64_t num_rt, int passes) {
+  int64_t cpp = num_sms() / passes;
+  const int64_t need = (num_rt + WG_MAX_RT - 1) / WG_MAX_RT;
+  if (cpp < need) cpp = need;
+  if (cpp > num_rt) cpp = num_rt;
+  return cpp < 1 ? 1 : (int)cpp;
+}
+
+// unit geometry: uc columns per unit (the consumers' 128 accumulator columns hold 128 / uc units), ncr column ranges
+template <class P>
+void unit_plan(P& p, int K, int Cin, int Cout) {
+  p.uc = Cout <= ACC_COLS ? Cout : (Cout % ACC_COLS == 0 ? ACC_COLS : 64);
+  p.ncr = Cout / p.uc;
+  p.num_subs = K * (Cin / 64);
+  p.num_units = (p.num_subs + 1) / 2 * p.ncr;
+  p.units_per_pass = ACC_COLS / p.uc;
+  if (p.units_per_pass > p.num_units) p.units_per_pass = p.num_units;
+  p.passes = (p.num_units + p.units_per_pass - 1) / p.units_per_pass;
+  p.units_per_pass = (p.num_units + p.passes - 1) / p.passes;
 }
 
 }  // namespace
@@ -664,7 +621,7 @@ extern "C" int pasco_conv_wgrad_tc(const float* in, int64_t n_in, const int32_t*
   const int n_op = precision == 3 ? 2 : 1;
   const int g_bytes = n_op * (Cout / 64) * WG_SUB_BYTES;
   const int a_bytes = n_op * 2 * WG_SUB_BYTES;
-  const int fixed = 1024 + (2 * MAX_STAGES + 6) * 8 + 32 + IDX_RING * 2 * WG_R * 4 + 16 * 8 * 4;
+  const int fixed = 1024 + (2 * MAX_STAGES + 4) * 8 + IDX_RING * 2 * WG_R * 4 + 16 * 8 * 4;
   int stages = (smem_optin - fixed - 2 * g_bytes) / a_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   PASCO_CHECK_ARG(stages >= 2, "pasco_conv_wgrad_tc: not enough shared memory");
@@ -674,32 +631,18 @@ extern "C" int pasco_conv_wgrad_tc(const float* in, int64_t n_in, const int32_t*
   p.in_pitch = in_pitch > 0 ? in_pitch : Cin;
   p.gout_pitch = gout_pitch > 0 ? gout_pitch : Cout;
   p.stages = stages;
-  p.num_subs = K * (Cin / 64);
-  p.num_units = (p.num_subs + 1) / 2;
-  p.units_per_pass = 512 / Cout;
-  if (p.units_per_pass > p.num_units) p.units_per_pass = p.num_units;
-  p.tmem_cols = pow2_cols(p.units_per_pass * Cout);
-  p.passes = (p.num_units + p.units_per_pass - 1) / p.units_per_pass;
-  p.units_per_pass = (p.num_units + p.passes - 1) / p.passes;   // balance the passes (8+6 → 7+7)
-  int64_t num_rt = (n_out + WG_R - 1) / WG_R;
-  int cpp = num_sms() / p.passes;
-  if (cpp < 1) cpp = 1;
-  if (cpp > num_rt) cpp = (int)num_rt;
-  p.ctas_per_pass = cpp;
+  unit_plan(p, K, Cin, Cout);
+  const int64_t num_rt = (n_out + WG_R - 1) / WG_R;
+  p.ctas_per_pass = ctas_per_pass(num_rt, p.passes);
   const size_t smem = (size_t)2 * g_bytes + (size_t)stages * a_bytes + fixed;
-  const int grid = p.passes * cpp;
-  cudaError_t e;
-  if (precision == 3) {
-    e = cudaFuncSetAttribute(k_wgrad_tc<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) k_wgrad_tc<3><<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
-  } else {
-    e = cudaFuncSetAttribute(k_wgrad_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) k_wgrad_tc<1><<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
-  }
-  if (e != cudaSuccess) {
-    set_error("pasco_conv_wgrad_tc: cudaFuncSetAttribute(%zu bytes) failed: %s", smem, cudaGetErrorString(e));
-    return -1;
-  }
+  cudaStream_t st = (cudaStream_t)s;
+  auto launch = [&](int grid) {
+    auto kern = precision == 3 ? k_wgrad_tc<3> : k_wgrad_tc<1>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) kern<<<grid, NUM_THREADS, smem, st>>>(p);
+    return e;
+  };
+  if (wgrad_launch(p, dW, st, "pasco_conv_wgrad_tc", launch) != 0) return -1;
   PASCO_CHECK_LAUNCH("pasco_conv_wgrad_tc");
   return 0;
 }
@@ -719,7 +662,7 @@ extern "C" int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int
   const int n_op = precision == 3 ? 2 : 1;
   const int g_bytes = n_op * (Cout / 64) * WG_SUB_BYTES;
   const int a_bytes = n_op * 2 * WG_SUB_BYTES;
-  const int fixed = 1024 + (2 * MAX_STAGES + 6) * 8 + 32;
+  const int fixed = 1024 + (2 * MAX_STAGES + 4) * 8;
   int stages = (smem_optin - fixed - 2 * g_bytes) / a_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   PASCO_CHECK_ARG(stages >= 2, "pasco_conv_wgrad_planes: not enough shared memory");
@@ -732,61 +675,30 @@ extern "C" int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int
   PASCO_CHECK_ARG(p.in_pitch % 8 == 0 && p.gout_pitch % 8 == 0 &&
                   (((uintptr_t)in_hi | (uintptr_t)in_lo | (uintptr_t)g_hi | (uintptr_t)g_lo) & 15) == 0,
                   "pasco_conv_wgrad_planes: planes must be 16-byte aligned with pitches multiple of 8 elements");
-  p.stages = stages;
-  p.depth = stages - 1 > 7 ? 7 : stages - 1;
-  static const int depth_env = [] { const char* e = getenv("PASCO_PL_DEPTH"); return e ? atoi(e) : 0; }();
-  if (depth_env > 0 && depth_env < p.depth) p.depth = depth_env;
-  p.num_subs = K * (Cin / 64);
-  p.num_units = (p.num_subs + 1) / 2;
-  const int units_cap = 512 / Cout;                             // accumulators that fit TMEM
-  p.units_per_pass = units_cap;
-  if (p.units_per_pass > p.num_units) p.units_per_pass = p.num_units;
-  p.tmem_cols = pow2_cols(p.units_per_pass * Cout);
-  p.passes = (p.num_units + p.units_per_pass - 1) / p.units_per_pass;
-  p.units_per_pass = (p.num_units + p.passes - 1) / p.passes;   // balance the passes (8+6 → 7+7) ...
-  // ... unless that makes the unit count odd: several MMA issuers need a common divisor of units and stages (kernel
-  // comment), so 14 units run as 8 + 6 rather than 7 + 7
-  if ((p.units_per_pass & 1) && p.units_per_pass + 1 <= units_cap && p.units_per_pass > 1) p.units_per_pass += 1;
+  // stages with a large divisor <= 7 (= the number of unit producer warps, see kernel)
   {
-    static const int nm_env = [] { const char* e = getenv("PASCO_WG_NM"); return e ? atoi(e) : 0; }();
-    const int nm_max = nm_env >= 1 && nm_env <= WG_MMA_WARPS ? nm_env : WG_MMA_WARPS;
-    int best = 1;
-    for (int c = 2; c <= nm_max; ++c)
-      if (p.units_per_pass % c == 0 && stages / c >= 1 && (stages / c) * c >= 2) best = c;
-    // stages: a multiple of the issuer count, and with a large divisor <= 7 (= the number of producer warps, see kernel)
-    {
-      int pick = 0, pick_w = 0;
-      for (int st = stages; st >= 2; --st) {
-        if (st % best) continue;
-        int w = 1;
-        for (int c = 2; c <= 7; ++c)
-          if (st % c == 0) w = c;
-        if (w > pick_w) { pick_w = w; pick = st; }
-      }
-      if (pick) stages = pick;
+    int pick = stages, pick_w = 0;
+    for (int st = stages; st >= 2; --st) {
+      int w = 1;
+      for (int c = 2; c <= 7; ++c)
+        if (st % c == 0) w = c;
+      if (w > pick_w) { pick_w = w; pick = st; }
     }
-    p.stages = stages;
-    p.depth = nm_max;                                           // most issuers a CTA may use
+    stages = pick;
   }
+  p.stages = stages;
+  unit_plan(p, K, Cin, Cout);
   const int64_t num_rt = (n_out + WG_R - 1) / WG_R;
-  int cpp = num_sms() / p.passes;
-  if (cpp < 1) cpp = 1;
-  if (cpp > num_rt) cpp = (int)num_rt;
-  p.ctas_per_pass = cpp;
+  p.ctas_per_pass = ctas_per_pass(num_rt, p.passes);
   const size_t smem = (size_t)2 * g_bytes + (size_t)stages * a_bytes + fixed;
-  const int grid = p.passes * cpp;
-  cudaError_t e;
-  if (precision == 3) {
-    e = cudaFuncSetAttribute(k_wgrad_pl<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) k_wgrad_pl<3><<<grid, NUM_THREADS_WPL, smem, (cudaStream_t)s>>>(p);
-  } else {
-    e = cudaFuncSetAttribute(k_wgrad_pl<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) k_wgrad_pl<1><<<grid, NUM_THREADS_WPL, smem, (cudaStream_t)s>>>(p);
-  }
-  if (e != cudaSuccess) {
-    set_error("pasco_conv_wgrad_planes: cudaFuncSetAttribute(%zu bytes) failed: %s", smem, cudaGetErrorString(e));
-    return -1;
-  }
+  cudaStream_t st = (cudaStream_t)s;
+  auto launch = [&](int grid) {
+    auto kern = precision == 3 ? k_wgrad_pl<3> : k_wgrad_pl<1>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) kern<<<grid, NUM_THREADS, smem, st>>>(p);
+    return e;
+  };
+  if (wgrad_launch(p, dW, st, "pasco_conv_wgrad_planes", launch) != 0) return -1;
   PASCO_CHECK_LAUNCH("pasco_conv_wgrad_planes");
   return 0;
 }

@@ -1,4 +1,4 @@
-// Masked cross-attention of a handful of queries (≤128) over ALL voxels of a scale, sm_100a (tcgen05 + TMEM).
+// Masked cross-attention of a handful of queries (≤128) over ALL voxels of a scale, sm_90a (wgmma).
 //
 //   O[q, h, :] = Σ_v softmax_v( Q[q,h,:]·K[v,h,:]·scale + mask[q,v] ) · V[v,h,:]
 //
@@ -7,30 +7,33 @@
 // through shared memory and keeps the query operand resident; FLOPs are negligible, the roofline is HBM:
 // 2 passes x P x H x D x 4 B (K twice, V once).
 //
-// Two passes share one kernel template (no online-softmax rescaling of the TMEM accumulator is needed):
-//   PASS 0  S = Q_h·K_hᵀ per 64-key tile (tcgen05, M=128 queries, N=64 keys, K=64 padded head dim) → per (chunk, h, q)
+// Two passes share one kernel template (no online-softmax rescaling of the accumulator is needed):
+//   PASS 0  S = Q_h·K_hᵀ per 64-key tile (wgmma, 2 x M=64 queries, N=64 keys, K=64 padded head dim) → per (chunk, h, q)
 //           running max m and Σ exp(s − m); `k_xattn_lse` merges the chunks into lse[h, q].
-//   PASS 1  S again, p = exp(s − lse) (already normalised), P → bf16 (hi+lo) K-major smem tile, O_h += P·V_h (tcgen05,
-//           V tile as MN-major B operand), accumulated in TMEM over all tiles of the CTA, then fp32 red.add into O.
-// A CTA = (head, key chunk); warps 0-3: one query row per thread (TMEM lane = row; mask, exp, row statistics),
-// warps 4-7: K/V tile gather (16 lanes per 256-byte padded row segment, fp32 → bf16 hi/lo split, 128-byte swizzle),
-// warp 8: single-thread MMA issue.  Operands are split bf16x3 like the convolution ("fp32" mode).
+//   PASS 1  S again, p = exp(s − lse) (already normalised), P → bf16 (hi+lo) K-major smem tile, O_h += P·V_h (wgmma,
+//           V tile as MN-major B operand), accumulated in registers over all tiles of the CTA; `k_xattn_osum` adds
+//           the chunks' shares in chunk order (deterministic: the attention mask of the next layer thresholds O-derived
+//           logits, so run-to-run rounding differences could flip mask bits).
+// A CTA = (head, key chunk); warps 0-3 (one warpgroup): issue the MMAs, pass each result through a [64 col][128 row]
+// fp32 scratch so that thread t then holds query row t (mask, exp, row statistics); warps 4-7: K/V tile gather (16
+// lanes per 256-byte padded row segment, fp32 → bf16 hi/lo split, 128-byte swizzle).  Operands are split bf16x3 like
+// the convolution ("fp32" mode).
 #include <math_constants.h>
 #include "common.cuh"
-#include "umma.cuh"
+#include "gmma.cuh"
 
 using namespace pasco;
-using namespace umma;
+using namespace gmma;
 
 namespace {
 
 constexpr int BK = 64;                      // keys per tile
-constexpr int QM = 128;                     // query rows (padded) = UMMA M
+constexpr int QM = 128;                     // query rows (padded) = 2 x wgmma M
 constexpr int DP = 64;                      // padded head dim = one 128-byte swizzle row of bf16
 constexpr int TILE_Q = QM * 128;            // 16 KB: [128 rows][64] bf16
 constexpr int TILE_K = BK * 128;            // 8 KB : [64 keys][64] bf16
-constexpr int NTHREADS = 9 * 32;
-constexpr int MMA_WARP = 8;
+constexpr int NTHREADS = 8 * 32;
+constexpr int SCRATCH = 64 * QM * 4;        // 32 KB: one [64 col][128 row] fp32 accumulator, row-contiguous per column
 
 struct XParams {
   const float* q;      // [Q, H*D]
@@ -38,8 +41,9 @@ struct XParams {
   const float* v;      // [P, H*D]
   const uint32_t* mask; // bit rows [Q, 2*ceil(P/64)]: bit j of word 2t + j/32 = key 64t + j masked; nullptr = none
   const float* lse;    // [H, Q]            (pass 1)
-  float* out;          // [Q, H*D] zeroed   (pass 1)
+  float* out;          // [Q, H*D]          (written by k_xattn_osum)
   float* ws;           // [chunks, H, Q, 2] (pass 0)
+  float* opart;        // [chunks, Q, H*D]  (pass 1: this chunk's share of O)
   int Q, H, D;
   int64_t P;
   int chunks;
@@ -47,17 +51,55 @@ struct XParams {
 };
 
 // smem layout (bytes from a 1024-aligned base)
-//   Q_hi | Q_lo                        2 x 16 KB
+//   Q_hi | Q_lo                                 2 x 16 KB
 //   stage s (x2): K_hi | K_lo | V_hi | V_lo     4 x 8 KB
-//   P_hi[2 k-blocks? no: 64 keys = 1 block] | P_lo   2 x 16 KB   (pass 1)
+//   P_hi | P_lo                                 2 x 16 KB   (pass 1)
+//   scratch                                     32 KB
 constexpr int OFF_Q = 0;
 constexpr int OFF_KV = 2 * TILE_Q;
 constexpr int KV_STAGE = 4 * TILE_K;
 constexpr int OFF_P = OFF_KV + 2 * KV_STAGE;
-constexpr int OFF_BAR = OFF_P + 2 * TILE_Q;
+constexpr int OFF_SCR = OFF_P + 2 * TILE_Q;
+constexpr int OFF_BAR = OFF_SCR + SCRATCH;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 
 __device__ __forceinline__ uint32_t sw_off(uint32_t row, uint32_t chunk16) { return row * 128u + ((chunk16 ^ (row & 7u)) << 4); }
+
+// D[128 rows][64] (+)= A[128 rows][16 k-steps of K-major smem, 64 K] · B[64 K][64 N], bf16x3; A K-major, B K-major (TB = 0)
+// with 16-element k-steps of 32 bytes, or MN-major (TB = 1) with 16-row k-steps of 2048 bytes
+template <int TB>
+__device__ __forceinline__ void mma_rows128(float (&d)[2][32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+  const uint32_t b_step = TB ? 128u : 2u, b_lbo = TB ? TILE_K : 16;
+#pragma unroll
+  for (int hm = 0; hm < 2; ++hm) {
+    const uint64_t ah = make_desc_sw128(a_hi + hm * 8192, 16, 1024), al = make_desc_sw128(a_lo + hm * 8192, 16, 1024);
+    const uint64_t bh = make_desc_sw128(b_hi, b_lbo, 1024), bl = make_desc_sw128(b_lo, b_lbo, 1024);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      wgmma_n64<0, TB>(d[hm], ah + 2 * j, bh + b_step * j);
+      wgmma_n64<0, TB>(d[hm], al + 2 * j, bh + b_step * j);
+      wgmma_n64<0, TB>(d[hm], ah + 2 * j, bl + b_step * j);
+    }
+  }
+}
+__device__ __forceinline__ void zero_acc(float (&d)[2][32]) {
+#pragma unroll
+  for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[hm][i] = 0.f;
+}
+// accumulator fragments of the row warpgroup (thread t = warp w, lane l) → scratch[col][row] → v[j] = D[t][j]
+__device__ __forceinline__ void acc_to_rows(const float (&d)[2][32], float* scr, float (&v)[64], int warp, int lane) {
+  named_sync(1, 128);                  // the previous readers of the scratch are done
+#pragma unroll
+  for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) scr[frag_col(i, lane) * QM + hm * 64 + frag_row(i, warp, lane)] = d[hm][i];
+  named_sync(1, 128);
+  const int row = warp * 32 + lane;
+#pragma unroll
+  for (int j = 0; j < 64; ++j) v[j] = scr[j * QM + row];
+}
 
 template <int PASS>
 __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant__ XParams p) {
@@ -66,12 +108,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* kv_full = bars;        // [2]
   uint64_t* kv_empty = bars + 2;   // [2]
-  uint64_t* s_full = bars + 4;     // [2]
-  uint64_t* s_empty = bars + 6;    // [2]
-  uint64_t* p_full = bars + 8;     // [1]
-  uint64_t* p_empty = bars + 9;    // [1]
-  uint64_t* o_full = bars + 10;    // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
+  float* scr = reinterpret_cast<float*>(smem + OFF_SCR);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int h = blockIdx.x % p.H;
@@ -86,16 +123,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
   if (threadIdx.x == 0) {
     for (int i = 0; i < 2; ++i) {
       mbar_init(smem_u32(kv_full + i), 4);
-      mbar_init(smem_u32(kv_empty + i), 1);
-      mbar_init(smem_u32(s_full + i), 1);
-      mbar_init(smem_u32(s_empty + i), 4);
+      mbar_init(smem_u32(kv_empty + i), 4);
     }
-    mbar_init(smem_u32(p_full), 4);
-    mbar_init(smem_u32(p_empty), 1);
-    mbar_init(smem_u32(o_full), 1);
     fence_barrier_init();
   }
-  if (warp == MMA_WARP) tmem_alloc(smem_u32(tmem_slot), 256);
   // ---- resident query operand: Q_h * scale → bf16 hi/lo, rows >= Q and columns >= D are zero ----
   for (int t = threadIdx.x; t < QM * 8; t += NTHREADS) {       // one 16-byte output chunk (8 bf16) per iteration
     const int row = t >> 3, c = t & 7;
@@ -113,14 +144,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
     *reinterpret_cast<uint4*>(smem + OFF_Q + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t TM_S = tmem_base;          // 2 x 64 columns
-  const uint32_t TM_O = tmem_base + 128;    // 64 columns
 
-  if (warp >= 4 && warp < 8) {
+  if (warp >= 4) {
     // ===================================== K / V tile gather =====================================
     const int gw = warp - 4;                 // 16 keys per warp
     const int chunk4 = lane & 15, rsub = lane >> 4;
@@ -160,60 +186,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
       if (lane == 0) mbar_arrive(smem_u32(kv_full + st));
       if (st == 1) phase ^= 1;
     }
-  } else if (warp == MMA_WARP) {
-    // ===================================== MMA issue =====================================
-    if (lane == 0 && my_tiles > 0) {
-      const uint32_t idesc_s = make_idesc_bf16(QM, BK, 0, 0);   // S[128 q][64 keys] = Q (K-major) · K (K-major)
-      const uint32_t idesc_o = make_idesc_bf16(QM, DP, 0, 1);   // O[128 q][64 d]   = P (K-major) · V (MN-major)
-      const uint32_t q_hi = smem_u32(smem + OFF_Q), q_lo = q_hi + TILE_Q;
-      const uint32_t p_hi = smem_u32(smem + OFF_P), p_lo = p_hi + TILE_Q;
-      auto issue_s = [&](int64_t it) {
-        const int st = (int)(it & 1);
-        mbar_wait(smem_u32(kv_full + st), (uint32_t)((it >> 1) & 1));
-        mbar_wait(smem_u32(s_empty + st), (uint32_t)(((it >> 1) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t k_hi = smem_u32(smem + OFF_KV + st * KV_STAGE), k_lo = k_hi + TILE_K;
-#pragma unroll
-        for (int j = 0; j < DP / 16; ++j) {
-          const uint64_t a_hi = make_desc_sw128(q_hi + j * 32, 16, 1024), a_lo = make_desc_sw128(q_lo + j * 32, 16, 1024);
-          const uint64_t b_hi = make_desc_sw128(k_hi + j * 32, 16, 1024), b_lo = make_desc_sw128(k_lo + j * 32, 16, 1024);
-          mma_bf16(TM_S + st * BK, a_hi, b_hi, idesc_s, j > 0 ? 1u : 0u);
-          mma_bf16(TM_S + st * BK, a_lo, b_hi, idesc_s, 1);
-          mma_bf16(TM_S + st * BK, a_hi, b_lo, idesc_s, 1);
-        }
-        mma_commit(smem_u32(s_full + st));
-        if (PASS == 0) mma_commit(smem_u32(kv_empty + st));
-      };
-      issue_s(0);
-      for (int64_t it = 0; it < my_tiles; ++it) {
-        if (it + 1 < my_tiles) issue_s(it + 1);
-        if (PASS == 1) {
-          const int st = (int)(it & 1);
-          mbar_wait(smem_u32(p_full), (uint32_t)(it & 1));
-          tc_fence_after();
-          const uint32_t v_hi = smem_u32(smem + OFF_KV + st * KV_STAGE + 2 * TILE_K), v_lo = v_hi + TILE_K;
-#pragma unroll
-          for (int j = 0; j < BK / 16; ++j) {
-            const uint64_t a_hi = make_desc_sw128(p_hi + j * 32, 16, 1024), a_lo = make_desc_sw128(p_lo + j * 32, 16, 1024);
-            // V tile: rows = keys (contraction), 128-byte rows of 64 head-dim values → MN-major B, 16 keys = 2 KB
-            const uint64_t b_hi = make_desc_sw128(v_hi + j * 2048, TILE_K, 1024), b_lo = make_desc_sw128(v_lo + j * 2048, TILE_K, 1024);
-            const uint32_t acc = (it > 0 || j > 0) ? 1u : 0u;
-            mma_bf16(TM_O, a_hi, b_hi, idesc_o, acc);
-            mma_bf16(TM_O, a_lo, b_hi, idesc_o, 1);
-            mma_bf16(TM_O, a_hi, b_lo, idesc_o, 1);
-          }
-          mma_commit(smem_u32(p_empty));
-          mma_commit(smem_u32(kv_empty + st));
-        }
-      }
-      if (PASS == 1) mma_commit(smem_u32(o_full));
-    }
   } else {
-    // ===================================== softmax rows (warps 0-3) =====================================
+    // ===================================== MMA + softmax rows (warps 0-3) =====================================
     const int qrow = warp * 32 + lane;
     const bool qok = qrow < p.Q;
+    const uint32_t q_hi = smem_u32(smem + OFF_Q), q_lo = q_hi + TILE_Q;
+    const uint32_t p_hi = smem_u32(smem + OFF_P), p_lo = p_hi + TILE_Q;
     float m_run = -CUDART_INF_F, l_run = 0.f;
     const float my_lse = (PASS == 1 && qok) ? __ldg(p.lse + (int64_t)h * p.Q + qrow) : 0.f;
+    float oacc[2][32];
+    zero_acc(oacc);
     for (int64_t it = 0; it < my_tiles; ++it) {
       const int st = (int)(it & 1);
       const int64_t key0 = (t0 + it) * BK;
@@ -237,25 +219,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
           }
         }
       }
-      mbar_wait(smem_u32(s_full + st), (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
+      mbar_wait(smem_u32(kv_full + st), (uint32_t)((it >> 1) & 1));
+      const uint32_t k_hi = smem_u32(smem + OFF_KV + st * KV_STAGE), k_lo = k_hi + TILE_K;
       float s[BK];
       {
-        float a[32], b[32];
-        const uint32_t taddr = TM_S + ((uint32_t)(warp * 32) << 16) + (uint32_t)(st * BK);
-        tmem_ld32(taddr, a);
-        tmem_ld32(taddr + 32, b);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          s[j] = a[j];
-          s[32 + j] = b[j];
-        }
+        float sacc[2][32];
+        zero_acc(sacc);
+        wg_fence();
+        mma_rows128<0>(sacc, q_hi, q_lo, k_hi, k_lo);   // S[128 q][64 keys] = Q (K-major) · K (K-major)
+        wg_commit();
+        wg_wait<0>();
+        acc_to_rows(sacc, scr, s, warp, lane);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(s_empty + st));
       if (PASS == 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(kv_empty + st));
         float mx = m_run;
 #pragma unroll
         for (int j = 0; j < BK; ++j)
@@ -269,7 +247,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
           m_run = mx;
         }
       } else {
-        mbar_wait(smem_u32(p_empty), (uint32_t)((it & 1) ^ 1));
         uint8_t* ph = smem + OFF_P;
 #pragma unroll
         for (int c = 0; c < 8; ++c) {       // 8 probabilities per 16-byte chunk
@@ -287,8 +264,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
           *reinterpret_cast<uint4*>(ph + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
         }
         fence_proxy_async_smem();
+        named_sync(1, 128);                 // the whole P tile is written
+        const uint32_t v_hi = k_hi + 2 * TILE_K, v_lo = v_hi + TILE_K;
+        wg_fence();
+        mma_rows128<1>(oacc, p_hi, p_lo, v_hi, v_lo);   // O[128 q][64 d] += P (K-major) · V (MN-major)
+        wg_commit();
+        wg_wait<0>();
         __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(p_full));
+        if (lane == 0) mbar_arrive(smem_u32(kv_empty + st));
       }
     }
     if (PASS == 0) {
@@ -297,30 +280,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
         w[0] = m_run;
         w[1] = l_run;
       }
-    } else if (my_tiles > 0) {
-      mbar_wait(smem_u32(o_full), 0);
-      tc_fence_after();
-      float a[32], b[32];
-      const uint32_t taddr = TM_O + ((uint32_t)(warp * 32) << 16);
-      tmem_ld32(taddr, a);
-      tmem_ld32(taddr + 32, b);
-      tmem_ld_wait();
+    } else {                                 // a chunk without tiles stores zeros
+      float o[DP];
+      acc_to_rows(oacc, scr, o, warp, lane);
       if (qok) {
-        float* orow = p.out + (int64_t)qrow * HD + h * p.D;
+        float* orow = p.opart + ((int64_t)chunk * p.Q + qrow) * HD + h * p.D;
 #pragma unroll
-        for (int d = 0; d < 32; ++d)
-          if (d < p.D) atomicAdd(orow + d, a[d]);
-#pragma unroll
-        for (int d = 0; d < 32; ++d)
-          if (32 + d < p.D) atomicAdd(orow + 32 + d, b[d]);
+        for (int d = 0; d < DP; ++d)
+          if (d < p.D) orow[d] = o[d];
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -337,6 +306,15 @@ __global__ void k_xattn_lse(const float* __restrict__ ws, int chunks, int HQ, fl
   lse[i] = M + logf(L);
 }
 
+// out[i] = Σ_c opart[c, i] in chunk order
+__global__ void k_xattn_osum(const float* __restrict__ opart, int chunks, int64_t n, float* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float acc = 0.f;
+    for (int c = 0; c < chunks; ++c) acc += __ldg(opart + c * n + i);
+    out[i] = acc;
+  }
+}
+
 int pick_chunks(int64_t P, int H) {
   int64_t tiles = (P + BK - 1) / BK;
   int c = (num_sms() + H - 1) / H;        // ~one CTA per SM
@@ -347,8 +325,7 @@ int pick_chunks(int64_t P, int H) {
 }  // namespace
 
 extern "C" int64_t pasco_xattn_workspace_bytes(int32_t Q, int64_t P, int32_t H, int32_t D) {
-  (void)D;
-  return (int64_t)pick_chunks(P, H) * H * Q * 2 * sizeof(float);
+  return (int64_t)pick_chunks(P, H) * Q * H * (2 + D) * sizeof(float);   // row statistics + per-chunk shares of O
 }
 
 extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* v, const uint32_t* mask, int32_t Q,
@@ -363,6 +340,7 @@ extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* 
   p.q = q; p.k = k; p.v = v; p.mask = mask; p.lse = lse; p.out = out; p.ws = workspace;
   p.Q = Q; p.H = H; p.D = D; p.P = P; p.scale = scale;
   p.chunks = pick_chunks(P, H);
+  p.opart = workspace + (int64_t)p.chunks * H * Q * 2;
   cudaStream_t st = (cudaStream_t)s;
   const int grid = p.chunks * H;
   cudaError_t e = cudaFuncSetAttribute(k_xattn_fwd<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
@@ -374,6 +352,7 @@ extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* 
   k_xattn_fwd<0><<<grid, NTHREADS, SMEM_BYTES, st>>>(p);
   k_xattn_lse<<<(H * Q + 127) / 128, 128, 0, st>>>(workspace, p.chunks, H * Q, lse);
   k_xattn_fwd<1><<<grid, NTHREADS, SMEM_BYTES, st>>>(p);
+  k_xattn_osum<<<grid_for((int64_t)Q * H * D, 256), 256, 0, st>>>(p.opart, p.chunks, (int64_t)Q * H * D, out);
   PASCO_CHECK_LAUNCH("pasco_xattn_forward");
   return 0;
 }
@@ -384,13 +363,11 @@ extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* 
 //   P = exp(S − lse) (masked → 0),  dP = dO·Vᵀ,  dS = P ∘ (dP − rowsum(dO ∘ O)),
 //   dV = Pᵀ·dO,  dK = dSᵀ·Qs,  dQ = scale · dS·K                       (Qs = scale·Q)
 //
-// Same CTA = (head, key chunk) decomposition and 64-key tiles as the forward.  Five tcgen05 GEMM groups per tile:
+// Same CTA = (head, key chunk) decomposition, warp roles and 64-key tiles as the forward.  Five wgmma GEMMs per tile:
 //   S  [128q x 64k] = Qs(K-major) · K(K-major)            dP [128q x 64k] = dO(K-major) · V(K-major)
-//   dVᵀ[ 64d x 64k] = dOᵀ(MN-major, M padded to 128 with a zero block) · P(MN-major)
-//   dKᵀ[ 64d x 64k] = Qsᵀ(MN-major, zero-padded)            · dS(MN-major)
-//   dQ [128q x 64d] += dS(K-major) · K(MN-major)              (accumulates in TMEM over the CTA's tiles)
-// dVᵀ/dKᵀ land with lane = head-dim index, so one warp store writes 32 consecutive floats of a key's row:
-// every dK/dV row is written exactly once (no atomics); dQ is added with fp32 red.add at the end.
+//   dVᵀ[ 64d x 64k] = dOᵀ(MN-major) · P(MN-major)          dKᵀ[ 64d x 64k] = Qsᵀ(MN-major) · dS(MN-major)
+//   dQ [128q x 64d] += dS(K-major) · K(MN-major)              (accumulates in registers over the CTA's tiles)
+// every dK/dV row is written exactly once (no atomics); each chunk stores its share of dQ, k_xattn_osum adds them in order.
 // ==================================================================================================================
 namespace {
 
@@ -398,6 +375,7 @@ struct XBwdParams {
   const float* q; const float* k; const float* v; const uint32_t* mask; const float* lse;
   const float* out; const float* dout;
   float* dq; float* dk; float* dv;
+  float* dqpart;       // [chunks, Q, H*D]: this chunk's share of dQ (summed in chunk order by k_xattn_osum)
   int Q, H, D;
   int64_t P;
   int chunks;
@@ -406,12 +384,24 @@ struct XBwdParams {
 
 constexpr int B_OFF_Q = 0;                          // Qs hi | lo           2 x 16 KB
 constexpr int B_OFF_DO = 2 * TILE_Q;                // dO hi | lo           2 x 16 KB
-constexpr int B_OFF_ZERO = 4 * TILE_Q;              // zero block           16 KB
-constexpr int B_OFF_KV = 5 * TILE_Q;                // 2 stages x (K hi|lo, V hi|lo) = 2 x 32 KB
+constexpr int B_OFF_KV = 4 * TILE_Q;                // 2 stages x (K hi|lo, V hi|lo) = 2 x 32 KB
 constexpr int B_OFF_P = B_OFF_KV + 2 * KV_STAGE;    // P hi | lo            2 x 16 KB
 constexpr int B_OFF_DS = B_OFF_P + 2 * TILE_Q;      // dS hi | lo           2 x 16 KB
-constexpr int B_OFF_BAR = B_OFF_DS + 2 * TILE_Q;
+constexpr int B_OFF_SCR = B_OFF_DS + 2 * TILE_Q;    // scratch              32 KB
+constexpr int B_OFF_BAR = B_OFF_SCR + SCRATCH;
 constexpr int B_SMEM_BYTES = B_OFF_BAR + 256 + 1024;
+
+// D[64 d][64 keys] = Aᵀ·B over the 128 query rows: A, B tiles of [128 q rows][128 B], both MN-major
+__device__ __forceinline__ void mma_t64(float (&d)[32], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+  const uint64_t ah = make_desc_sw128(a_hi, TILE_Q, 1024), al = make_desc_sw128(a_lo, TILE_Q, 1024);
+  const uint64_t bh = make_desc_sw128(b_hi, TILE_Q, 1024), bl = make_desc_sw128(b_lo, TILE_Q, 1024);
+#pragma unroll
+  for (int j = 0; j < QM / 16; ++j) {                  // 16 rows = 2048 bytes = 128 address units per k-step
+    wgmma_n64<1, 1>(d, ah + 128 * j, bh + 128 * j);
+    wgmma_n64<1, 1>(d, al + 128 * j, bh + 128 * j);
+    wgmma_n64<1, 1>(d, ah + 128 * j, bl + 128 * j);
+  }
+}
 
 __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant__ XBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -419,14 +409,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B_OFF_BAR);
   uint64_t* kv_full = bars;         // [2]
   uint64_t* kv_empty = bars + 2;    // [2]
-  uint64_t* sdp_full = bars + 4;    // [2]
-  uint64_t* sdp_empty = bars + 6;   // [2]
-  uint64_t* pds_full = bars + 8;
-  uint64_t* pds_empty = bars + 9;
-  uint64_t* dvk_full = bars + 10;
-  uint64_t* dvk_empty = bars + 11;
-  uint64_t* dq_full = bars + 12;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
+  float* scr = reinterpret_cast<float*>(smem + B_OFF_SCR);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int h = blockIdx.x % p.H;
@@ -441,19 +424,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
   if (threadIdx.x == 0) {
     for (int i = 0; i < 2; ++i) {
       mbar_init(smem_u32(kv_full + i), 4);
-      mbar_init(smem_u32(kv_empty + i), 1);
-      mbar_init(smem_u32(sdp_full + i), 1);
-      mbar_init(smem_u32(sdp_empty + i), 4);
+      mbar_init(smem_u32(kv_empty + i), 4);
     }
-    mbar_init(smem_u32(pds_full), 4);
-    mbar_init(smem_u32(pds_empty), 1);
-    mbar_init(smem_u32(dvk_full), 1);
-    mbar_init(smem_u32(dvk_empty), 4);
-    mbar_init(smem_u32(dq_full), 1);
     fence_barrier_init();
   }
-  if (warp == MMA_WARP) tmem_alloc(smem_u32(tmem_slot), 512);
-  // resident operands: Qs = scale*Q_h and dO_h as bf16 hi/lo [128 rows][64], zero block
+  // resident operands: Qs = scale*Q_h and dO_h as bf16 hi/lo [128 rows][64]
   for (int t = threadIdx.x; t < QM * 8; t += NTHREADS) {
     const int row = t >> 3, c = t & 7;
     float f[8], g[8];
@@ -474,17 +449,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
     split4(make_float4(g[4], g[5], g[6], g[7]), h1, l1);
     *reinterpret_cast<uint4*>(smem + B_OFF_DO + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
     *reinterpret_cast<uint4*>(smem + B_OFF_DO + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-    *reinterpret_cast<uint4*>(smem + B_OFF_ZERO + t * 16) = make_uint4(0u, 0u, 0u, 0u);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t TM_S = tmem_base, TM_DP = tmem_base + 128, TM_DVT = tmem_base + 256, TM_DKT = tmem_base + 320,
-                 TM_DQ = tmem_base + 384;
 
-  if (warp >= 4 && warp < 8) {
+  if (warp >= 4) {
     // ===================================== K / V tile gather (as forward pass 1) =====================================
     const int gw = warp - 4;
     const int chunk4 = lane & 15, rsub = lane >> 4;
@@ -520,113 +489,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
       if (lane == 0) mbar_arrive(smem_u32(kv_full + st));
       if (st == 1) phase ^= 1;
     }
-  } else if (warp == MMA_WARP) {
-    if (lane == 0 && my_tiles > 0) {
-      const uint32_t id_kk = make_idesc_bf16(QM, BK, 0, 0);   // K-major x K-major
-      const uint32_t id_mm = make_idesc_bf16(QM, BK, 1, 1);   // MN-major x MN-major
-      const uint32_t id_km = make_idesc_bf16(QM, DP, 0, 1);   // K-major x MN-major
-      const uint32_t q_hi = smem_u32(smem + B_OFF_Q), q_lo = q_hi + TILE_Q;
-      const uint32_t o_hi = smem_u32(smem + B_OFF_DO), o_lo = o_hi + TILE_Q;
-      const uint32_t zero = smem_u32(smem + B_OFF_ZERO);
-      const uint32_t p_hi = smem_u32(smem + B_OFF_P), p_lo = p_hi + TILE_Q;
-      const uint32_t s_hi = smem_u32(smem + B_OFF_DS), s_lo = s_hi + TILE_Q;
-      auto gemm_kk = [&](uint32_t d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const uint64_t ah = make_desc_sw128(a_hi + j * 32, 16, 1024), al = make_desc_sw128(a_lo + j * 32, 16, 1024);
-          const uint64_t bh = make_desc_sw128(b_hi + j * 32, 16, 1024), bl = make_desc_sw128(b_lo + j * 32, 16, 1024);
-          mma_bf16(d, ah, bh, id_kk, j > 0 ? 1u : 0u);
-          mma_bf16(d, al, bh, id_kk, 1);
-          mma_bf16(d, ah, bl, id_kk, 1);
-        }
-      };
-      // D[128 (64 real + zero block)][64 keys] = Aᵀ·B with A, B tiles of [128 q rows][128 B]: contraction over the q rows
-      auto gemm_mm = [&](uint32_t d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
-#pragma unroll
-        for (int j = 0; j < QM / 16; ++j) {
-          const uint64_t ah = make_desc_sw128(a_hi + j * 2048, zero - a_hi, 1024), al = make_desc_sw128(a_lo + j * 2048, zero - a_lo, 1024);
-          const uint64_t bh = make_desc_sw128(b_hi + j * 2048, 16, 1024), bl = make_desc_sw128(b_lo + j * 2048, 16, 1024);
-          mma_bf16(d, ah, bh, id_mm, j > 0 ? 1u : 0u);
-          mma_bf16(d, al, bh, id_mm, 1);
-          mma_bf16(d, ah, bl, id_mm, 1);
-        }
-      };
-      auto issue_a = [&](int64_t it) {
-        const int st = (int)(it & 1);
-        mbar_wait(smem_u32(kv_full + st), (uint32_t)((it >> 1) & 1));
-        mbar_wait(smem_u32(sdp_empty + st), (uint32_t)(((it >> 1) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t k_hi = smem_u32(smem + B_OFF_KV + st * KV_STAGE), k_lo = k_hi + TILE_K;
-        const uint32_t v_hi = k_hi + 2 * TILE_K, v_lo = v_hi + TILE_K;
-        gemm_kk(TM_S + st * BK, q_hi, q_lo, k_hi, k_lo);
-        gemm_kk(TM_DP + st * BK, o_hi, o_lo, v_hi, v_lo);
-        mma_commit(smem_u32(sdp_full + st));
-      };
-      issue_a(0);
-      for (int64_t it = 0; it < my_tiles; ++it) {
-        if (it + 1 < my_tiles) issue_a(it + 1);
-        const int st = (int)(it & 1);
-        mbar_wait(smem_u32(pds_full), (uint32_t)(it & 1));
-        mbar_wait(smem_u32(dvk_empty), (uint32_t)((it & 1) ^ 1));
-        tc_fence_after();
-        gemm_mm(TM_DVT, o_hi, o_lo, p_hi, p_lo);     // dVᵀ = dOᵀ · P
-        gemm_mm(TM_DKT, q_hi, q_lo, s_hi, s_lo);     // dKᵀ = Qsᵀ · dS
-        {                                            // dQ += dS · K   (K tile as MN-major B: 16 keys = 2 KB)
-          const uint32_t k_hi = smem_u32(smem + B_OFF_KV + st * KV_STAGE), k_lo = k_hi + TILE_K;
-#pragma unroll
-          for (int j = 0; j < BK / 16; ++j) {
-            const uint64_t ah = make_desc_sw128(s_hi + j * 32, 16, 1024), al = make_desc_sw128(s_lo + j * 32, 16, 1024);
-            const uint64_t bh = make_desc_sw128(k_hi + j * 2048, TILE_K, 1024), bl = make_desc_sw128(k_lo + j * 2048, TILE_K, 1024);
-            mma_bf16(TM_DQ, ah, bh, id_km, (it > 0 || j > 0) ? 1u : 0u);
-            mma_bf16(TM_DQ, al, bh, id_km, 1);
-            mma_bf16(TM_DQ, ah, bl, id_km, 1);
-          }
-        }
-        mma_commit(smem_u32(dvk_full));
-        mma_commit(smem_u32(pds_empty));
-        mma_commit(smem_u32(kv_empty + st));
-      }
-      mma_commit(smem_u32(dq_full));
-    }
   } else {
-    // ===================================== query rows: P / dS, then the dK/dV epilogue of the previous tile ==========
+    // ===================================== MMA + query rows (warps 0-3) =====================================
     const int qrow = warp * 32 + lane;
     const bool qok = qrow < p.Q;
+    const uint32_t q_hi = smem_u32(smem + B_OFF_Q), q_lo = q_hi + TILE_Q;
+    const uint32_t o_hi = smem_u32(smem + B_OFF_DO), o_lo = o_hi + TILE_Q;
+    const uint32_t p_hi = smem_u32(smem + B_OFF_P), p_lo = p_hi + TILE_Q;
+    const uint32_t s_hi = smem_u32(smem + B_OFF_DS), s_lo = s_hi + TILE_Q;
     float my_lse = 0.f, my_delta = 0.f;
     if (qok) {
       my_lse = __ldg(p.lse + (int64_t)h * p.Q + qrow);
       for (int d = 0; d < p.D; ++d)
         my_delta += __ldg(p.dout + (int64_t)qrow * HD + h * p.D + d) * __ldg(p.out + (int64_t)qrow * HD + h * p.D + d);
     }
-    // write-out of dVᵀ/dKᵀ of tile e: lane = head-dim index (warps 0,1 hold d = 0..63), column = key
-    auto epilogue = [&](int64_t e) {
-      mbar_wait(smem_u32(dvk_full), (uint32_t)(e & 1));
-      tc_fence_after();
-      const int d = warp * 32 + lane;
-      if (warp < 2) {
-        const int64_t key0 = (t0 + e) * BK;
-#pragma unroll
-        for (int which = 0; which < 2; ++which) {
-          float* dst = which == 0 ? p.dv : p.dk;
-          const uint32_t taddr = (which == 0 ? TM_DVT : TM_DKT) + ((uint32_t)(warp * 32) << 16);
-          float a[32], b[32];
-          tmem_ld32(taddr, a);
-          tmem_ld32(taddr + 32, b);
-          tmem_ld_wait();
-          if (d < p.D) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (key0 + j < p.P) dst[(key0 + j) * HD + h * p.D + d] = a[j];
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (key0 + 32 + j < p.P) dst[(key0 + 32 + j) * HD + h * p.D + d] = b[j];
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(dvk_empty));
-    };
+    float dq[2][32];
+    zero_acc(dq);
     for (int64_t it = 0; it < my_tiles; ++it) {
       const int st = (int)(it & 1);
       const int64_t key0 = (t0 + it) * BK;
@@ -649,34 +527,29 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
           }
         }
       }
-      mbar_wait(smem_u32(sdp_full + st), (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
+      mbar_wait(smem_u32(kv_full + st), (uint32_t)((it >> 1) & 1));
+      const uint32_t k_hi = smem_u32(smem + B_OFF_KV + st * KV_STAGE), k_lo = k_hi + TILE_K;
+      const uint32_t v_hi = k_hi + 2 * TILE_K, v_lo = v_hi + TILE_K;
       float pr[BK], ds[BK];
       {
-        float a[32], b[32];
-        const uint32_t ts = TM_S + ((uint32_t)(warp * 32) << 16) + (uint32_t)(st * BK);
-        tmem_ld32(ts, a);
-        tmem_ld32(ts + 32, b);
-        tmem_ld_wait();
+        float acc[2][32], a[BK];
+        zero_acc(acc);
+        wg_fence();
+        mma_rows128<0>(acc, q_hi, q_lo, k_hi, k_lo);    // S
+        wg_commit();
+        wg_wait<0>();
+        acc_to_rows(acc, scr, a, warp, lane);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          pr[j] = ((mbits[0] >> j) & 1u) ? 0.f : __expf(a[j] - my_lse);
-          pr[32 + j] = ((mbits[1] >> j) & 1u) ? 0.f : __expf(b[j] - my_lse);
-        }
-        const uint32_t td = TM_DP + ((uint32_t)(warp * 32) << 16) + (uint32_t)(st * BK);
-        tmem_ld32(td, a);
-        tmem_ld32(td + 32, b);
-        tmem_ld_wait();
+        for (int j = 0; j < BK; ++j) pr[j] = ((mbits[j >> 5] >> (j & 31)) & 1u) ? 0.f : __expf(a[j] - my_lse);
+        zero_acc(acc);
+        wg_fence();
+        mma_rows128<0>(acc, o_hi, o_lo, v_hi, v_lo);    // dP
+        wg_commit();
+        wg_wait<0>();
+        acc_to_rows(acc, scr, a, warp, lane);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          ds[j] = pr[j] * (a[j] - my_delta);
-          ds[32 + j] = pr[32 + j] * (b[j] - my_delta);
-        }
+        for (int j = 0; j < BK; ++j) ds[j] = pr[j] * (a[j] - my_delta);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(sdp_empty + st));
-      mbar_wait(smem_u32(pds_empty), (uint32_t)((it & 1) ^ 1));
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
         uint2 h0, l0, h1, l1;
@@ -691,35 +564,40 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
         *reinterpret_cast<uint4*>(smem + B_OFF_DS + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
       }
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(pds_full));
-      if (it > 0) epilogue(it - 1);
-    }
-    if (my_tiles > 0) {
-      epilogue(my_tiles - 1);
-      mbar_wait(smem_u32(dq_full), 0);
-      tc_fence_after();
-      float a[32], b[32];
-      const uint32_t taddr = TM_DQ + ((uint32_t)(warp * 32) << 16);
-      tmem_ld32(taddr, a);
-      tmem_ld32(taddr + 32, b);
-      tmem_ld_wait();
-      if (qok) {
-        float* row = p.dq + (int64_t)qrow * HD + h * p.D;
+      named_sync(1, 128);                               // the whole P / dS tiles are written
+      {
+        float dvt[32], dkt[32];
 #pragma unroll
-        for (int d = 0; d < 32; ++d)
-          if (d < p.D) atomicAdd(row + d, a[d] * p.scale);
+        for (int i = 0; i < 32; ++i) dvt[i] = dkt[i] = 0.f;
+        wg_fence();
+        mma_t64(dvt, o_hi, o_lo, p_hi, p_lo);           // dVᵀ = dOᵀ · P
+        mma_t64(dkt, q_hi, q_lo, s_hi, s_lo);           // dKᵀ = Qsᵀ · dS
+        mma_rows128<1>(dq, s_hi, s_lo, k_hi, k_lo);     // dQ += dS · K   (K tile as MN-major B: 16 keys = 2 KB)
+        wg_commit();
+        wg_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(kv_empty + st));
 #pragma unroll
-        for (int d = 0; d < 32; ++d)
-          if (32 + d < p.D) atomicAdd(row + 32 + d, b[d] * p.scale);
+        for (int i = 0; i < 32; ++i) {                  // row = head-dim index, column = key of the tile
+          const int d = frag_row(i, warp, lane);
+          const int64_t key = key0 + frag_col(i, lane);
+          if (d < p.D && key < p.P) {
+            p.dv[key * HD + h * p.D + d] = dvt[i];
+            p.dk[key * HD + h * p.D + d] = dkt[i];
+          }
+        }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    {                                        // a chunk without tiles stores zeros
+      float a[DP];
+      acc_to_rows(dq, scr, a, warp, lane);
+      if (qok) {
+        float* row = p.dqpart + ((int64_t)chunk * p.Q + qrow) * HD + h * p.D;
+#pragma unroll
+        for (int d = 0; d < DP; ++d)
+          if (d < p.D) row[d] = a[d] * p.scale;
+      }
+    }
   }
 }
 
@@ -742,7 +620,16 @@ extern "C" int pasco_xattn_backward(const float* q, const float* k, const float*
     set_error("pasco_xattn_backward: cudaFuncSetAttribute(%d) failed: %s", B_SMEM_BYTES, cudaGetErrorString(e));
     return -1;
   }
-  k_xattn_bwd<<<p.chunks * H, NTHREADS, B_SMEM_BYTES, (cudaStream_t)s>>>(p);
+  cudaStream_t st = (cudaStream_t)s;
+  const int64_t n = (int64_t)Q * H * D;
+  e = ws_alloc((void**)&p.dqpart, (size_t)p.chunks * n * sizeof(float), st);
+  if (e != cudaSuccess) {
+    set_error("pasco_xattn_backward: workspace of %lld bytes: %s", (long long)p.chunks * n * 4, cudaGetErrorString(e));
+    return -1;
+  }
+  k_xattn_bwd<<<p.chunks * H, NTHREADS, B_SMEM_BYTES, st>>>(p);
+  k_xattn_osum<<<grid_for(n, 256), 256, 0, st>>>(p.dqpart, p.chunks, n, dq);
+  cudaFreeAsync(p.dqpart, st);
   PASCO_CHECK_LAUNCH("pasco_xattn_backward");
   return 0;
 }

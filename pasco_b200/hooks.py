@@ -1,4 +1,4 @@
-"""Opt-in hooks that route the UNMODIFIED reference's mask-transformer hot spots onto the sm_100a attention kernels.
+"""Opt-in hooks that route the UNMODIFIED reference's mask-transformer hot spots onto the sm_90a attention kernels.
 
 The MinkowskiEngine surface (`pasco_b200.me`) already carries every sparse-tensor op of the reference.  Two pieces of
 PaSCo's transformer are plain torch in the reference and therefore outside that surface:
@@ -9,7 +9,7 @@ PaSCo's transformer are plain torch in the reference and therefore outside that 
     [1, 100, X/s, Y/s, Z/s] volume (839 MB at scale 1) built only to be sampled at the key voxels.
 
 `install()` replaces those two methods — at run time, on the imported classes, without touching the reference's files —
-with calls into the engine: the K/V projections on the tcgen05 GEMM (ops.linear), the masked softmax·V as
+with calls into the engine: the K/V projections on the wgmma GEMM (ops.linear), the masked softmax·V as
 `pasco_xattn_forward/backward` (ops.MaskedCrossAttention: streaming two-pass softmax, bit-packed mask rows, no [Q, P]
 score volume in HBM) and the mask as a sparse max-pool + hash look-up.  Same parameters, same state_dict, same results
 within the fp32 tolerance (tests/test_dropin_reference.py runs the reference with and without the hooks).
@@ -43,7 +43,7 @@ def _cross_attention_forward(self, q_embed, bb_feat, attn_mask=None, padding_mas
         qb = q_embed[b] if query_pos is None else q_embed[b] + query_pos[b]
         kv = bb_feat[b] if pos is None else bb_feat[b] + pos[b]
         Q = F.linear(qb, wq, bq)
-        K = ops.linear(kv.contiguous(), wk, bk)                    # tcgen05 GEMM over all voxels
+        K = ops.linear(kv.contiguous(), wk, bk)                    # wgmma GEMM over all voxels
         V = ops.linear(kv.contiguous(), wv, bv)
         m = attn_mask[b * h] if attn_mask is not None else None    # all heads of an item share one mask
         outs.append(mha.out_proj(ops.MaskedCrossAttention.apply(Q, K, V, m, h)))

@@ -1,4 +1,4 @@
-"""`MinkowskiEngine`-compatible operator surface of the sm_100a engine — the drop-in boundary
+"""`MinkowskiEngine`-compatible operator surface of the sm_90a engine — the drop-in boundary
 (SURVEY.md §8b).  `compat/MinkowskiEngine` re-exports this module so that PaSCo's
 `import MinkowskiEngine as ME` resolves here.
 
@@ -467,7 +467,7 @@ class _Convolution(MinkowskiModuleBase):
             raise RuntimeError(f"Channel size mismatch {x.shape[1]} != {self.in_channels}")
         cm, in_key = x.coordinate_manager, x.coordinate_map_key
         if self.use_mm:
-            # ME does F.mm here; tall inputs with 64-multiple channels take the tcgen05 GEMM (ops.LinearTC), the rest
+            # ME does F.mm here; tall inputs with 64-multiple channels take the wgmma GEMM (ops.LinearTC), the rest
             # stays the fp32 library GEMM
             out = ops.linear(x.F, self.kernel.t(), self.bias.view(-1) if self.bias is not None else None)
             return SparseTensor(out, coordinate_map_key=in_key, coordinate_manager=cm)

@@ -331,7 +331,7 @@ class KernelMap:
 
 
 class PackedWeights:
-    """UMMA shared-memory images of one weight tensor (forward and transposed), owned by the module
+    """Tensor-core shared-memory images of one weight tensor (forward and transposed), owned by the module
     that owns the parameter and re-packed whenever the parameter changes (optimizer step, load_state_dict,
     device move).  Keyed by (data_ptr, version, shape) of that one parameter only."""
 
@@ -786,8 +786,8 @@ def pack_mask_bits(mask: torch.Tensor) -> torch.Tensor:
 
 class MaskedCrossAttention(torch.autograd.Function):
     """out[q] = concat_h softmax_v(scale·q_h·k_h[v] | mask[q,v]) · v_h[v]  — blocks.py:73-92 with the mask of
-    transformer_predictor_v2.py:220-289.  Forward: two streaming tcgen05 passes; backward: one streaming pass with
-    five tcgen05 GEMM groups per 64-key tile that recomputes the probabilities from the saved log-sum-exp (xattn.cu)."""
+    transformer_predictor_v2.py:220-289.  Forward: two streaming wgmma passes; backward: one streaming pass with
+    five wgmma GEMMs per 64-key tile that recomputes the probabilities from the saved log-sum-exp (xattn.cu)."""
 
     @staticmethod
     def forward(ctx, q, k, v, mask, heads: int):
@@ -849,7 +849,7 @@ def _gemm_rows(x: torch.Tensor, w_nk: torch.Tensor, bias: Optional[torch.Tensor]
 
 
 class LinearTC(torch.autograd.Function):
-    """y = x @ Wᵀ + b for tall x [N, Cin] on the tcgen05 conv kernel (bf16x3 / bf16 like the convolutions) instead of
+    """y = x @ Wᵀ + b for tall x [N, Cin] on the wgmma conv kernel (bf16x3 / bf16 like the convolutions) instead of
     an fp32 CUDA-core library GEMM.  W is [Cout, Cin] (torch Linear layout)."""
 
     @staticmethod

@@ -41,12 +41,12 @@ def test_abi_version_and_error_string(lib):
     assert lib.pasco_conv_packed_bytes(27, 64, 64) == 27 * 64 * 64 * 4
 
 
-def test_library_is_sm100a_with_tcgen05_and_bulk_copy():
+def test_library_is_sm90a_with_wgmma_and_bulk_copy(lib):
     from pasco_b200 import _lib
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass or "SM100a" in sass or "sm_100" in sass
-    assert "UTCHMMA" in sass or "UTCMMA" in sass, "no tcgen05.mma in the SASS"
-    assert "LDTM" in sass, "no tcgen05.ld in the SASS"
+    assert "arch = sm_90a" in sass
+    assert "HGMMA" in sass, "no wgmma in the SASS"
+    assert "SYNCS" in sass, "no mbarrier in the SASS"
     assert "UBLKCP" in sass, "no bulk async copy in the SASS"
 
 

@@ -122,7 +122,7 @@ def test_degenerate_inputs():
 
 @pytest.mark.gpu
 def test_criterion_on_the_device_matches_reference(gold):
-    """Same fixture on cuda:0 (first run: profiles/r02_criterion_gpu.log)."""
+    """Same fixture on cuda:0."""
     dev = torch.device("cuda:0")
     out, batch, freqs, crit, leaves = _inputs(gold, grad=True)
 

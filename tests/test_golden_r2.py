@@ -1,4 +1,4 @@
-"""Round-2 parity pins (VERDICT r1 "What's weak" 1-2): the engine-native PascoNet on the B200 against golden summaries
+"""Round-2 parity pins (VERDICT r1 "What's weak" 1-2): the engine-native PascoNet on the GPU against golden summaries
 the UNMODIFIED reference produced on the CPU oracle (tests/golden/make_golden_r2.py, committed r2_*.npz / r2_*.json):
 
   * benchmark scale (256x256x32 @10 %): no-cap forward and the cap branch with a deterministic keep-set — coordinate
@@ -179,16 +179,13 @@ def test_full_network_gradients_match_reference():
         # tolerance: the measured conditioning of this gradient in the reference itself.  A 1e-6 relative perturbation of
         # the inputs (outputs move by 3e-6) moves it by `sens` through flipped ReLU / argmax masks, ~sqrt(perturbation);
         # the engine's outputs differ from the oracle's by ~2e-5 → allow 8 x sens (+ 2e-3 floor);
-        # measured: 2.3x - 4.7x sens in the deep layers (profiles/r02_gradient_parity.json); the fp32 atomics of the weight
-        # gradient make the flip pattern vary a little from run to run, hence the margin
+        # the flip pattern depends on the summation order of the fp32 gradients, hence the margin
         tol = 2e-3 + 8.0 * sens
         rep[n] = {"rel_l2": round(rel_l2, 6), "rel_norm": round(rel_norm, 6), "cos": round(cos, 7), "ref_sens_1e-6": round(sens, 6),
                   "tol": round(tol, 5)}
         if rel_l2 > tol or rel_norm > 3e-3 or cos < 0.999:
             bad.append(n)
     print("gradient parity:", json.dumps(rep, indent=0))
-    os.makedirs(os.path.join(os.path.dirname(HERE), "gpurun_out"), exist_ok=True)
-    json.dump(rep, open(os.path.join(os.path.dirname(HERE), "gpurun_out", "r2_gradient_parity.json"), "w"), indent=1)
     assert not bad, {n: rep[n] for n in bad}
 
 

@@ -277,7 +277,7 @@ def test_conv_plane_and_register_gather_are_bit_identical(prec, cin, cout):
         ops.set_precision("fp32")
     assert torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][2], res[1][2])
     assert res[0][1] is not None and relerr(res[0][1], res[1][1]) <= 1e-12
-    assert relerr(res[0][3], res[1][3]) <= 1e-5          # dW: fp32 atomics, order differs
+    assert relerr(res[0][3], res[1][3]) <= 1e-5          # dW: the two kernels sum in different orders
     assert res[0][0].abs().sum() > 0
 
 
@@ -349,7 +349,7 @@ def test_conv_split_k_matches_unsplit(kernel, cin, cout, bias):
         ok = src >= 0
         ref_f[ok] += Fd[src[ok]] @ Wd[k]
         ref_g[ok] += Gd[src[ok]] @ Wd[koff[k]].t()
-    # 245 x 64 products accumulate in fp32 inside TMEM: 1e-4 of the output range (the parity bound is 1e-3)
+    # 245 x 64 products accumulate in fp32 register accumulators: 1e-4 of the output range (the parity bound is 1e-3)
     for o_f, o_g in outs:
         assert relerr(o_f, ref_f) <= 1e-4 and relerr(o_g, ref_g) <= 1e-4
     assert relerr(outs[0][0], outs[1][0]) <= 2e-4 and relerr(outs[0][1], outs[1][1]) <= 2e-4
@@ -359,7 +359,7 @@ def test_conv_split_k_matches_unsplit(kernel, cin, cout, bias):
 
 def test_conv_many_tiles_per_cta(ME):
     """~59k voxels: every persistent CTA walks several 128-row tiles (and several 64-row wgrad tiles
-    accumulating in TMEM), unlike the small cases above."""
+    accumulating in registers), unlike the small cases above."""
     from pasco_b200 import ops
     ops.set_precision("fp32")
     e = _run_conv_case(ME, "k3", 64, 64, TOL_TIGHT, shape=(64, 64, 32), p=0.225)
@@ -401,7 +401,7 @@ def test_conv_benchmark_scale_rows_match_fp64():
         src = nbr[k].long()
         ok = src >= 0
         ref_w = Fd[src[ok]].t() @ Gd[ok]
-        assert relerr(dW[k], ref_w) <= 1e-4, k        # ~650 k rows accumulate per entry in fp32 (TMEM + fp32 atomics)
+        assert relerr(dW[k], ref_w) <= 1e-4, k        # ~650 k rows accumulate per entry in fp32 (registers + the CTA partials summed in order)
 
 
 def test_conv_tile_tail_and_single_voxel(ME):

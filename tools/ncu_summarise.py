@@ -1,6 +1,6 @@
-"""Summarise Nsight Compute reports (.ncu-rep, `--set full`) into the JSON committed under profiles/.
+"""Summarise Nsight Compute reports (.ncu-rep, `--set full`) into one JSON summary.
 
-    python tools/ncu_summarise.py gpurun_out/a.ncu-rep [b.ncu-rep ...] --out profiles/r02_ncu_xyz.json [--note "..."]
+    python tools/ncu_summarise.py a.ncu-rep [b.ncu-rep ...] --out summary.json [--note "..."]
 
 Per kernel NAME (launches of the same kernel are averaged, min/max duration kept): duration, DRAM bytes read + written and
 the achieved DRAM GB/s against the measured copy bandwidth of MEASURED_PEAKS.json, L2 / L1 throughput %, tensor-pipe %,
