@@ -11,7 +11,7 @@
 //               the fused BatchNorm affine + activation of the producing layer, split fp32 → bf16 hi (+ lo), and
 //               store the 128x64 tile into shared memory in the 128-byte-swizzled K-major layout.  Loads of
 //               slot s+1 are in flight in registers while slot s is converted and stored.
-//   warps 8-15  two consumer warpgroups: warpgroup g issues wgmma (M=64 rows [64 g, 64 g + 64), N=64 or 16, K=16)
+//   warps 8-15  two consumer warpgroups: warpgroup g issues wgmma (M=64 rows [64 g, 64 g + 64), N=128, 64 or 16, K=16)
 //               into register accumulators, then adds the bias and stores its fp32 rows.
 //   warp  16    streams the pre-swizzled weight slices with bulk async copies into their own ring (warps 17-19 only
 //               complete its warpgroup, whose registers go to the gather and consumer warpgroups).
@@ -37,10 +37,14 @@ constexpr int CONS_WARP0 = NUM_GATHER_WARPS;                    // warpgroup-ali
 constexpr int LOAD_WARP = CONS_WARP0 + NUM_CONS_WARPS;          // first warp of the last warpgroup; its 3 others idle
 constexpr int NUM_THREADS = (LOAD_WARP + 4) * 32;              // 640 = 5 warpgroups (96 registers each at launch)
 // setmaxnreg budgets (640 x 96 at launch): the loader warpgroup keeps 24 and the registers it releases go to the gather
-// and consumer warpgroups, 2 x 128 x (GATHER_REGS - 96) + 2 x 128 x (CONS_REGS - 96) <= 128 x (96 - 24).  With these
-// budgets ptxas reports no spills in any variant (at 96 the register-gather producers spilled).
-constexpr int GATHER_REGS = 112, CONS_REGS = 112, LOAD_REGS = 24;
-static_assert(2 * 128 * (GATHER_REGS - 96) + 2 * 128 * (CONS_REGS - 96) <= 128 * (96 - LOAD_REGS), "setmaxnreg budget");
+// and consumer warpgroups, 2 x 128 x (gather - 96) + 2 x 128 x (consumer - 96) <= 128 x (96 - 24).  The register-gather
+// producers (k_conv_tc) hold two slots of loads and spill at 112, so they get 120 and the consumers 104; the plane-gather
+// producers (k_conv_pl) only issue copies, so there the consumers get 120.  With these budgets ptxas reports no spills.
+constexpr int LOAD_REGS = 24;
+constexpr int TC_GATHER_REGS = 120, TC_CONS_REGS = 104;
+constexpr int PL_GATHER_REGS = 104, PL_CONS_REGS = 120;
+static_assert(2 * 128 * (TC_GATHER_REGS - 96) + 2 * 128 * (TC_CONS_REGS - 96) <= 128 * (96 - LOAD_REGS), "setmaxnreg budget");
+static_assert(2 * 128 * (PL_GATHER_REGS - 96) + 2 * 128 * (PL_CONS_REGS - 96) <= 128 * (96 - LOAD_REGS), "setmaxnreg budget");
 constexpr int ROWS_PER_WARP = BLOCK_M / NUM_GATHER_WARPS;       // 16
 constexpr int LOADS_PER_SLOT = ROWS_PER_WARP / 2;               // float4 per lane per slot
 constexpr int TILES_PER_IDX_STEP = 32 / ROWS_PER_WARP;          // tiles whose indices one warp-wide cp.async covers
@@ -190,6 +194,10 @@ __device__ __forceinline__ void role_weight_loader(const ConvParams& p, const Pi
 // rows itself.  acc[c] holds accumulator columns [c CH, c CH + CH); the group's T tiles sit side by side, tile t in
 // columns [t ncols, (t + 1) ncols).  Every consumer warp arrives on the ring "empty" barriers (expected count 8), so a
 // stage is refilled only after both warpgroups' MMAs on it have completed.
+// Retire: one wgmma group stays in flight.  After committing slot n the warpgroup waits for all but the newest group
+// (wait_group 1), i.e. for slot n - 1, and only then releases slot n - 1's A stage (and its B stage after the B stage's
+// last tile), so the MMAs of consecutive slots overlap.  The ring needs sa >= 3 for a slot to be filled ahead of the
+// one being multiplied and the one held back.  The item's last slot is drained (wait_group 0) before the epilogue.
 // The epilogue adds the bias, stores fp32 rows and optionally accumulates the per-channel sum and sum of squares of
 // what was stored (the BatchNorm statistics of the next layer): per warp over its rows with shuffles, then in fp64 in
 // shared memory, one global fp64 atomic per channel and CTA.
@@ -200,6 +208,15 @@ __device__ __forceinline__ void role_consumer(const ConvParams& p, const Pipe& p
   const bool want_stats = pl.stat_acc != nullptr;
   int sa = 0, sb = 0;
   uint32_t pa = 0, pb = 0;
+  int held_a = -1, held_b = -1;     // stages of the slot whose MMAs may still be in flight (-1: none)
+  auto release_held = [&]() {
+    __syncwarp();
+    if (lane == 0) {
+      if (held_a >= 0) mbar_arrive(smem_u32(pl.aempty + held_a));
+      if (held_b >= 0) mbar_arrive(smem_u32(pl.bempty + held_b));
+    }
+    held_a = held_b = -1;
+  };
   for (int64_t v = blockIdx.x; v < pl.num_items; v += gridDim.x) {
     const int64_t group = item_group(p, v);
     const int k0 = item_ks(p, v) * p.kchunk, k1 = k0 + p.kchunk < p.K ? k0 + p.kchunk : p.K;
@@ -217,47 +234,67 @@ __device__ __forceinline__ void role_consumer(const ConvParams& p, const Pipe& p
           if (CPASYNC_A) fence_proxy_async_smem();   // the A stage was written by cp.async copies (generic proxy)
           const uint32_t a_hi = smem_u32(pl.a_smem + (size_t)sa * pl.a_stage_bytes) + (uint32_t)g * (64 * 128), a_lo = a_hi + A_TILE_BYTES;
           const uint64_t da_hi = make_desc_sw128(a_hi, 16, 1024), da_lo = make_desc_sw128(a_lo, 16, 1024);
-          wg_fence();
+          // one chunk's k-steps (3 products each in bf16x3 mode) into acc[c], B columns from `col` of the weight slice
+          auto mma_chunk = [&](float (&a)[CH / 2], int col) {
+            const uint64_t db_hi = make_desc_sw128(b_hi + (uint32_t)col * 128u, 16, 1024);
+            const uint64_t db_lo = make_desc_sw128(b_lo + (uint32_t)col * 128u, 16, 1024);
 #pragma unroll
-          for (int c = 0; c < NCH; ++c) {
-            const int col = c * CH - t * p.ncols;     // chunk column inside tile t
-            if (col >= 0 && col < ncols) {
-              const uint64_t db_hi = make_desc_sw128(b_hi + (uint32_t)col * 128u, 16, 1024);
-              const uint64_t db_lo = make_desc_sw128(b_lo + (uint32_t)col * 128u, 16, 1024);
-#pragma unroll
-              for (int j = 0; j < KBLK / 16; ++j) {   // the start-address field (16-byte units) advances by 2 per 32 bytes
-                if constexpr (CH == 64) {
-                  wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(acc[c]), da_hi + 2 * j, db_hi + 2 * j);
-                  if (NSPLIT == 3) {
-                    wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(acc[c]), da_lo + 2 * j, db_hi + 2 * j);
-                    wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(acc[c]), da_hi + 2 * j, db_lo + 2 * j);
-                  }
-                } else {
-                  wgmma_n16(*reinterpret_cast<float(*)[8]>(acc[c]), da_hi + 2 * j, db_hi + 2 * j);
-                  if (NSPLIT == 3) {
-                    wgmma_n16(*reinterpret_cast<float(*)[8]>(acc[c]), da_lo + 2 * j, db_hi + 2 * j);
-                    wgmma_n16(*reinterpret_cast<float(*)[8]>(acc[c]), da_hi + 2 * j, db_lo + 2 * j);
-                  }
+            for (int j = 0; j < KBLK / 16; ++j) {   // the start-address field (16-byte units) advances by 2 per 32 bytes
+              if constexpr (CH == 128) {
+                wgmma_n128<0, 0>(a, da_hi + 2 * j, db_hi + 2 * j);
+                if (NSPLIT == 3) {
+                  wgmma_n128<0, 0>(a, da_lo + 2 * j, db_hi + 2 * j);
+                  wgmma_n128<0, 0>(a, da_hi + 2 * j, db_lo + 2 * j);
+                }
+              } else if constexpr (CH == 64) {
+                wgmma_n64<0, 0>(a, da_hi + 2 * j, db_hi + 2 * j);
+                if (NSPLIT == 3) {
+                  wgmma_n64<0, 0>(a, da_lo + 2 * j, db_hi + 2 * j);
+                  wgmma_n64<0, 0>(a, da_hi + 2 * j, db_lo + 2 * j);
+                }
+              } else {
+                wgmma_n16(a, da_hi + 2 * j, db_hi + 2 * j);
+                if (NSPLIT == 3) {
+                  wgmma_n16(a, da_lo + 2 * j, db_hi + 2 * j);
+                  wgmma_n16(a, da_hi + 2 * j, db_lo + 2 * j);
                 }
               }
             }
+          };
+          wg_fence();
+          if constexpr (CH == 128) {
+            // column ranges of exactly 128 (C_out % 128 == 0): T = 1 and the tile fills chunk 0, so the slot's MMAs and
+            // its commit are one basic block
+            mma_chunk(acc[0], 0);
+            wg_commit();
+          } else {
+            // the tile's chunks: each chain is committed inside its own branch
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) {
+              const int col = c * CH - t * p.ncols;     // chunk column inside tile t
+              if (col >= 0 && col < ncols) {
+                mma_chunk(acc[c], col);
+                wg_commit();
+              }
+            }
           }
-          wg_commit();
-          wg_wait<0>();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(pl.aempty + sa));
+          wg_wait<1>();                        // the previous slot's MMAs are complete
+          release_held();
+          held_a = sa;
+          held_b = t == pl.T - 1 ? sb : -1;    // the B stage is free after its last tile's MMAs
           if (++sa == p.sa) {
             sa = 0;
             pa ^= 1;
           }
         }
-        if (lane == 0) mbar_arrive(smem_u32(pl.bempty + sb));
         if (++sb == p.sb) {
           sb = 0;
           pb ^= 1;
         }
       }
     }
+    wg_wait<0>();
+    release_held();
     // ---- epilogue ----
     float* out_part = p.out + item_ks(p, v) * p.n_out * p.out_pitch;    // this split's partial output
     const int n0 = item_n0(p, v);
@@ -313,7 +350,8 @@ __device__ __forceinline__ void role_consumer(const ConvParams& p, const Pipe& p
 template <int NSPLIT, bool CPASYNC_A>
 __device__ __forceinline__ void run_consumer(const ConvParams& p, const Pipe& pl, int warp, int lane) {
   const int g = (warp - CONS_WARP0) >> 2, wq = (warp - CONS_WARP0) & 3;
-  if (p.Cout % 64 == 0) role_consumer<NSPLIT, CPASYNC_A, 64>(p, pl, g, wq, lane);
+  if (p.Cout % 128 == 0) role_consumer<NSPLIT, CPASYNC_A, 128>(p, pl, g, wq, lane);   // column ranges of exactly 128
+  else if (p.Cout % 64 == 0) role_consumer<NSPLIT, CPASYNC_A, 64>(p, pl, g, wq, lane);
   else role_consumer<NSPLIT, CPASYNC_A, 16>(p, pl, g, wq, lane);
 }
 
@@ -336,7 +374,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
   uint64_t* bempty = bars + 3 * MAX_STAGES;       // [MAX_STAGES]
   double* stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;   // [2*Cout]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
   const int KB = p.Cin / KBLK;
   const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
   const int64_t num_groups = (num_tiles + T - 1) / T;
@@ -362,7 +400,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
   pl.num_items = num_groups * p.ksplit * p.nsplit;
 
   if (warp < NUM_GATHER_WARPS) {
-    reg_alloc<GATHER_REGS>();
+    reg_alloc<TC_GATHER_REGS>();
     // ===================================== gather producers =====================================
     const int chunk = lane & 15;  // 16-byte fp32 chunk inside the 64-channel block
     const int rsub = lane >> 4;   // which of the 2 rows this half-warp handles per step
@@ -530,7 +568,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
     reg_dealloc<LOAD_REGS>();
     if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, n_op);
   } else {
-    reg_alloc<CONS_REGS>();
+    reg_alloc<TC_CONS_REGS>();
     run_consumer<NSPLIT, false>(p, pl, warp, lane);
   }
 }
@@ -575,7 +613,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
   uint64_t* bempty = bars + 3 * MAX_STAGES;       // [MAX_STAGES]
   double* stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;   // [2*Cout]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
   const int KB = p.Cin / KBLK;
   const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
   const int64_t num_groups = (num_tiles + T - 1) / T;
@@ -601,7 +639,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
   pl.num_items = num_groups * p.ksplit * p.nsplit;
 
   if (warp < NUM_GATHER_WARPS) {
-    reg_alloc<GATHER_REGS>();
+    reg_alloc<PL_GATHER_REGS>();
     // ===================================== plane-gather producers =====================================
     // ONE WARP PER SLOT: warp w fills the slots n ≡ w (mod 8) of the CTA's slot sequence (work item → k → kb → tile),
     // all 128 rows of the tile.  (A first version let every warp fill 16 rows of EVERY slot: ncu showed ~300
@@ -711,7 +749,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
     reg_dealloc<LOAD_REGS>();
     if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, n_op);
   } else {
-    reg_alloc<CONS_REGS>();
+    reg_alloc<PL_CONS_REGS>();
     run_consumer<NSPLIT, true>(p, pl, warp, lane);
   }
 }
@@ -801,7 +839,7 @@ int conv_forward_impl(const float* in, int64_t n_in, const int32_t* nbr, int32_t
     sa = (smem_optin - fixed - sb * b_stage) / a_stage;
   }
   if (sa > MAX_STAGES) sa = MAX_STAGES;
-  PASCO_CHECK_ARG(sa >= 2, "pasco_conv_forward_tc: not enough shared memory (Cout=%d)", Cout);
+  PASCO_CHECK_ARG(sa >= 3, "pasco_conv_forward_tc: not enough shared memory (Cout=%d)", Cout);   // see role_consumer
   ConvParams p;
   p.in = in; p.nbr = nbr; p.wpk = (const uint8_t*)packed_w; p.bias = bias;
   p.in_scale = in_scale; p.in_shift = in_shift; p.out = out; p.stats = stats;
@@ -891,8 +929,8 @@ extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t
   int sa = (smem_optin - fixed - sb * b_stage) / a_stage;
   if (sa > MAX_STAGES) sa = MAX_STAGES;
   static const int sa_env = [] { const char* e = getenv("PASCO_PL_SA"); return e ? atoi(e) : 0; }();
-  if (sa_env >= 2 && sa_env < sa) sa = sa_env;
-  PASCO_CHECK_ARG(sa >= 2, "pasco_conv_forward_planes: not enough shared memory (Cout=%d)", Cout);
+  if (sa_env >= 3 && sa_env < sa) sa = sa_env;
+  PASCO_CHECK_ARG(sa >= 3, "pasco_conv_forward_planes: not enough shared memory (Cout=%d)", Cout);   // see role_consumer
   ConvParams p;
   p.in = nullptr; p.nbr = nbr; p.wpk = (const uint8_t*)packed_w; p.bias = bias;
   p.in_scale = nullptr; p.in_shift = nullptr; p.out = out; p.stats = stats;

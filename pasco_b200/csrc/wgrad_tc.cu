@@ -241,7 +241,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
   uint64_t* gfull_bar = bars + 2 * MAX_STAGES;       // [2]
   uint64_t* gempty_bar = bars + 2 * MAX_STAGES + 2;  // [2]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
   const int CB = p.Cin / 64;
   const int pass = blockIdx.x % p.passes;
   const int cta_in_pass = blockIdx.x / p.passes;
@@ -452,7 +452,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
   uint64_t* gfull_bar = bars + 2 * MAX_STAGES;       // [2]
   uint64_t* gempty_bar = bars + 2 * MAX_STAGES + 2;  // [2]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
   const int CB = p.Cin / 64;
   const int pass = blockIdx.x % p.passes;
   const int cta_in_pass = blockIdx.x / p.passes;

@@ -6,22 +6,28 @@ assignments are sound for `k_wgrad_pl` (and, without the gout ring, `k_conv_pl`)
   * consumers (the kernels): nc warpgroups each consume EVERY slot in order; a stage is free once all nc have arrived
     (`every=True`) — sound for any nc;
   * one warp fills every gout tile (double buffer).
+With `lag=True` a consumer keeps one wgmma group in flight: it releases slot n - 1 (and, after a row tile's last unit,
+that tile's gout buffer) only once it has taken slot n, and releases its last slot at the end.  `k_conv_pl` does this and
+maps onto the replay with W = sa producer warps, its weight ring as the gout ring (`gbufs` = its depth sb, 2 or 3) and
+its T tiles per weight slice as the units.  In `k_conv_tc` all 8 gather warps fill every slot and each waits on every
+slot's "empty" barrier in order; a slot is full once the last of them has arrived, so each behaves as the single
+producer Wu = 1 of the replay.
 The earlier kernels split the units over nm MMA issuers instead (issuer m owned units u = m (mod nm), `every=False`),
 which is sound only if nm divides both `nunits` and `stages`; the two issuer configurations that hung / corrupted tiles on
 the GPU (7 producers on 8 stages with 2 issuers, 4 issuers on 6 stages) still fail here and pin the rule.
     python tools/pipeline_sim.py"""
 import random
 def passed(cnt, parity): return (cnt & 1) != parity
-def sim(Wu, nunits, stages, nm, rts, seed, every=False):
+def sim(Wu, nunits, stages, nm, rts, seed, every=False, lag=False, gbufs=2):
     rnd=random.Random(seed)
-    full=[0]*stages; empty=[0]*stages; gfull=[0,0]; gempty=[0,0]; arrived=[0]*stages
+    full=[0]*stages; empty=[0]*stages; gfull=[0]*gbufs; gempty=[0]*gbufs; arrived=[0]*stages
     data=[None]*stages   # which ord currently in stage (to detect overwrite-before-consume)
     consumed=set(); err=[]
     total=rts*nunits
     def g_filler():
         for rti in range(rts):
-            gb=rti&1
-            while not passed(gempty[gb], ((rti>>1)&1)^1): yield
+            gb=rti%gbufs
+            while not passed(gempty[gb], ((rti//gbufs)&1)^1): yield
             gfull[gb]+=1; yield
     def producer(w):
         o=w; st=w; ph=0
@@ -32,25 +38,39 @@ def sim(Wu, nunits, stages, nm, rts, seed, every=False):
             o+=Wu; st+=Wu
             if st>=stages: st-=stages; ph^=1
             yield
+    def release(st, o):
+        arrived[st]+=1
+        if not every or arrived[st]==nm:   # every=True: the stage is free once all nm consumers arrived
+            arrived[st]=0; consumed.add(o); empty[st]+=1
+    def release_g(gb):
+        gcommit[gb]+=1
+        if gcommit[gb]%nm==0: gempty[gb]+=1
     def issuer(m):
         st=0; ph=0
+        held=None                          # lag=True: (stage, ord, gout buffer or None) of the slot still in flight
         for git in range(rts):
-            gb=git&1
-            while not passed(gfull[gb], (git>>1)&1): yield
+            gb=git%gbufs
+            while not passed(gfull[gb], (git//gbufs)&1): yield
             for u in range(nunits):
                 if every or u%nm==m:
                     while not passed(full[st], ph): yield
                     o=git*nunits+u
                     if data[st]!=o: err.append(('wrongdata',o,data[st]))
-                    arrived[st]+=1
-                    if not every or arrived[st]==nm:   # every=True: the stage is free once all nm consumers arrived
-                        arrived[st]=0; consumed.add(o); empty[st]+=1
+                    if lag:
+                        if held is not None:
+                            release(held[0], held[1])
+                            if held[2] is not None: release_g(held[2])
+                        held=(st, o, gb if u==nunits-1 else None)
+                    else:
+                        release(st, o)
                 st+=1
                 if st==stages: st=0; ph^=1
                 yield
-            gcommit[gb]+=1
-            if gcommit[gb]%nm==0: gempty[gb]+=1
-    gcommit=[0,0]
+            if not lag: release_g(gb)
+        if held is not None:
+            release(held[0], held[1])
+            if held[2] is not None: release_g(held[2])
+    gcommit=[0]*gbufs
     agents=[g_filler()]+[producer(w) for w in range(Wu)]+[issuer(m) for m in range(nm)]
     alive=list(range(len(agents))); idle=0
     while alive:
@@ -82,6 +102,9 @@ if __name__ == "__main__":
     for stages in range(2, 9):                      # the current kernels: two consumer warpgroups see every slot
         res=[sim(producer_choice(stages),4,stages,2,14,s,every=True) for s in range(40)]
         print("consumers", stages, {k:res.count(k) for k in set(res)})
+    for sa in range(3, 9):                          # k_conv_pl, one wgmma group in flight per consumer
+        res=[sim(W,t,sa,2,14,s,every=True,lag=True,gbufs=sb) for W in (sa,1) for t in (1,2,4) for sb in (2,3) for s in range(5)]
+        print("lagged conv consumers", sa, {k:res.count(k) for k in set(res)})
     for (Wu,nunits,stages,nm) in ((7,8,8,2),(4,8,8,2),(4,8,8,4),(6,8,6,2),(6,6,6,3),(4,4,4,4),(5,4,5,1),(7,7,8,1),(2,2,2,2),(6,8,6,4)):
         res=[sim(Wu,nunits,stages,nm,14,s) for s in range(80)]
         print((Wu,nunits,stages,nm), {k:res.count(k) for k in set(res)})
