@@ -134,16 +134,15 @@ int pasco_conv_pack_weights(const float* W, int32_t K, int32_t Cin, int32_t Cout
                             pasco_stream_t s);
 /* koff_map (host int32[K] or NULL): packed weight slice used for table row k; must be the identity
  * (NULL) or the reversal K-1-k (mirrored offsets of the input gradient).  K <= 1024.
- * bias: float32[Cout] or NULL.  in_scale/in_shift: optional per-input-channel affine applied
- * in the gather prologue (fused BatchNorm), in_act: 0 none, 1 ReLU, 2 LeakyReLU(0.01) after it.
+ * bias: float32[Cout] or NULL.  The input rows are read as they are; a BatchNorm + activation in front of the
+ * convolution is fused into pasco_split_planes instead (plane-gather path below).
  * stats: optional float64[2*Cout] accumulating column sum / sum of squares of the output.
  * in_pitch / out_pitch: row strides in floats (0 = Cin / Cout) so that a column block of a wider matrix can be
  * read / written in place — dense Linear layers run as K = 1, nbr = NULL convolutions in column chunks <= 256.  */
 int pasco_conv_forward_tc(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out,
                           int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
-                          const float* bias, const float* in_scale, const float* in_shift, int32_t in_act,
-                          double* stats, float* out, int32_t precision, int64_t in_pitch, int64_t out_pitch,
-                          pasco_stream_t s);
+                          const float* bias, double* stats, float* out, int32_t precision, int64_t in_pitch,
+                          int64_t out_pitch, pasco_stream_t s);
 /* Split-K form of the same convolution for shapes with few output tiles and many offsets (the dense bottleneck of
  * layers.py:646-726 runs as 32 tiles x 245 offsets: one CTA per tile would leave most SMs idle).  The offsets are
  * cut into ranges, every (tile, range) pair is a work item whose partial result goes to the caller's workspace, and a
@@ -151,10 +150,9 @@ int pasco_conv_forward_tc(const float* in, int64_t n_in, const int32_t* nbr, int
  * pasco_conv_splitk_workspace_bytes returns 0 when the shape is not worth splitting (then call pasco_conv_forward_tc). */
 int64_t pasco_conv_splitk_workspace_bytes(int32_t K, int64_t n_out, int32_t Cout);
 int pasco_conv_forward_splitk(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out, int32_t Cin,
-                              int32_t Cout, const void* packed_w, const int32_t* koff_map, const float* bias,
-                              const float* in_scale, const float* in_shift, int32_t in_act, float* out, int32_t precision,
-                              int64_t in_pitch, int64_t out_pitch, void* workspace, int64_t workspace_bytes,
-                              pasco_stream_t s);
+                              int32_t Cout, const void* packed_w, const int32_t* koff_map, const float* bias, float* out,
+                              int32_t precision, int64_t in_pitch, int64_t out_pitch, void* workspace,
+                              int64_t workspace_bytes, pasco_stream_t s);
 
 /* Plane-gather path (the default for every gathered convolution): the activations are split ONCE per tensor into bf16
  * planes x = hi + lo (lo = NULL for precision 1) by pasco_split_planes — optionally fused with y = act(x*scale + shift),
@@ -176,9 +174,8 @@ int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int64_t n_in, 
 
 /* dW[k] = sum_o in[nbr[k,o],:]^T @ gout[o,:]   (wgmma, MN-major operands); dW float32 [K,Cin,Cout] zeroed by caller */
 int pasco_conv_wgrad_tc(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out, int32_t Cin,
-                        int32_t Cout, const float* gout, const float* in_scale, const float* in_shift,
-                        int32_t in_act, float* dW, int32_t precision, int64_t in_pitch, int64_t gout_pitch,
-                        pasco_stream_t s);
+                        int32_t Cout, const float* gout, float* dW, int32_t precision, int64_t in_pitch,
+                        int64_t gout_pitch, pasco_stream_t s);
 
 /* CUDA-core fp32 reference path of the same contraction (any Cin/Cout; validation + odd shapes) */
 int pasco_conv_forward_simt(const float* in, const int32_t* nbr, int32_t K, int64_t n_out, int32_t Cin,

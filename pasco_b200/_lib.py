@@ -40,13 +40,13 @@ PROTOTYPES = {
     "pasco_dense_occupancy": (C.c_int, [_p, _i32, _i32, _i64, _p, _p]),
     "pasco_conv_packed_bytes": (_i64, [_i32, _i32, _i32]),
     "pasco_conv_pack_weights": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p]),
-    "pasco_conv_forward_tc": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _p, _i32, _p, _p, _i32, _i64, _i64, _p]),
+    "pasco_conv_forward_tc": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _p, _i32, _i64, _i64, _p]),
     "pasco_conv_splitk_workspace_bytes": (_i64, [_i32, _i64, _i32]),
-    "pasco_conv_forward_splitk": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _p, _i32, _p, _i32, _i64, _i64, _p, _i64, _p]),
+    "pasco_conv_forward_splitk": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _i32, _i64, _i64, _p, _i64, _p]),
     "pasco_split_planes": (C.c_int, [_p, _i64, _i32, _i64, _p, _p, _i32, _p, _p, _p]),
     "pasco_conv_forward_planes": (C.c_int, [_p, _p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _p, _i32, _i64, _i64, _p]),
     "pasco_conv_wgrad_planes": (C.c_int, [_p, _p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _i32, _i64, _i64, _p]),
-    "pasco_conv_wgrad_tc": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _i32, _p, _i32, _i64, _i64, _p]),
+    "pasco_conv_wgrad_tc": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _i32, _i64, _i64, _p]),
     "pasco_conv_forward_simt": (C.c_int, [_p, _p, _i32, _i64, _i32, _i32, _p, _i32, _p, _p, _p, _p]),
     "pasco_conv_wgrad_simt": (C.c_int, [_p, _p, _i32, _i64, _i32, _i32, _p, _p, _p]),
     "pasco_maxpool_forward": (C.c_int, [_p, _p, _i64, _i32, _p, _p]),

@@ -7,10 +7,9 @@
 // slice W[k] is fetched from L2 once per group instead of once per tile.  Outputs wider than 128 channels are cut into
 // column ranges, one work item each.  Warp roles:
 //   warps 0-7   gather: load the neighbour rows of a tile (coalesced 16-byte loads, 16 lanes per 256-byte row
-//               segment; neighbour indices arrive through a cp.async ring one offset ahead), optionally apply
-//               the fused BatchNorm affine + activation of the producing layer, split fp32 → bf16 hi (+ lo), and
-//               store the 128x64 tile into shared memory in the 128-byte-swizzled K-major layout.  Loads of
-//               slot s+1 are in flight in registers while slot s is converted and stored.
+//               segment; neighbour indices arrive through a cp.async ring one offset ahead), split fp32 → bf16
+//               hi (+ lo), and store the 128x64 tile into shared memory in the 128-byte-swizzled K-major layout.
+//               Loads of slot s+1 are in flight in registers while slot s is converted and stored.
 //   warps 8-15  two consumer warpgroups: warpgroup g issues wgmma (M=64 rows [64 g, 64 g + 64), N=128, 64 or 16, K=16)
 //               into register accumulators, then adds the bias and stores its fp32 rows.
 //   warp  16    streams the pre-swizzled weight slices with bulk async copies into their own ring (warps 17-19 only
@@ -21,7 +20,6 @@
 // hi·hi + lo·hi + hi·lo accumulate in fp32 — ~2^-16 relative error, well inside the 1e-3 parity bound.
 #include "common.cuh"
 #include "gmma.cuh"
-#include <cstdlib>
 
 using namespace pasco;
 using namespace gmma;
@@ -52,27 +50,26 @@ constexpr int MAX_STAGES = 8;
 constexpr int ACC_COLS = 128;               // accumulator columns per consumer warpgroup (64 fp32 registers per thread)
 
 struct ConvParams {
-  const float* in;
+  const float* in;     // k_conv_tc: the fp32 input rows
+  const uint16_t* pl_hi;   // k_conv_pl: the input as pre-split bf16 planes x = hi + lo, [n_in, Cin] each
+  const uint16_t* pl_lo;
   const int32_t* nbr;  // [K, n_out] or nullptr (identity)
   const uint8_t* wpk;  // packed weights
   const float* bias;
-  const float* in_scale;
-  const float* in_shift;
   float* out;
   double* stats;       // optional [2*Cout]: column sums / sums of squares of `out` accumulate here (fused BN statistics)
   int64_t n_out;
   int64_t out_pitch;   // row stride of out (floats)
-  int64_t in_pitch;    // row stride of in (floats)
-  int K, Cin, Cout, in_act;
+  int64_t in_pitch;    // row stride of in (floats) or of the planes (elements)
+  int K, Cin, Cout;
+  // split-K: offset range ks < ksplit covers [ks*kchunk, (ks+1)*kchunk); partial results go to
+  // out + ks * n_out * out_pitch (summed by k_splitk_reduce).  kchunk sits here rather than beside ksplit: with this
+  // layout of the int fields ptxas emits about 1 % fewer instructions in the conv kernels.
+  int kchunk;
   int sa, sb, tiles_per_group;
   int nsplit, ncols;          // output columns in ranges of ncols (the last one may be narrower), one work item each
   int koff_base, koff_step;   // weight slice of table row k = koff_base + koff_step * k
-  int ksplit, kchunk;         // split-K: offset range ks covers [ks*kchunk, (ks+1)*kchunk); partial results go to
-                              // out + ks * n_out * out_pitch (summed by k_splitk_reduce)
-  // k_conv_pl only: the input as pre-split bf16 planes x = hi + lo, [n_in, Cin] each with row pitch pl_pitch (elements)
-  const uint16_t* pl_hi;
-  const uint16_t* pl_lo;
-  int64_t pl_pitch;
+  int ksplit;                 // offset ranges (1: no split)
 };
 
 // ------------------------------------------------------------------------------------------------------------
@@ -113,22 +110,6 @@ __global__ void k_pack_weights(const float* __restrict__ W, int K, int Cin, int 
 // ------------------------------------------------------------------------------------------------------------
 // forward / dgrad kernel
 // ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float act_apply(float z, int act) {
-  if (act == 1) return fmaxf(z, 0.f);
-  if (act == 2) return z > 0.f ? z : 0.01f * z;
-  return z;
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// cp.async helpers for the neighbour-index ring
-// ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void cp_async4(uint32_t dst_smem, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst_smem), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 constexpr int IDX_RING = 6;  // neighbour-index ring depth (entries of T*128 ints, one per (tile group, offset))
 
 // position of a gather warp inside the flat slot sequence  group → k → kb → t
@@ -147,12 +128,53 @@ struct SlotIt {
 struct Pipe {
   uint8_t* a_smem;          // [sa][A_hi | A_lo]
   uint8_t* b_smem;          // [sb][B_hi | B_lo]
+  int* idx_ring;            // k_conv_tc: [IDX_RING][T*128] neighbour indices
   uint64_t *afull, *aempty, *bfull, *bempty;
   double* stat_acc;         // [2*Cout] per-CTA accumulators in shared memory (nullptr: no fused statistics)
   int a_stage_bytes, b_tile;
   int KB, T;
-  int64_t num_tiles, num_groups, num_items;
+  int64_t num_items;
 };
+
+// The preamble of both kernels: carve the dynamic shared memory into
+//   [sa] A stages | [sb] B stages | idx_bytes of index ring | 4 x MAX_STAGES barriers | [2*Cout] statistics,
+// zero the statistics and initialise the barriers.  An A "full" barrier completes after afull_arrivals arrivals: one per
+// gather warp in k_conv_tc, one cp.async arrival per lane of the filling warp in k_conv_pl.
+template <int NSPLIT>
+__device__ __forceinline__ Pipe pipe_setup(const ConvParams& p, uint8_t* smem_raw, int idx_bytes, uint32_t afull_arrivals) {
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  constexpr int n_op = (NSPLIT == 3) ? 2 : 1;
+  Pipe pl;
+  pl.b_tile = p.ncols * 128;
+  pl.a_stage_bytes = n_op * A_TILE_BYTES;
+  pl.a_smem = smem;
+  pl.b_smem = smem + (size_t)p.sa * pl.a_stage_bytes;
+  pl.idx_ring = reinterpret_cast<int*>(pl.b_smem + (size_t)p.sb * n_op * pl.b_tile);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(pl.idx_ring) + idx_bytes);
+  pl.afull = bars;
+  pl.aempty = bars + MAX_STAGES;
+  pl.bfull = bars + 2 * MAX_STAGES;
+  pl.bempty = bars + 3 * MAX_STAGES;
+  pl.stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;
+  pl.KB = p.Cin / KBLK;
+  pl.T = p.tiles_per_group;
+  const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
+  pl.num_items = (num_tiles + pl.T - 1) / pl.T * p.ksplit * p.nsplit;
+
+  if (pl.stat_acc)
+    for (int i = threadIdx.x; i < 2 * p.Cout; i += NUM_THREADS) pl.stat_acc[i] = 0.0;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < MAX_STAGES; ++s) {
+      mbar_init(smem_u32(pl.afull + s), afull_arrivals);
+      mbar_init(smem_u32(pl.aempty + s), NUM_CONS_WARPS);
+      mbar_init(smem_u32(pl.bfull + s), 1);
+      mbar_init(smem_u32(pl.bempty + s), NUM_CONS_WARPS);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  return pl;
+}
 
 // work item v = (tile group, offset range, column range): columns vary fastest, then offset ranges
 __device__ __forceinline__ int64_t item_group(const ConvParams& p, int64_t v) { return v / ((int64_t)p.ksplit * p.nsplit); }
@@ -355,56 +377,19 @@ __device__ __forceinline__ void run_consumer(const ConvParams& p, const Pipe& pl
   else role_consumer<NSPLIT, CPASYNC_A, 16>(p, pl, g, wq, lane);
 }
 
-template <int NSPLIT, bool PROLOGUE>
+template <int NSPLIT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int n_op = (NSPLIT == 3) ? 2 : 1;
-  const int b_tile = p.ncols * 128;
-  const int a_stage_bytes = n_op * A_TILE_BYTES;
-  const int b_stage_bytes = n_op * b_tile;
-  const int T = p.tiles_per_group;
-  uint8_t* a_smem = smem;                                           // [sa][A_hi | A_lo]
-  uint8_t* b_smem = smem + (size_t)p.sa * a_stage_bytes;            // [sb][B_hi | B_lo]
-  int* idx_ring = reinterpret_cast<int*>(b_smem + (size_t)p.sb * b_stage_bytes);   // [IDX_RING][T*128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(idx_ring + IDX_RING * T * BLOCK_M);
-  uint64_t* afull = bars;                         // [MAX_STAGES]
-  uint64_t* aempty = bars + MAX_STAGES;           // [MAX_STAGES]
-  uint64_t* bfull = bars + 2 * MAX_STAGES;        // [MAX_STAGES]
-  uint64_t* bempty = bars + 3 * MAX_STAGES;       // [MAX_STAGES]
-  double* stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;   // [2*Cout]
-
+  const Pipe pl = pipe_setup<NSPLIT>(p, smem_raw, IDX_RING * p.tiles_per_group * BLOCK_M * (int)sizeof(int), NUM_GATHER_WARPS);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
-  const int KB = p.Cin / KBLK;
-  const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
-  const int64_t num_groups = (num_tiles + T - 1) / T;
-
-  if (stat_acc)
-    for (int i = threadIdx.x; i < 2 * p.Cout; i += NUM_THREADS) stat_acc[i] = 0.0;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) {
-      mbar_init(smem_u32(afull + s), NUM_GATHER_WARPS);
-      mbar_init(smem_u32(aempty + s), NUM_CONS_WARPS);
-      mbar_init(smem_u32(bfull + s), 1);
-      mbar_init(smem_u32(bempty + s), NUM_CONS_WARPS);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  Pipe pl;
-  pl.a_smem = a_smem; pl.b_smem = b_smem;
-  pl.afull = afull; pl.aempty = aempty; pl.bfull = bfull; pl.bempty = bempty;
-  pl.stat_acc = stat_acc;
-  pl.a_stage_bytes = a_stage_bytes; pl.b_tile = b_tile;
-  pl.KB = KB; pl.T = T; pl.num_tiles = num_tiles; pl.num_groups = num_groups;
-  pl.num_items = num_groups * p.ksplit * p.nsplit;
+  const int T = pl.T, KB = pl.KB;
+  int* idx_ring = pl.idx_ring;
 
   if (warp < NUM_GATHER_WARPS) {
     reg_alloc<TC_GATHER_REGS>();
     // ===================================== gather producers =====================================
     const int chunk = lane & 15;  // 16-byte fp32 chunk inside the 64-channel block
     const int rsub = lane >> 4;   // which of the 2 rows this half-warp handles per step
-    const bool affine = PROLOGUE && p.in_scale != nullptr;
 
     // async prefetch of the neighbour indices of (group, k) into ring slot gk % IDX_RING: this warp's 32 rows of
     // each of the group's tiles
@@ -477,10 +462,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
     uint32_t phase = 0;
 
     float4 va[LOADS_PER_SLOT], vb[LOADS_PER_SLOT];
-    uint32_t valid_a = 0, valid_b = 0;
 
     // issue the 16 row-segment loads of one slot into registers
-    auto issue = [&](SlotIt& it, float4 (&v)[LOADS_PER_SLOT], uint32_t& valid) {
+    auto issue = [&](SlotIt& it, float4 (&v)[LOADS_PER_SLOT]) {
       if (it.kb == 0 && it.t == 0) {
         // first use of ring entry gk: it was prefetched IDX_RING-1 entries ago; keep the ring primed
         cp_async_wait<IDX_RING - 2>();
@@ -489,41 +473,25 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
       }
       const int* irow = idx_ring + (it.gk % IDX_RING) * T * BLOCK_M + it.t * BLOCK_M + warp * ROWS_PER_WARP;
       const int cbase = it.kb * KBLK + chunk * 4;
-      valid = 0;
       int srcs[LOADS_PER_SLOT];
 #pragma unroll
       for (int i = 0; i < LOADS_PER_SLOT; ++i) srcs[i] = irow[i * 2 + rsub];
 #pragma unroll
       for (int i = 0; i < LOADS_PER_SLOT; ++i) {
         v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (srcs[i] >= 0) {
-          v[i] = __ldg(reinterpret_cast<const float4*>(p.in + (int64_t)srcs[i] * p.in_pitch + cbase));
-          valid |= 1u << i;
-        }
+        if (srcs[i] >= 0) v[i] = __ldg(reinterpret_cast<const float4*>(p.in + (int64_t)srcs[i] * p.in_pitch + cbase));
       }
     };
     // convert + store one slot into its A stage and publish it
-    auto store = [&](const SlotIt& it, float4 (&v)[LOADS_PER_SLOT], uint32_t valid) {
-      mbar_wait(smem_u32(aempty + stage), phase ^ 1);
-      uint8_t* dst = a_smem + (size_t)stage * a_stage_bytes;
-      float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (PROLOGUE && affine) {
-        const int cbase = it.kb * KBLK + chunk * 4;
-        sc = __ldg(reinterpret_cast<const float4*>(p.in_scale + cbase));
-        sh = __ldg(reinterpret_cast<const float4*>(p.in_shift + cbase));
-      }
+    auto store = [&](float4 (&v)[LOADS_PER_SLOT]) {
+      mbar_wait(smem_u32(pl.aempty + stage), phase ^ 1);
+      uint8_t* dst = pl.a_smem + (size_t)stage * pl.a_stage_bytes;
       // byte offset of (row warp*16 + rsub, 16-byte chunk) inside the swizzled tile; row i*2 adds i*256 and flips
       // the chunk by (i*2 & 7)
       const uint32_t row_base = (uint32_t)(warp * ROWS_PER_WARP + rsub);
 #pragma unroll
       for (int i = 0; i < LOADS_PER_SLOT; ++i) {
-        float4 x = v[i];
-        if (PROLOGUE && ((valid >> i) & 1u)) {
-          x.x = act_apply(fmaf(x.x, sc.x, sh.x), p.in_act);
-          x.y = act_apply(fmaf(x.y, sc.y, sh.y), p.in_act);
-          x.z = act_apply(fmaf(x.z, sc.z, sh.z), p.in_act);
-          x.w = act_apply(fmaf(x.w, sc.w, sh.w), p.in_act);
-        }
+        const float4 x = v[i];
         const uint32_t trow = row_base + i * 2;
         const uint32_t off = trow * 128u + ((((uint32_t)chunk >> 1) ^ (trow & 7u)) << 4) + (((uint32_t)chunk & 1u) << 3);
         if (NSPLIT == 3) {
@@ -537,7 +505,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
       }
       fence_proxy_async_smem();
       __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(afull + stage));
+      if (lane == 0) mbar_arrive(smem_u32(pl.afull + stage));
       if (++stage == p.sa) {
         stage = 0;
         phase ^= 1;
@@ -545,28 +513,28 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
     };
 
     if (ld.valid) {
-      issue(ld, va, valid_a);
+      issue(ld, va);
       advance(ld);
       while (st.valid) {
         if (ld.valid) {
-          issue(ld, vb, valid_b);
+          issue(ld, vb);
           advance(ld);
         }
-        store(st, va, valid_a);
+        store(va);
         advance(st);
         if (!st.valid) break;
         if (ld.valid) {
-          issue(ld, va, valid_a);
+          issue(ld, va);
           advance(ld);
         }
-        store(st, vb, valid_b);
+        store(vb);
         advance(st);
       }
     }
     cp_async_wait<0>();
   } else if (warp >= LOAD_WARP) {
     reg_dealloc<LOAD_REGS>();
-    if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, n_op);
+    if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, NSPLIT == 3 ? 2 : 1);
   } else {
     reg_alloc<TC_CONS_REGS>();
     run_consumer<NSPLIT, false>(p, pl, warp, lane);
@@ -587,56 +555,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
 // cp.async.mbarrier.arrive.noinc on the slot's "full" barrier (expected count = 32), so the barrier completes when the
 // last copy has landed — no wait_group, no software publish step, and the producers run up to `sa` slots ahead of the
 // MMA.  The consumers add a generic→async proxy fence after their barrier wait.
-__device__ __forceinline__ void cp_async16_zfill(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
-}
-// the mbarrier receives one arrival from this thread once all its cp.async copies issued so far have completed
-__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-
 template <int NSPLIT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constant__ ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int n_op = (NSPLIT == 3) ? 2 : 1;
-  const int b_tile = p.ncols * 128;
-  const int a_stage_bytes = n_op * A_TILE_BYTES;
-  const int b_stage_bytes = n_op * b_tile;
-  const int T = p.tiles_per_group;
-  uint8_t* a_smem = smem;                                           // [sa][A_hi | A_lo]
-  uint8_t* b_smem = smem + (size_t)p.sa * a_stage_bytes;            // [sb][B_hi | B_lo]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(b_smem + (size_t)p.sb * b_stage_bytes);
-  uint64_t* afull = bars;                         // [MAX_STAGES]
-  uint64_t* aempty = bars + MAX_STAGES;           // [MAX_STAGES]
-  uint64_t* bfull = bars + 2 * MAX_STAGES;        // [MAX_STAGES]
-  uint64_t* bempty = bars + 3 * MAX_STAGES;       // [MAX_STAGES]
-  double* stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;   // [2*Cout]
-
+  const Pipe pl = pipe_setup<NSPLIT>(p, smem_raw, 0, 32);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
-  const int KB = p.Cin / KBLK;
-  const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
-  const int64_t num_groups = (num_tiles + T - 1) / T;
-
-  if (stat_acc)
-    for (int i = threadIdx.x; i < 2 * p.Cout; i += NUM_THREADS) stat_acc[i] = 0.0;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < MAX_STAGES; ++s) {
-      mbar_init(smem_u32(afull + s), 32);   // one cp.async arrival per lane of the warp that fills the slot
-      mbar_init(smem_u32(aempty + s), NUM_CONS_WARPS);
-      mbar_init(smem_u32(bfull + s), 1);
-      mbar_init(smem_u32(bempty + s), NUM_CONS_WARPS);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  Pipe pl;
-  pl.a_smem = a_smem; pl.b_smem = b_smem;
-  pl.afull = afull; pl.aempty = aempty; pl.bfull = bfull; pl.bempty = bempty;
-  pl.stat_acc = stat_acc;
-  pl.a_stage_bytes = a_stage_bytes; pl.b_tile = b_tile;
-  pl.KB = KB; pl.T = T; pl.num_tiles = num_tiles; pl.num_groups = num_groups;
-  pl.num_items = num_groups * p.ksplit * p.nsplit;
+  const int T = pl.T, KB = pl.KB;
 
   if (warp < NUM_GATHER_WARPS) {
     reg_alloc<PL_GATHER_REGS>();
@@ -708,11 +632,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
     Idx4 q0 = load_idx(it0), q1 = load_idx(it1);
     const uint8_t* base_hi = reinterpret_cast<const uint8_t*>(p.pl_hi);
     const uint8_t* base_lo = reinterpret_cast<const uint8_t*>(p.pl_lo);
-    const int64_t pitch_b = p.pl_pitch * 2;
+    const int64_t pitch_b = p.in_pitch * 2;
     int stage = warp;                               // ring position of this warp's current slot (warp < W <= sa)
     uint32_t phase = 0;
     auto observe = [&]() {                          // wait until the slot's stage is free
-      mbar_wait(smem_u32(aempty + stage), phase ^ 1);
+      mbar_wait(smem_u32(pl.aempty + stage), phase ^ 1);
     };
     auto next_stage = [&]() {                       // this warp's next slot is W slots on (at most one wrap: W <= sa)
       stage += W;
@@ -724,7 +648,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
     while (it0.valid) {
       const Idx4 q2 = load_idx(it2);                // indices of this warp's slot after next
       observe();
-      const uint32_t dst0 = smem_u32(a_smem + (size_t)stage * a_stage_bytes) + (uint32_t)sub * 128u;
+      const uint32_t dst0 = smem_u32(pl.a_smem + (size_t)stage * pl.a_stage_bytes) + (uint32_t)sub * 128u;
       const int64_t coff_b = ((int64_t)it0.kb * KBLK + ch * 8) * 2;
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
@@ -737,7 +661,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
         cp_async16_zfill(dst0 + off, base_hi + boff, nbytes);
         if (NSPLIT == 3) cp_async16_zfill(dst0 + A_TILE_BYTES + off, base_lo + boff, nbytes);
       }
-      cp_async_mbar_arrive_noinc(smem_u32(afull + stage));
+      cp_async_mbar_arrive_noinc(smem_u32(pl.afull + stage));
       next_stage();
       it0 = it1; it1 = it2;
       advance_n(it2, W);
@@ -747,7 +671,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
     cp_async_wait<0>();
   } else if (warp >= LOAD_WARP) {
     reg_dealloc<LOAD_REGS>();
-    if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, n_op);
+    if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, NSPLIT == 3 ? 2 : 1);
   } else {
     reg_alloc<PL_CONS_REGS>();
     run_consumer<NSPLIT, true>(p, pl, warp, lane);
@@ -810,111 +734,27 @@ __global__ void k_splitk_reduce(const float* __restrict__ part, int ksplit, int6
   }
 }
 
-int conv_forward_impl(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out,
-                                     int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
-                                     const float* bias, const float* in_scale, const float* in_shift, int32_t in_act,
-                                     double* stats, float* out, int32_t precision, int64_t in_pitch, int64_t out_pitch,
-                                     int ksplit, float* workspace, pasco_stream_t s) {
-  PASCO_CHECK_ARG(precision == 1 || precision == 3, "pasco_conv_forward_tc: precision must be 1 (bf16) or 3 (bf16x3)");
-  PASCO_CHECK_ARG(Cin % KBLK == 0, "pasco_conv_forward_tc: Cin (%d) must be a multiple of 64", Cin);
-  PASCO_CHECK_ARG(Cout % 16 == 0 && Cout >= 16 && Cout <= 256, "pasco_conv_forward_tc: Cout (%d) must be a multiple of 16 in [16,256]", Cout);
-  PASCO_CHECK_ARG(K >= 1 && K <= 1024, "pasco_conv_forward_tc: K (%d) out of range", K);
-  PASCO_CHECK_ARG((((uintptr_t)in | (uintptr_t)out | (uintptr_t)packed_w) & 15) == 0, "pasco_conv_forward_tc: pointers must be 16-byte aligned");
-  if (n_out == 0) return 0;
-  int dev = 0, smem_optin = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  const int n_op = precision == 3 ? 2 : 1;
-  int64_t tiles = (n_out + BLOCK_M - 1) / BLOCK_M;
-  int nsplit, ncols, T;
-  column_plan(Cout, tiles, nsplit, ncols, T);
-  if (ksplit > 1) T = 1;
-  const int a_stage = n_op * A_TILE_BYTES, b_stage = n_op * ncols * 128;
-  const int idx_bytes = IDX_RING * T * BLOCK_M * 4;
-  const int fixed = 1024 /*align slack*/ + idx_bytes + 4 * MAX_STAGES * 8 + (stats ? 2 * Cout * 8 : 0);
-  int sb = 2;
-  int sa = (smem_optin - fixed - sb * b_stage) / a_stage;
-  if (sa > 5) {  // room to spare: deepen the weight ring first
-    sb = 3;
-    sa = (smem_optin - fixed - sb * b_stage) / a_stage;
-  }
-  if (sa > MAX_STAGES) sa = MAX_STAGES;
-  PASCO_CHECK_ARG(sa >= 3, "pasco_conv_forward_tc: not enough shared memory (Cout=%d)", Cout);   // see role_consumer
-  ConvParams p;
-  p.in = in; p.nbr = nbr; p.wpk = (const uint8_t*)packed_w; p.bias = bias;
-  p.in_scale = in_scale; p.in_shift = in_shift; p.out = out; p.stats = stats;
-  p.n_out = n_out;
-  p.out_pitch = out_pitch > 0 ? out_pitch : Cout;
-  p.ksplit = 1; p.kchunk = K;
-  if (ksplit > 1) {       // partial outputs [ksplit, n_out, Cout] into the workspace, bias added by the reduction
-    p.ksplit = ksplit; p.kchunk = (K + ksplit - 1) / ksplit;
-    p.ksplit = (K + p.kchunk - 1) / p.kchunk;       // no empty ranges
-    p.out = workspace; p.out_pitch = Cout; p.bias = nullptr; p.stats = nullptr;
-  }
-  p.in_pitch = in_pitch > 0 ? in_pitch : Cin;
-  PASCO_CHECK_ARG(p.out_pitch % 4 == 0 && p.in_pitch % 4 == 0, "pasco_conv_forward_tc: pitches must be multiples of 4 floats");
-  p.K = K; p.Cin = Cin; p.Cout = Cout; p.in_act = in_act;
-  p.pl_hi = nullptr; p.pl_lo = nullptr; p.pl_pitch = 0;
-  p.sa = sa; p.sb = sb; p.tiles_per_group = T; p.nsplit = nsplit; p.ncols = ncols;
-  p.koff_base = 0; p.koff_step = 1;
-  if (koff_map) {
-    bool ident = true, rev = true;
-    for (int k = 0; k < K; ++k) {
-      ident = ident && koff_map[k] == k;
-      rev = rev && koff_map[k] == K - 1 - k;
-    }
-    PASCO_CHECK_ARG(ident || rev, "pasco_conv_forward_tc: koff_map must be the identity or the reversal");
-    if (!ident) { p.koff_base = K - 1; p.koff_step = -1; }
-  }
-  const size_t smem = (size_t)sa * a_stage + (size_t)sb * b_stage + fixed;
-  const int64_t items = (tiles + T - 1) / T * p.ksplit * nsplit;
-  const int grid = (int)(items < num_sms() ? items : num_sms());
-  cudaError_t e;
-  const bool prologue = in_scale != nullptr || in_act != 0;
-  auto launch = [&](auto kern) {
-    cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (err == cudaSuccess) kern<<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
-    return err;
-  };
-  if (precision == 3) e = prologue ? launch(k_conv_tc<3, true>) : launch(k_conv_tc<3, false>);
-  else e = prologue ? launch(k_conv_tc<1, true>) : launch(k_conv_tc<1, false>);
-  if (e != cudaSuccess) {
-    set_error("pasco_conv_forward_tc: cudaFuncSetAttribute(%zu bytes) failed: %s", smem, cudaGetErrorString(e));
-    return -1;
-  }
-  PASCO_CHECK_LAUNCH("pasco_conv_forward_tc");
-  if (p.ksplit > 1) {
-    k_splitk_reduce<<<grid_for(n_out * (Cout / 4), 256), 256, 0, (cudaStream_t)s>>>(workspace, p.ksplit, n_out, Cout, bias, out,
-                                                                                out_pitch > 0 ? out_pitch : Cout);
-    PASCO_CHECK_LAUNCH("pasco_conv_forward_tc(split-K reduce)");
-  }
-  return 0;
-}
-
-}  // namespace
-
-extern "C" int pasco_conv_forward_tc(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out,
-                                     int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
-                                     const float* bias, const float* in_scale, const float* in_shift, int32_t in_act,
-                                     double* stats, float* out, int32_t precision, int64_t in_pitch, int64_t out_pitch,
-                                     pasco_stream_t s) {
-  return conv_forward_impl(in, n_in, nbr, K, n_out, Cin, Cout, packed_w, koff_map, bias, in_scale, in_shift, in_act, stats, out,
-                           precision, in_pitch, out_pitch, 1, nullptr, s);
-}
-
-extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t n_in, const int32_t* nbr, int32_t K,
-                                         int64_t n_out, int32_t Cin, int32_t Cout, const void* packed_w,
-                                         const int32_t* koff_map, const float* bias, double* stats, float* out,
-                                         int32_t precision, int64_t plane_pitch, int64_t out_pitch, pasco_stream_t s) {
-  PASCO_CHECK_ARG(precision == 1 || precision == 3, "pasco_conv_forward_planes: precision must be 1 or 3");
-  PASCO_CHECK_ARG(hi != nullptr && (precision == 1 || lo != nullptr), "pasco_conv_forward_planes: missing plane (precision 3 needs hi and lo)");
-  PASCO_CHECK_ARG(Cin % KBLK == 0, "pasco_conv_forward_planes: Cin (%d) must be a multiple of 64", Cin);
-  PASCO_CHECK_ARG(Cout % 16 == 0 && Cout >= 16 && Cout <= 256, "pasco_conv_forward_planes: Cout (%d) must be a multiple of 16 in [16,256]", Cout);
-  PASCO_CHECK_ARG(K >= 1 && K <= 1024, "pasco_conv_forward_planes: K (%d) out of range", K);
-  const int64_t pitch = plane_pitch > 0 ? plane_pitch : Cin;
-  PASCO_CHECK_ARG(pitch % 8 == 0 && (((uintptr_t)hi | (uintptr_t)lo | (uintptr_t)out | (uintptr_t)packed_w) & 15) == 0,
-                  "pasco_conv_forward_planes: planes must be 16-byte aligned with a pitch multiple of 8 elements");
-  (void)n_in;
+// The host half of every forward / input-gradient launch.  The gathered operand is either fp32 rows `in` (register
+// gather, k_conv_tc; split over the offsets when ksplit > 1) or, when `hi` is set, bf16 planes hi [+ lo] (plane gather,
+// k_conv_pl); in_pitch is its row stride in floats or plane elements (0 = Cin).  Error messages name the entry point fn.
+int conv_launch(const char* fn, const float* in, const void* hi, const void* lo, int64_t in_pitch, const int32_t* nbr,
+                int32_t K, int64_t n_out, int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
+                const float* bias, double* stats, float* out, int32_t precision, int64_t out_pitch, int ksplit,
+                float* workspace, pasco_stream_t s) {
+  const bool planes = hi != nullptr;
+  PASCO_CHECK_ARG(precision == 1 || precision == 3, "%s: precision must be 1 (bf16) or 3 (bf16x3)", fn);
+  PASCO_CHECK_ARG(Cin % KBLK == 0, "%s: Cin (%d) must be a multiple of 64", fn, Cin);
+  PASCO_CHECK_ARG(Cout % 16 == 0 && Cout >= 16 && Cout <= 256, "%s: Cout (%d) must be a multiple of 16 in [16,256]", fn, Cout);
+  PASCO_CHECK_ARG(K >= 1 && K <= 1024, "%s: K (%d) out of range", fn, K);
+  if (in_pitch <= 0) in_pitch = Cin;
+  if (out_pitch <= 0) out_pitch = Cout;
+  if (planes)
+    PASCO_CHECK_ARG(in_pitch % 8 == 0 && (((uintptr_t)hi | (uintptr_t)lo) & 15) == 0,
+                    "%s: planes must be 16-byte aligned with a pitch multiple of 8 elements", fn);
+  else
+    PASCO_CHECK_ARG(in_pitch % 4 == 0 && ((uintptr_t)in & 15) == 0, "%s: in must be 16-byte aligned with a pitch multiple of 4 floats", fn);
+  PASCO_CHECK_ARG(out_pitch % 4 == 0 && (((uintptr_t)out | (uintptr_t)packed_w) & 15) == 0,
+                  "%s: out and the packed weights must be 16-byte aligned, out_pitch a multiple of 4 floats", fn);
   if (n_out == 0) return 0;
   int dev = 0, smem_optin = 0;
   cudaGetDevice(&dev);
@@ -923,24 +763,31 @@ extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t
   const int64_t tiles = (n_out + BLOCK_M - 1) / BLOCK_M;
   int nsplit, ncols, T;
   column_plan(Cout, tiles, nsplit, ncols, T);
+  if (ksplit > 1) T = 1;
+  // shared memory (pipe_setup): sa A stages, sb B stages, the neighbour-index ring of k_conv_tc, barriers, statistics
   const int a_stage = n_op * A_TILE_BYTES, b_stage = n_op * ncols * 128;
-  const int fixed = 1024 + 4 * MAX_STAGES * 8 + (stats ? 2 * Cout * 8 : 0);
+  const int idx_bytes = planes ? 0 : IDX_RING * T * BLOCK_M * 4;
+  const int fixed = 1024 /*align slack*/ + idx_bytes + 4 * MAX_STAGES * 8 + (stats ? 2 * Cout * 8 : 0);
   int sb = 2;
   int sa = (smem_optin - fixed - sb * b_stage) / a_stage;
+  if (!planes && sa > 5) {  // register gather with room to spare: deepen the weight ring first
+    sb = 3;
+    sa = (smem_optin - fixed - sb * b_stage) / a_stage;
+  }
   if (sa > MAX_STAGES) sa = MAX_STAGES;
-  static const int sa_env = [] { const char* e = getenv("PASCO_PL_SA"); return e ? atoi(e) : 0; }();
-  if (sa_env >= 3 && sa_env < sa) sa = sa_env;
-  PASCO_CHECK_ARG(sa >= 3, "pasco_conv_forward_planes: not enough shared memory (Cout=%d)", Cout);   // see role_consumer
+  PASCO_CHECK_ARG(sa >= 3, "%s: not enough shared memory (Cout=%d)", fn, Cout);   // see role_consumer
   ConvParams p;
-  p.in = nullptr; p.nbr = nbr; p.wpk = (const uint8_t*)packed_w; p.bias = bias;
-  p.in_scale = nullptr; p.in_shift = nullptr; p.out = out; p.stats = stats;
-  p.n_out = n_out;
-  p.out_pitch = out_pitch > 0 ? out_pitch : Cout;
-  p.in_pitch = Cin;
-  PASCO_CHECK_ARG(p.out_pitch % 4 == 0, "pasco_conv_forward_planes: out_pitch must be a multiple of 4 floats");
-  p.K = K; p.Cin = Cin; p.Cout = Cout; p.in_act = 0;
+  p.in = in; p.pl_hi = (const uint16_t*)hi; p.pl_lo = (const uint16_t*)lo; p.in_pitch = in_pitch;
+  p.nbr = nbr; p.wpk = (const uint8_t*)packed_w; p.bias = bias; p.out = out; p.stats = stats;
+  p.n_out = n_out; p.out_pitch = out_pitch;
+  p.K = K; p.Cin = Cin; p.Cout = Cout;
   p.sa = sa; p.sb = sb; p.tiles_per_group = T; p.nsplit = nsplit; p.ncols = ncols;
   p.ksplit = 1; p.kchunk = K;
+  if (ksplit > 1) {       // partial outputs [ksplit, n_out, Cout] into the workspace, bias added by the reduction
+    p.kchunk = (K + ksplit - 1) / ksplit;
+    p.ksplit = (K + p.kchunk - 1) / p.kchunk;       // no empty ranges
+    p.out = workspace; p.out_pitch = Cout; p.bias = nullptr; p.stats = nullptr;
+  }
   p.koff_base = 0; p.koff_step = 1;
   if (koff_map) {
     bool ident = true, rev = true;
@@ -948,25 +795,46 @@ extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t
       ident = ident && koff_map[k] == k;
       rev = rev && koff_map[k] == K - 1 - k;
     }
-    PASCO_CHECK_ARG(ident || rev, "pasco_conv_forward_planes: koff_map must be the identity or the reversal");
+    PASCO_CHECK_ARG(ident || rev, "%s: koff_map must be the identity or the reversal", fn);
     if (!ident) { p.koff_base = K - 1; p.koff_step = -1; }
   }
-  p.pl_hi = (const uint16_t*)hi; p.pl_lo = (const uint16_t*)lo; p.pl_pitch = pitch;
   const size_t smem = (size_t)sa * a_stage + (size_t)sb * b_stage + fixed;
-  const int64_t items = (tiles + T - 1) / T * nsplit;
+  const int64_t items = (tiles + T - 1) / T * p.ksplit * nsplit;
   const int grid = (int)(items < num_sms() ? items : num_sms());
-  auto launch = [&](auto kern) {
-    cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (err == cudaSuccess) kern<<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
-    return err;
-  };
-  const cudaError_t e = precision == 3 ? launch(k_conv_pl<3>) : launch(k_conv_pl<1>);
+  void (*kern)(ConvParams) = planes ? (precision == 3 ? k_conv_pl<3> : k_conv_pl<1>)
+                                    : (precision == 3 ? k_conv_tc<3> : k_conv_tc<1>);
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) {
-    set_error("pasco_conv_forward_planes: cudaFuncSetAttribute(%zu bytes) failed: %s", smem, cudaGetErrorString(e));
+    set_error("%s: cudaFuncSetAttribute(%zu bytes) failed: %s", fn, smem, cudaGetErrorString(e));
     return -1;
   }
-  PASCO_CHECK_LAUNCH("pasco_conv_forward_planes");
+  kern<<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
+  PASCO_CHECK_LAUNCH(fn);
+  if (p.ksplit > 1) {
+    k_splitk_reduce<<<grid_for(n_out * (Cout / 4), 256), 256, 0, (cudaStream_t)s>>>(workspace, p.ksplit, n_out, Cout, bias, out,
+                                                                                out_pitch);
+    PASCO_CHECK_LAUNCH(fn);
+  }
   return 0;
+}
+
+}  // namespace
+
+extern "C" int pasco_conv_forward_tc(const float* in, int64_t /*n_in*/, const int32_t* nbr, int32_t K, int64_t n_out,
+                                     int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
+                                     const float* bias, double* stats, float* out, int32_t precision, int64_t in_pitch,
+                                     int64_t out_pitch, pasco_stream_t s) {
+  return conv_launch("pasco_conv_forward_tc", in, nullptr, nullptr, in_pitch, nbr, K, n_out, Cin, Cout, packed_w, koff_map,
+                     bias, stats, out, precision, out_pitch, 1, nullptr, s);
+}
+
+extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t /*n_in*/, const int32_t* nbr, int32_t K,
+                                         int64_t n_out, int32_t Cin, int32_t Cout, const void* packed_w,
+                                         const int32_t* koff_map, const float* bias, double* stats, float* out,
+                                         int32_t precision, int64_t plane_pitch, int64_t out_pitch, pasco_stream_t s) {
+  PASCO_CHECK_ARG(hi != nullptr && (precision == 1 || lo != nullptr), "pasco_conv_forward_planes: missing plane (precision 3 needs hi and lo)");
+  return conv_launch("pasco_conv_forward_planes", nullptr, hi, lo, plane_pitch, nbr, K, n_out, Cin, Cout, packed_w, koff_map,
+                     bias, stats, out, precision, out_pitch, 1, nullptr, s);
 }
 
 extern "C" int64_t pasco_conv_splitk_workspace_bytes(int32_t K, int64_t n_out, int32_t Cout) {
@@ -974,16 +842,15 @@ extern "C" int64_t pasco_conv_splitk_workspace_bytes(int32_t K, int64_t n_out, i
   return ks > 1 ? (int64_t)ks * n_out * Cout * 4 : 0;
 }
 
-extern "C" int pasco_conv_forward_splitk(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out,
+extern "C" int pasco_conv_forward_splitk(const float* in, int64_t /*n_in*/, const int32_t* nbr, int32_t K, int64_t n_out,
                                          int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
-                                         const float* bias, const float* in_scale, const float* in_shift, int32_t in_act,
-                                         float* out, int32_t precision, int64_t in_pitch, int64_t out_pitch, void* workspace,
-                                         int64_t workspace_bytes, pasco_stream_t s) {
+                                         const float* bias, float* out, int32_t precision, int64_t in_pitch,
+                                         int64_t out_pitch, void* workspace, int64_t workspace_bytes, pasco_stream_t s) {
   const int ks = splitk_plan(K, n_out);
   PASCO_CHECK_ARG(ks > 1, "pasco_conv_forward_splitk: this shape is not split (workspace_bytes = 0): call pasco_conv_forward_tc");
   PASCO_CHECK_ARG(workspace != nullptr && workspace_bytes >= (int64_t)ks * n_out * Cout * 4,
                   "pasco_conv_forward_splitk: workspace too small (%lld bytes)", (long long)workspace_bytes);
   PASCO_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "pasco_conv_forward_splitk: workspace must be 16-byte aligned");
-  return conv_forward_impl(in, n_in, nbr, K, n_out, Cin, Cout, packed_w, koff_map, bias, in_scale, in_shift, in_act, nullptr, out,
-                           precision, in_pitch, out_pitch, ks, (float*)workspace, s);
+  return conv_launch("pasco_conv_forward_splitk", in, nullptr, nullptr, in_pitch, nbr, K, n_out, Cin, Cout, packed_w, koff_map,
+                     bias, nullptr, out, precision, out_pitch, ks, (float*)workspace, s);
 }

@@ -1,4 +1,5 @@
-// Thin inline-PTX layer for sm_90a: mbarrier, bulk async copy, warpgroup MMA (wgmma) and its shared-memory descriptors.
+// Thin inline-PTX layer for sm_90a: mbarrier, bulk and cp.async copies, warpgroup MMA (wgmma) and its shared-memory
+// descriptors.
 // Bit layouts follow the PTX ISA "matrix descriptor" and "wgmma register fragment" sections; the kernels own their
 // pipelines.
 #pragma once
@@ -62,6 +63,22 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
+}
+
+// ---- cp.async (LDGSTS) global → shared ----------------------------------------------------------------
+__device__ __forceinline__ void cp_async4(uint32_t dst_smem, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst_smem), "l"(src) : "memory");
+}
+// 16 bytes, of which the first src_bytes are read and the rest zero-filled (src_bytes = 0: no memory access)
+__device__ __forceinline__ void cp_async16_zfill(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// the mbarrier receives one arrival from this thread once all its cp.async copies issued so far have completed
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
 
 // named barrier over `nthreads` threads (whole warps), ids 1.. (0 is __syncthreads)

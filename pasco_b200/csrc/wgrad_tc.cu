@@ -8,7 +8,6 @@
 // one range of UC output columns (UC = Cout up to 128); consumer warpgroup h accumulates sub-tile h of the CTA's units
 // in registers (at most 128 columns per thread set), walks its share of 64-row tiles, and finally stores its partial
 // dW into its own workspace slot; k_wgrad_sum adds the slots of a pass in CTA order (deterministic, no atomics).
-#include <stdlib.h>
 #include "common.cuh"
 #include "gmma.cuh"
 
@@ -29,15 +28,16 @@ constexpr int WG_R = 64;                  // voxel rows per tile (contraction bl
 constexpr int WG_SUB_BYTES = WG_R * 128;  // one [64 rows][64 ch] bf16 tile = 8 KB
 
 struct WgradParams {
-  const float* in;
-  const int32_t* nbr;
+  const float* in;                // k_wgrad_tc: fp32 rows of the layer input and of the output gradient
   const float* gout;
-  const float* in_scale;
-  const float* in_shift;
-  float* dW;
+  const uint16_t* in_hi;          // k_wgrad_pl: the same as pre-split bf16 planes (hi [+ lo])
+  const uint16_t* in_lo;
+  const uint16_t* g_hi;
+  const uint16_t* g_lo;
+  const int32_t* nbr;
   int64_t n_out;
-  int64_t in_pitch, gout_pitch;   // row strides (floats)
-  int K, Cin, Cout, in_act;
+  int64_t in_pitch, gout_pitch;   // row strides (floats, or elements of the planes)
+  int K, Cin, Cout;
   int stages;
   int units_per_pass, num_units, num_subs, passes, ctas_per_pass;
   int uc, ncr;                    // columns per unit, column ranges (unit u = sub-tile pair u / ncr, columns of range u % ncr)
@@ -47,60 +47,29 @@ struct WgradParams {
 
 constexpr int IDX_RING = 16;   // unit slots are short: fetch neighbour indices 15 slots ahead (HBM-latency bound otherwise)
 
-__device__ __forceinline__ void cp_async4(uint32_t dst_smem, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst_smem), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ float act_apply(float z, int act) {
-  if (act == 1) return fmaxf(z, 0.f);
-  if (act == 2) return z > 0.f ? z : 0.01f * z;
-  return z;
-}
-
 // One [WG_R rows][64 ch] sub-tile is gathered by 8 warps x 8 rows; lanes (l & 7) of a warp hold the source row of
 // tile row w*8 + (l & 7).  Loads and the convert+store are separate so several sub-tiles can be in flight.
 struct SubRegs {
   float4 v[WLOADS];
-  uint32_t valid;
 };
 
 __device__ __forceinline__ void sub_load(SubRegs& r, const float* __restrict__ src, int ld, int cbase_blk, int idx, int lane) {
   const int chunk = lane & 15, rsub = lane >> 4;
   const int cbase = cbase_blk + chunk * 4;
-  r.valid = 0;
 #pragma unroll
   for (int i = 0; i < WLOADS; ++i) {
     const int s = __shfl_sync(0xffffffffu, idx, i * 2 + rsub);
     r.v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (s >= 0) {
-      r.v[i] = __ldg(reinterpret_cast<const float4*>(src + (int64_t)s * ld + cbase));
-      r.valid |= 1u << i;
-    }
+    if (s >= 0) r.v[i] = __ldg(reinterpret_cast<const float4*>(src + (int64_t)s * ld + cbase));
   }
 }
 
-template <int NSPLIT, bool AFFINE_OK>
-__device__ __forceinline__ void sub_store(const SubRegs& r, uint8_t* dst_hi, uint8_t* dst_lo, int cbase_blk, int warp, int lane,
-                                          const float* scale, const float* shift, int act) {
+template <int NSPLIT>
+__device__ __forceinline__ void sub_store(const SubRegs& r, uint8_t* dst_hi, uint8_t* dst_lo, int warp, int lane) {
   const int chunk = lane & 15, rsub = lane >> 4;
-  float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-  const bool affine = AFFINE_OK && scale != nullptr;
-  if (affine) {
-    sc = __ldg(reinterpret_cast<const float4*>(scale + cbase_blk + chunk * 4));
-    sh = __ldg(reinterpret_cast<const float4*>(shift + cbase_blk + chunk * 4));
-  }
 #pragma unroll
   for (int i = 0; i < WLOADS; ++i) {
-    float4 x = r.v[i];
-    if (AFFINE_OK && (affine || act) && ((r.valid >> i) & 1u)) {
-      x.x = act_apply(fmaf(x.x, sc.x, sh.x), act);
-      x.y = act_apply(fmaf(x.y, sc.y, sh.y), act);
-      x.z = act_apply(fmaf(x.z, sc.z, sh.z), act);
-      x.w = act_apply(fmaf(x.w, sc.w, sh.w), act);
-    }
+    const float4 x = r.v[i];
     const uint32_t trow = (uint32_t)(warp * WROWS + i * 2 + rsub);
     const uint32_t off = trow * 128u + ((((uint32_t)chunk >> 1) ^ (trow & 7u)) << 4) + (((uint32_t)chunk & 1u) << 3);
     if (NSPLIT == 3) {
@@ -118,8 +87,8 @@ __device__ __forceinline__ void sub_store(const SubRegs& r, uint8_t* dst_hi, uin
 // [64 q, 64 q + 64) of the pass's accumulator, i.e. column block q % (uc / 64) of unit q / (uc / 64).  Every consumer
 // warp arrives on the ring "empty" barriers (expected count 8).  After the CTA's last row tile it stores its partial dW
 // into its workspace slot: row (u * 128 + 64 hh + channel), column within the unit.
-template <int NSPLIT, bool CPASYNC, class P>
-__device__ __forceinline__ void wgrad_consumer(const P& p, const uint8_t* g_smem, const uint8_t* a_smem, int g_bytes, int a_bytes,
+template <int NSPLIT, bool CPASYNC>
+__device__ __forceinline__ void wgrad_consumer(const WgradParams& p, const uint8_t* g_smem, const uint8_t* a_smem, int g_bytes, int a_bytes,
                                                uint64_t* full_bar, uint64_t* empty_bar, uint64_t* gfull_bar, uint64_t* gempty_bar,
                                                int unit0, int nunits, int cta_in_pass, int64_t num_rt, int hh, int wq, int lane) {
   const int NB = p.Cout / 64, UNB = p.uc / 64, CB = p.Cin / 64;
@@ -187,8 +156,7 @@ __device__ __forceinline__ void wgrad_consumer(const P& p, const uint8_t* g_smem
 }
 
 // dW[k][ci][co] += Σ_c part[c * passes + pass][...] over the CTAs c of the pass that owns (k, ci, co), in CTA order
-template <class P>
-__global__ void k_wgrad_sum(const P p, float* __restrict__ dW) {
+__global__ void k_wgrad_sum(const WgradParams p, float* __restrict__ dW) {
   const int CB = p.Cin / 64;
   const int64_t total = (int64_t)p.K * p.Cin * p.Cout;
   for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
@@ -203,26 +171,6 @@ __global__ void k_wgrad_sum(const P p, float* __restrict__ dW) {
     for (int c = 0; c < p.ctas_per_pass; ++c) acc += __ldg(src + (int64_t)c * p.passes * p.slot);
     dW[e] += acc;
   }
-}
-
-// the per-CTA partials, summed in a fixed order into dW: stream-ordered workspace around the launch
-template <class P, class Launch>
-int wgrad_launch(P& p, float* dW, cudaStream_t st, const char* name, Launch launch) {
-  p.slot = (int64_t)p.units_per_pass * 128 * p.uc;
-  const int grid = p.passes * p.ctas_per_pass;
-  cudaError_t e = ws_alloc((void**)&p.part, (size_t)grid * p.slot * sizeof(float), st);
-  if (e != cudaSuccess) {
-    set_error("%s: workspace of %lld bytes: %s", name, (long long)grid * p.slot * 4, cudaGetErrorString(e));
-    return -1;
-  }
-  e = launch(grid);
-  if (e == cudaSuccess) k_wgrad_sum<P><<<grid_for((int64_t)p.K * p.Cin * p.Cout, 256), 256, 0, st>>>(p, dW);
-  cudaFreeAsync(p.part, st);
-  if (e != cudaSuccess) {
-    set_error("%s: cudaFuncSetAttribute failed: %s", name, cudaGetErrorString(e));
-    return -1;
-  }
-  return 0;
 }
 
 template <int NSPLIT>
@@ -332,11 +280,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
         if (j == 0) mbar_wait(smem_u32(gempty_bar + gb), ((git >> 1) & 1) ^ 1);
         uint8_t* g = g_smem + (size_t)gb * g_bytes;
         const int nb = j * 2;
-        sub_store<NSPLIT, false>(r[0], g + (size_t)nb * WG_SUB_BYTES, g + (size_t)(NB + nb) * WG_SUB_BYTES, 0, warp, lane,
-                                 nullptr, nullptr, 0);
-        if (dj[2] >= 0)
-          sub_store<NSPLIT, false>(r[1], g + (size_t)(nb + 1) * WG_SUB_BYTES, g + (size_t)(NB + nb + 1) * WG_SUB_BYTES, 0,
-                                   warp, lane, nullptr, nullptr, 0);
+        sub_store<NSPLIT>(r[0], g + (size_t)nb * WG_SUB_BYTES, g + (size_t)(NB + nb) * WG_SUB_BYTES, warp, lane);
+        if (dj[2] >= 0) sub_store<NSPLIT>(r[1], g + (size_t)(nb + 1) * WG_SUB_BYTES, g + (size_t)(NB + nb + 1) * WG_SUB_BYTES, warp, lane);
         if (j == GS - 1) {
           fence_proxy_async_smem();
           __syncwarp();
@@ -346,9 +291,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
         mbar_wait(smem_u32(empty_bar + stage), phase ^ 1);
         uint8_t* a = a_smem + (size_t)stage * a_bytes;
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-          sub_store<NSPLIT, true>(r[h], a + (size_t)h * WG_SUB_BYTES, a + (size_t)(2 + h) * WG_SUB_BYTES, dj[1 + h], warp, lane,
-                                  p.in_scale, p.in_shift, p.in_act);
+        for (int h = 0; h < 2; ++h) sub_store<NSPLIT>(r[h], a + (size_t)h * WG_SUB_BYTES, a + (size_t)(2 + h) * WG_SUB_BYTES, warp, lane);
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(full_bar + stage));
@@ -412,32 +355,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
 // tile, slots 1.. = one unit of two gathered sub-tiles each; every producer thread arrives on the slot's "full" barrier
 // with cp.async.mbarrier.arrive.noinc (count = 32 lanes of the filling warp), so the hardware completes it when the last
 // copy has landed and the producers run a whole ring ahead of the MMA.
-struct WgradPlParams {
-  const uint16_t* in_hi;
-  const uint16_t* in_lo;
-  const uint16_t* g_hi;
-  const uint16_t* g_lo;
-  const int32_t* nbr;
-  float* dW;
-  int64_t n_out;
-  int64_t in_pitch, gout_pitch;   // row strides (bf16 elements)
-  int K, Cin, Cout;
-  int stages;
-  int units_per_pass, num_units, num_subs, passes, ctas_per_pass;
-  int uc, ncr;
-  float* part;
-  int64_t slot;
-};
-
-__device__ __forceinline__ void cp_async16_zfill(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-
 template <int NSPLIT>
-__global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_constant__ WgradPlParams p) {
+__global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_constant__ WgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int n_op = (NSPLIT == 3) ? 2 : 1;
@@ -592,8 +511,7 @@ int ctas_per_pass(int64_t num_rt, int passes) {
 }
 
 // unit geometry: uc columns per unit (the consumers' 128 accumulator columns hold 128 / uc units), ncr column ranges
-template <class P>
-void unit_plan(P& p, int K, int Cin, int Cout) {
+void unit_plan(WgradParams& p, int K, int Cin, int Cout) {
   p.uc = Cout <= ACC_COLS ? Cout : (Cout % ACC_COLS == 0 ? ACC_COLS : 64);
   p.ncr = Cout / p.uc;
   p.num_subs = K * (Cin / 64);
@@ -604,79 +522,34 @@ void unit_plan(P& p, int K, int Cin, int Cout) {
   p.units_per_pass = (p.num_units + p.passes - 1) / p.passes;
 }
 
-}  // namespace
-
-extern "C" int pasco_conv_wgrad_tc(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out,
-                                   int32_t Cin, int32_t Cout, const float* gout, const float* in_scale,
-                                   const float* in_shift, int32_t in_act, float* dW, int32_t precision,
-                                   int64_t in_pitch, int64_t gout_pitch, pasco_stream_t s) {
-  PASCO_CHECK_ARG(precision == 1 || precision == 3, "pasco_conv_wgrad_tc: precision must be 1 or 3");
+// The host half of both weight-gradient launches.  The caller sets the operands of p: fp32 rows in / gout (register
+// gather, k_wgrad_tc) or, when in_hi is set, their bf16 planes (plane gather, k_wgrad_pl), with row pitches (0 = Cin /
+// Cout).  The per-CTA partials are summed in a fixed order into dW through a stream-ordered workspace.
+int wgrad_launch(const char* fn, WgradParams& p, int64_t n_out, int32_t K, int32_t Cin, int32_t Cout, float* dW,
+                 int32_t precision, pasco_stream_t s) {
+  const bool planes = p.in_hi != nullptr;
+  PASCO_CHECK_ARG(precision == 1 || precision == 3, "%s: precision must be 1 or 3", fn);
   PASCO_CHECK_ARG(Cin % 64 == 0 && Cout % 64 == 0 && Cout <= 256,
-                  "pasco_conv_wgrad_tc: Cin (%d) and Cout (%d) must be multiples of 64, Cout <= 256", Cin, Cout);
-  (void)n_in;
+                  "%s: Cin (%d) and Cout (%d) must be multiples of 64, Cout <= 256", fn, Cin, Cout);
+  if (p.in_pitch <= 0) p.in_pitch = Cin;
+  if (p.gout_pitch <= 0) p.gout_pitch = Cout;
+  if (planes)
+    PASCO_CHECK_ARG(p.in_pitch % 8 == 0 && p.gout_pitch % 8 == 0 &&
+                    (((uintptr_t)p.in_hi | (uintptr_t)p.in_lo | (uintptr_t)p.g_hi | (uintptr_t)p.g_lo) & 15) == 0,
+                    "%s: planes must be 16-byte aligned with pitches multiple of 8 elements", fn);
   if (n_out == 0) return 0;
   int dev = 0, smem_optin = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  // shared memory: two gout tiles, the unit stages, barriers and, for k_wgrad_tc, its index ring and slot descriptors
   const int n_op = precision == 3 ? 2 : 1;
   const int g_bytes = n_op * (Cout / 64) * WG_SUB_BYTES;
   const int a_bytes = n_op * 2 * WG_SUB_BYTES;
-  const int fixed = 1024 + (2 * MAX_STAGES + 4) * 8 + IDX_RING * 2 * WG_R * 4 + 16 * 8 * 4;
+  const int fixed = 1024 + (2 * MAX_STAGES + 4) * 8 + (planes ? 0 : IDX_RING * 2 * WG_R * 4 + 16 * 8 * 4);
   int stages = (smem_optin - fixed - 2 * g_bytes) / a_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
-  PASCO_CHECK_ARG(stages >= 2, "pasco_conv_wgrad_tc: not enough shared memory");
-  WgradParams p;
-  p.in = in; p.nbr = nbr; p.gout = gout; p.in_scale = in_scale; p.in_shift = in_shift; p.dW = dW;
-  p.n_out = n_out; p.K = K; p.Cin = Cin; p.Cout = Cout; p.in_act = in_act;
-  p.in_pitch = in_pitch > 0 ? in_pitch : Cin;
-  p.gout_pitch = gout_pitch > 0 ? gout_pitch : Cout;
-  p.stages = stages;
-  unit_plan(p, K, Cin, Cout);
-  const int64_t num_rt = (n_out + WG_R - 1) / WG_R;
-  p.ctas_per_pass = ctas_per_pass(num_rt, p.passes);
-  const size_t smem = (size_t)2 * g_bytes + (size_t)stages * a_bytes + fixed;
-  cudaStream_t st = (cudaStream_t)s;
-  auto launch = [&](int grid) {
-    auto kern = precision == 3 ? k_wgrad_tc<3> : k_wgrad_tc<1>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) kern<<<grid, NUM_THREADS, smem, st>>>(p);
-    return e;
-  };
-  if (wgrad_launch(p, dW, st, "pasco_conv_wgrad_tc", launch) != 0) return -1;
-  PASCO_CHECK_LAUNCH("pasco_conv_wgrad_tc");
-  return 0;
-}
-
-extern "C" int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int64_t n_in, const int32_t* nbr, int32_t K,
-                                       int64_t n_out, int32_t Cin, int32_t Cout, const void* g_hi, const void* g_lo,
-                                       float* dW, int32_t precision, int64_t in_pitch, int64_t gout_pitch, pasco_stream_t s) {
-  PASCO_CHECK_ARG(precision == 1 || precision == 3, "pasco_conv_wgrad_planes: precision must be 1 or 3");
-  PASCO_CHECK_ARG(in_hi && g_hi && (precision == 1 || (in_lo && g_lo)), "pasco_conv_wgrad_planes: missing plane");
-  PASCO_CHECK_ARG(Cin % 64 == 0 && Cout % 64 == 0 && Cout <= 256,
-                  "pasco_conv_wgrad_planes: Cin (%d) and Cout (%d) must be multiples of 64, Cout <= 256", Cin, Cout);
-  (void)n_in;
-  if (n_out == 0) return 0;
-  int dev = 0, smem_optin = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  const int n_op = precision == 3 ? 2 : 1;
-  const int g_bytes = n_op * (Cout / 64) * WG_SUB_BYTES;
-  const int a_bytes = n_op * 2 * WG_SUB_BYTES;
-  const int fixed = 1024 + (2 * MAX_STAGES + 4) * 8;
-  int stages = (smem_optin - fixed - 2 * g_bytes) / a_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  PASCO_CHECK_ARG(stages >= 2, "pasco_conv_wgrad_planes: not enough shared memory");
-  WgradPlParams p;
-  p.in_hi = (const uint16_t*)in_hi; p.in_lo = (const uint16_t*)in_lo; p.g_hi = (const uint16_t*)g_hi; p.g_lo = (const uint16_t*)g_lo;
-  p.nbr = nbr; p.dW = dW;
-  p.n_out = n_out; p.K = K; p.Cin = Cin; p.Cout = Cout;
-  p.in_pitch = in_pitch > 0 ? in_pitch : Cin;
-  p.gout_pitch = gout_pitch > 0 ? gout_pitch : Cout;
-  PASCO_CHECK_ARG(p.in_pitch % 8 == 0 && p.gout_pitch % 8 == 0 &&
-                  (((uintptr_t)in_hi | (uintptr_t)in_lo | (uintptr_t)g_hi | (uintptr_t)g_lo) & 15) == 0,
-                  "pasco_conv_wgrad_planes: planes must be 16-byte aligned with pitches multiple of 8 elements");
-  // stages with a large divisor <= 7 (= the number of unit producer warps, see kernel)
-  {
+  PASCO_CHECK_ARG(stages >= 2, "%s: not enough shared memory", fn);
+  if (planes) {   // the stage count with the largest divisor <= 7 (= the number of unit producer warps, see k_wgrad_pl)
     int pick = stages, pick_w = 0;
     for (int st = stages; st >= 2; --st) {
       int w = 1;
@@ -686,19 +559,51 @@ extern "C" int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int
     }
     stages = pick;
   }
+  p.n_out = n_out; p.K = K; p.Cin = Cin; p.Cout = Cout;
   p.stages = stages;
   unit_plan(p, K, Cin, Cout);
-  const int64_t num_rt = (n_out + WG_R - 1) / WG_R;
-  p.ctas_per_pass = ctas_per_pass(num_rt, p.passes);
+  p.ctas_per_pass = ctas_per_pass((n_out + WG_R - 1) / WG_R, p.passes);
+  p.slot = (int64_t)p.units_per_pass * 128 * p.uc;
   const size_t smem = (size_t)2 * g_bytes + (size_t)stages * a_bytes + fixed;
-  cudaStream_t st = (cudaStream_t)s;
-  auto launch = [&](int grid) {
-    auto kern = precision == 3 ? k_wgrad_pl<3> : k_wgrad_pl<1>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) kern<<<grid, NUM_THREADS, smem, st>>>(p);
-    return e;
-  };
-  if (wgrad_launch(p, dW, st, "pasco_conv_wgrad_planes", launch) != 0) return -1;
-  PASCO_CHECK_LAUNCH("pasco_conv_wgrad_planes");
+  const int grid = p.passes * p.ctas_per_pass;
+  const cudaStream_t st = (cudaStream_t)s;
+  cudaError_t e = ws_alloc((void**)&p.part, (size_t)grid * p.slot * sizeof(float), st);
+  if (e != cudaSuccess) {
+    set_error("%s: workspace of %lld bytes: %s", fn, (long long)grid * p.slot * 4, cudaGetErrorString(e));
+    return -1;
+  }
+  void (*kern)(WgradParams) = planes ? (precision == 3 ? k_wgrad_pl<3> : k_wgrad_pl<1>)
+                                     : (precision == 3 ? k_wgrad_tc<3> : k_wgrad_tc<1>);
+  e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e == cudaSuccess) {
+    kern<<<grid, NUM_THREADS, smem, st>>>(p);
+    k_wgrad_sum<<<grid_for((int64_t)K * Cin * Cout, 256), 256, 0, st>>>(p, dW);
+  }
+  cudaFreeAsync(p.part, st);
+  if (e != cudaSuccess) {
+    set_error("%s: cudaFuncSetAttribute failed: %s", fn, cudaGetErrorString(e));
+    return -1;
+  }
+  PASCO_CHECK_LAUNCH(fn);
   return 0;
+}
+
+}  // namespace
+
+extern "C" int pasco_conv_wgrad_tc(const float* in, int64_t /*n_in*/, const int32_t* nbr, int32_t K, int64_t n_out,
+                                   int32_t Cin, int32_t Cout, const float* gout, float* dW, int32_t precision,
+                                   int64_t in_pitch, int64_t gout_pitch, pasco_stream_t s) {
+  WgradParams p = {};
+  p.in = in; p.gout = gout; p.nbr = nbr; p.in_pitch = in_pitch; p.gout_pitch = gout_pitch;
+  return wgrad_launch("pasco_conv_wgrad_tc", p, n_out, K, Cin, Cout, dW, precision, s);
+}
+
+extern "C" int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int64_t /*n_in*/, const int32_t* nbr, int32_t K,
+                                       int64_t n_out, int32_t Cin, int32_t Cout, const void* g_hi, const void* g_lo,
+                                       float* dW, int32_t precision, int64_t in_pitch, int64_t gout_pitch, pasco_stream_t s) {
+  PASCO_CHECK_ARG(in_hi && g_hi && (precision == 1 || (in_lo && g_lo)), "pasco_conv_wgrad_planes: missing plane");
+  WgradParams p = {};
+  p.in_hi = (const uint16_t*)in_hi; p.in_lo = (const uint16_t*)in_lo; p.g_hi = (const uint16_t*)g_hi; p.g_lo = (const uint16_t*)g_lo;
+  p.nbr = nbr; p.in_pitch = in_pitch; p.gout_pitch = gout_pitch;
+  return wgrad_launch("pasco_conv_wgrad_planes", p, n_out, K, Cin, Cout, dW, precision, s);
 }

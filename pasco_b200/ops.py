@@ -24,7 +24,6 @@ _PRECISION = 3          # 3 = bf16x3 split ("fp32" parity mode), 1 = plain bf16 
 _FORCE_SIMT = False     # validation switch: run every conv on the CUDA-core path
 _SIMT_KINDS = None      # validation switch: subset of {'fwd','dgrad','wgrad'} forced onto the CUDA-core path
 _SPLIT_K = True          # few-tile / many-offset convs (dense bottleneck) are split over the offsets
-_FUSE_BN_STATS = True    # forward convs leave their output's column statistics for the BatchNorm that follows
 _PENDING_STATS = None
 _USE_PLANES = True      # gathered convs (K > 1) read pre-split bf16 planes with zero-fill cp.async copies (k_conv_pl /
                         # k_wgrad_pl); False = the round-1 register-gather kernels (kept for cross-checks)
@@ -365,25 +364,33 @@ def split_planes(x: torch.Tensor, scale=None, shift=None, act: int = 0):
     return hi, lo
 
 
-def _planes_ok(c_contract: int, kk: int, nbr) -> bool:
-    return _USE_PLANES and nbr is not None and kk > 1 and c_contract % 64 == 0
-
-
-def _tc_ok(c_contract: int, c_out: int, K: int, kind: str = "fwd") -> bool:
-    if _SIMT_KINDS is not None and kind in _SIMT_KINDS:
-        return False
-    return (not _FORCE_SIMT) and c_contract % 64 == 0 and c_out % 16 == 0 and 16 <= c_out <= 256 and K <= 1024
+def conv_path(kind: str, c_contract: int, c_out: int, K: int, nbr, n_rows: int) -> str:
+    """The kernels one convolution launch runs on: 'planes' (pasco_conv_forward_planes / pasco_conv_wgrad_planes),
+    'splitk' (pasco_conv_forward_splitk), 'regs' (pasco_conv_forward_tc / pasco_conv_wgrad_tc) or 'simt' (CUDA cores).
+    kind 'fwd' / 'dgrad': c_contract gathered channels → c_out channels of n_rows output rows through K offsets of the
+    neighbour table nbr (None: identity rows); 'wgrad': c_contract = Cin, c_out = Cout (never split, n_rows unused)."""
+    if _FORCE_SIMT or (_SIMT_KINDS is not None and kind in _SIMT_KINDS) or c_contract % 64:
+        return "simt"
+    if kind == "wgrad":
+        if c_out % 64 or c_out > 256:
+            return "simt"
+    elif c_out % 16 or not 16 <= c_out <= 256 or K > 1024:
+        return "simt"
+    elif _SPLIT_K and load().pasco_conv_splitk_workspace_bytes(K, n_rows, c_out) > 0:
+        return "splitk"
+    return "planes" if _USE_PLANES and nbr is not None and K > 1 else "regs"
 
 
 def conv_apply(feats: torch.Tensor, weight: torch.Tensor, nbr: Optional[torch.Tensor], n_out: int,
                transpose_w: bool, koff: Optional[Sequence[int]], bias: Optional[torch.Tensor] = None,
-               in_scale=None, in_shift=None, in_act: int = 0, packs: Optional[PackedWeights] = None,
-               want_stats: bool = False, planes=None, planes_out: Optional[list] = None) -> torch.Tensor:
-    """out[o] = Σ_k act(feats·scale+shift)[nbr[k,o]] @ Wk, Wk = W[koff[k]] (transposed when transpose_w).
+               packs: Optional[PackedWeights] = None, want_stats: bool = False, planes=None,
+               planes_out: Optional[list] = None) -> torch.Tensor:
+    """out[o] = Σ_k feats[nbr[k,o]] @ Wk, Wk = W[koff[k]] (transposed when transpose_w).
     want_stats: the kernel's epilogue also accumulates the column sums / sums of squares of `out` (the training-mode
     BatchNorm statistics of the layer that follows) and leaves them for BatchNormAct (see take_pending_stats).
-    planes: (hi, lo) bf16 planes of act(feats·scale+shift) if the caller already has them; planes_out: a list that
-    receives the planes this call made (the backward pass reuses them for the weight gradient)."""
+    planes: (hi, lo) bf16 planes of the gathered rows if the caller already has them (BNActConv passes the planes of
+    act(BN(x))); planes_out: a list that receives the planes this call made (the backward pass reuses them for the
+    weight gradient)."""
     K, Cin, Cout = weight.shape
     c_contract, c_out = (Cout, Cin) if transpose_w else (Cin, Cout)
     assert feats.shape[1] == c_contract
@@ -397,40 +404,28 @@ def conv_apply(feats: torch.Tensor, weight: torch.Tensor, nbr: Optional[torch.Te
         ev0.record()
     global _PENDING_STATS
     _PENDING_STATS = None            # statistics of an earlier launch never survive another convolution
-    use_tc = _tc_ok(c_contract, c_out, kk, "dgrad" if transpose_w else "fwd")
-    split_k = use_tc and _SPLIT_K and load().pasco_conv_splitk_workspace_bytes(kk, n_out, c_out) > 0
-    path = "simt"
-    if use_tc and not split_k and _planes_ok(c_contract, kk, nbr):
-        path = "planes"
-        hi, lo = planes if planes is not None else split_planes(feats, in_scale, in_shift, in_act)
+    path = conv_path("dgrad" if transpose_w else "fwd", c_contract, c_out, kk, nbr, n_out)
+    stats = None
+    if want_stats and path in ("planes", "regs") and n_out >= 4096:
+        stats = torch.zeros(2, c_out, dtype=torch.float64, device=feats.device)
+    if path == "planes":
+        hi, lo = planes if planes is not None else split_planes(feats)
         if planes_out is not None:
             planes_out.append((hi, lo))
-        stats = None
-        if want_stats and _FUSE_BN_STATS and n_out >= 4096:
-            stats = torch.zeros(2, c_out, dtype=torch.float64, device=feats.device)
         call("pasco_conv_forward_planes", ptr(hi), ptr(lo), feats.shape[0], ptr(nbr), kk, n_out, c_contract, c_out,
              ptr((packs or PackedWeights()).get(weight, transpose_w)), koff_arr, ptr(bias), ptr(stats), ptr(out),
              _PRECISION, 0, 0)
-        if stats is not None:
-            _PENDING_STATS = (weakref.ref(out), out.data_ptr(), out._version, tuple(out.shape), stats)
-    elif use_tc and _SPLIT_K and (ws_bytes := load().pasco_conv_splitk_workspace_bytes(kk, n_out, c_out)) > 0:
-        path = "splitk"
+    elif path == "splitk":
+        ws_bytes = load().pasco_conv_splitk_workspace_bytes(kk, n_out, c_out)
         ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=feats.device)
         call("pasco_conv_forward_splitk", ptr(feats), feats.shape[0], ptr(nbr), kk, n_out, c_contract, c_out,
-             ptr((packs or PackedWeights()).get(weight, transpose_w)), koff_arr, ptr(bias), ptr(in_scale), ptr(in_shift), in_act,
-             ptr(out), _PRECISION, 0, 0, ptr(ws), ws_bytes)
-    elif use_tc:
-        path = "regs"
-        stats = None
-        if want_stats and _FUSE_BN_STATS and n_out >= 4096:
-            stats = torch.zeros(2, c_out, dtype=torch.float64, device=feats.device)
+             ptr((packs or PackedWeights()).get(weight, transpose_w)), koff_arr, ptr(bias), ptr(out), _PRECISION, 0, 0,
+             ptr(ws), ws_bytes)
+    elif path == "regs":
         call("pasco_conv_forward_tc", ptr(feats), feats.shape[0], ptr(nbr), kk, n_out, c_contract, c_out,
-             ptr((packs or PackedWeights()).get(weight, transpose_w)), koff_arr, ptr(bias), ptr(in_scale), ptr(in_shift), in_act,
-             ptr(stats), ptr(out), _PRECISION, 0, 0)
-        if stats is not None:
-            _PENDING_STATS = (weakref.ref(out), out.data_ptr(), out._version, tuple(out.shape), stats)
+             ptr((packs or PackedWeights()).get(weight, transpose_w)), koff_arr, ptr(bias), ptr(stats), ptr(out),
+             _PRECISION, 0, 0)
     else:
-        assert in_scale is None and in_act == 0, "fused prologue needs the tensor-core path"
         if nbr is None:
             nbr = torch.arange(n_out, dtype=torch.int32, device=feats.device).view(1, -1)
         call("pasco_conv_forward_simt", ptr(feats), ptr(nbr), kk, n_out, c_contract, c_out,
@@ -441,7 +436,9 @@ def conv_apply(feats: torch.Tensor, weight: torch.Tensor, nbr: Optional[torch.Te
         prof.append(("dgrad" if transpose_w else "fwd", ev0, ev1,
                      dict(n_in=feats.shape[0], n_out=n_out, K=kk, Cin=c_contract, Cout=c_out,
                           pairs=PAIR_COUNTS.get(nbr.data_ptr()) if nbr is not None else None,
-                          tc=use_tc, precision=_PRECISION, path=path)))
+                          tc=path != "simt", precision=_PRECISION, path=path)))
+    if stats is not None:
+        _PENDING_STATS = (weakref.ref(out), out.data_ptr(), out._version, tuple(out.shape), stats)
     return out
 
 
@@ -465,15 +462,10 @@ def split_k(flag: bool) -> None:
     _SPLIT_K = bool(flag)
 
 
-def fuse_bn_stats(flag: bool) -> None:
-    global _FUSE_BN_STATS
-    _FUSE_BN_STATS = bool(flag)
-
-
 def conv_wgrad(feats: torch.Tensor, gout: torch.Tensor, nbr: Optional[torch.Tensor], K: int, Cin: int, Cout: int,
-               in_scale=None, in_shift=None, in_act: int = 0, in_planes=None, g_planes=None) -> torch.Tensor:
-    """in_planes / g_planes: (hi, lo) bf16 planes of act(feats·scale+shift) and of gout when the caller has them
-    (the forward pass made the former, the input-gradient launch of the same backward the latter)."""
+               in_planes=None, g_planes=None) -> torch.Tensor:
+    """in_planes / g_planes: (hi, lo) bf16 planes of the gathered rows and of gout when the caller has them (the forward
+    pass made the former, the backward pass splits the latter once for the input and the weight gradient)."""
     n_out = gout.shape[0]
     dW = torch.zeros(K, Cin, Cout, dtype=torch.float32, device=feats.device)
     feats, gout = feats.contiguous(), gout.contiguous()
@@ -481,18 +473,16 @@ def conv_wgrad(feats: torch.Tensor, gout: torch.Tensor, nbr: Optional[torch.Tens
     if prof is not None:
         ev0 = torch.cuda.Event(enable_timing=True)
         ev0.record()
-    tc = _tc_ok(Cin, 64, 1, "wgrad") and Cin % 64 == 0 and Cout % 64 == 0 and Cout <= 256
-    path = "planes" if tc and _planes_ok(Cin, K, nbr) else ("regs" if tc else "simt")
-    if tc and _planes_ok(Cin, K, nbr):
-        ih, il = in_planes if in_planes is not None else split_planes(feats, in_scale, in_shift, in_act)
+    path = conv_path("wgrad", Cin, Cout, K, nbr, n_out)
+    if path == "planes":
+        ih, il = in_planes if in_planes is not None else split_planes(feats)
         gh, gl = g_planes if g_planes is not None else split_planes(gout)
         call("pasco_conv_wgrad_planes", ptr(ih), ptr(il), feats.shape[0], ptr(nbr), K, n_out, Cin, Cout, ptr(gh), ptr(gl),
              ptr(dW), _PRECISION, 0, 0)
-    elif tc:
-        call("pasco_conv_wgrad_tc", ptr(feats), feats.shape[0], ptr(nbr), K, n_out, Cin, Cout, ptr(gout),
-             ptr(in_scale), ptr(in_shift), in_act, ptr(dW), _PRECISION, 0, 0)
+    elif path == "regs":
+        call("pasco_conv_wgrad_tc", ptr(feats), feats.shape[0], ptr(nbr), K, n_out, Cin, Cout, ptr(gout), ptr(dW),
+             _PRECISION, 0, 0)
     else:
-        assert in_scale is None and in_act == 0
         if nbr is None:
             nbr = torch.arange(n_out, dtype=torch.int32, device=feats.device).view(1, -1)
         call("pasco_conv_wgrad_simt", ptr(feats), ptr(nbr), K, n_out, Cin, Cout, ptr(gout), ptr(dW))
@@ -501,7 +491,7 @@ def conv_wgrad(feats: torch.Tensor, gout: torch.Tensor, nbr: Optional[torch.Tens
         ev1.record()
         prof.append(("wgrad", ev0, ev1, dict(n_in=feats.shape[0], n_out=n_out, K=K, Cin=Cin, Cout=Cout,
                                              pairs=PAIR_COUNTS.get(nbr.data_ptr()) if nbr is not None else None,
-                                             tc=tc, precision=_PRECISION, path=path)))
+                                             tc=path != "simt", precision=_PRECISION, path=path)))
     return dW
 
 
@@ -538,8 +528,8 @@ class SparseConv(torch.autograd.Function):
         gin = gw = gb = None
         K, Cin, Cout = weight.shape
         g_planes = None
-        if _planes_ok(Cout, K, kmap.nbr) and _tc_ok(Cout, Cin, K, "dgrad") and \
-                (ctx.needs_input_grad[0] and ctx.needs_input_grad[1]):
+        if ctx.needs_input_grad[0] and ctx.needs_input_grad[1] and "planes" in (
+                conv_path("dgrad", Cout, Cin, K, kmap.nbr, kmap.n_in), conv_path("wgrad", Cin, Cout, K, kmap.nbr, kmap.n_out)):
             g_planes = split_planes(g)          # one split of the output gradient serves dgrad (gather) and wgrad (B operand)
         if ctx.needs_input_grad[0]:
             nbr_t, koff_t = kmap.transposed()
@@ -720,11 +710,10 @@ def bn_act_conv(bn, x: torch.Tensor, act: int, group, weight, bias, kmap: "Kerne
     """conv(act(BatchNorm(x))) — fused (BNActConv) when the layer runs on the plane-gather tensor-core path in training
     mode, the two separate nodes otherwise."""
     K, Cin, Cout = weight.shape
-    fused = (bn.training and bn.running_mean is not None and x.is_cuda and _planes_ok(Cin, kmap.K, kmap.nbr)
-             and _tc_ok(Cin, Cout, kmap.K, "fwd") and _tc_ok(Cout, Cin, kmap.K, "dgrad") and _tc_ok(Cin, 64, 1, "wgrad")
-             and Cout % 64 == 0 and Cout <= 256
-             and not (_SPLIT_K and load().pasco_conv_splitk_workspace_bytes(kmap.K, kmap.n_out, Cout) > 0)
-             and not (_SPLIT_K and load().pasco_conv_splitk_workspace_bytes(kmap.K, kmap.n_in, Cin) > 0))
+    fused = (bn.training and bn.running_mean is not None and x.is_cuda
+             and conv_path("fwd", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) == "planes"
+             and conv_path("dgrad", Cout, Cin, kmap.K, kmap.nbr, kmap.n_in) == "planes"
+             and conv_path("wgrad", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) == "planes")
     if not fused:
         return SparseConv.apply(batchnorm_rows(bn, x, act, group), weight, bias, kmap, packs)
     with torch.no_grad():
@@ -844,8 +833,8 @@ def _gemm_rows(x: torch.Tensor, w_nk: torch.Tensor, bias: Optional[torch.Tensor]
         wchunk = w_nk[c0:c0 + cw].contiguous()                       # [cw, K]  == ME layout [1, Cin'=cw, Cout'=K]
         packed = PackedWeights().get(wchunk.view(1, cw, kdim), True)  # B[n][k] = w[n][k]
         b = bias[c0:c0 + cw].contiguous() if bias is not None else None
-        call("pasco_conv_forward_tc", ptr(x), n_rows, None, 1, n_rows, kdim, cw, ptr(packed), None, ptr(b), None, None, 0,
-             None, C.c_void_p(_data_ptr_at(out, c0)), _PRECISION, 0, N)
+        call("pasco_conv_forward_tc", ptr(x), n_rows, None, 1, n_rows, kdim, cw, ptr(packed), None, ptr(b), None,
+             C.c_void_p(_data_ptr_at(out, c0)), _PRECISION, 0, N)
 
 
 class LinearTC(torch.autograd.Function):
@@ -876,7 +865,7 @@ class LinearTC(torch.autograd.Function):
                 cw = min(256, cin - c0)
                 dw = torch.zeros(1, cout, cw, dtype=torch.float32, device=x.device)
                 call("pasco_conv_wgrad_tc", ptr(gy), gy.shape[0], None, 1, gy.shape[0], cout, cw,
-                     C.c_void_p(_data_ptr_at(x, c0)), None, None, 0, ptr(dw), _PRECISION, 0, cin)
+                     C.c_void_p(_data_ptr_at(x, c0)), ptr(dw), _PRECISION, 0, cin)
                 gw[:, c0:c0 + cw] = dw[0]
         if ctx.has_bias and ctx.needs_input_grad[2]:
             gb = gy.sum(0)
