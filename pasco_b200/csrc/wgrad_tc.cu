@@ -23,7 +23,8 @@ constexpr int NUM_THREADS = (CONS_WARP0 + NUM_CONS_WARPS) * 32;   // 512
 constexpr int ACC_COLS = 128;                        // accumulator columns per consumer thread set (64 registers)
 constexpr int WROWS = 64 / NUM_GATHER_WARPS;         // rows of a 64-row tile per gather warp
 constexpr int WLOADS = WROWS / 2;                    // float4 loads per lane per sub-tile
-constexpr int MAX_STAGES = 8;
+constexpr int MAX_STAGES = 8;             // unit (A) ring
+constexpr int MAX_GSTAGES = 4;            // gout ring
 constexpr int WG_R = 64;                  // voxel rows per tile (contraction block)
 constexpr int WG_SUB_BYTES = WG_R * 128;  // one [64 rows][64 ch] bf16 tile = 8 KB
 
@@ -38,7 +39,8 @@ struct WgradParams {
   int64_t n_out;
   int64_t in_pitch, gout_pitch;   // row strides (floats, or elements of the planes)
   int K, Cin, Cout;
-  int stages;
+  int stages, gstages;            // depths of the unit ring and of the gout ring
+  int gblocks;                    // 64-column blocks of gout per gout tile (see gout_block)
   int units_per_pass, num_units, num_subs, passes, ctas_per_pass;
   int uc, ncr;                    // columns per unit, column ranges (unit u = sub-tile pair u / ncr, columns of range u % ncr)
   float* part;                    // [grid][slot]: partial dW of CTA b = cta_in_pass * passes + pass
@@ -83,64 +85,108 @@ __device__ __forceinline__ void sub_store(const SubRegs& r, uint8_t* dst_hi, uin
   }
 }
 
+// The gout tile of a row tile holds only the 64-column blocks of gout that the CTA's units read, hi blocks then lo
+// blocks: with uc = 128 (one unit per pass) the unit's two blocks, with uc = 64 the block of each unit (one block when
+// Cout = 64, where both units share it).  Block b of the tile is gout column block gout_block(p, unit0, b).
+__device__ __forceinline__ int gout_block(const WgradParams& p, int unit0, int b) {
+  return p.uc == 128 ? (unit0 % p.ncr) * 2 + b : (unit0 + b) % p.ncr;
+}
+// 64-column blocks of gout one CTA copies per row tile (at most gblocks)
+__device__ __forceinline__ int gout_nblocks(const WgradParams& p, int nunits) {
+  return p.uc == 128 ? 2 : (p.ncr > 1 ? nunits : 1);
+}
+
 // Consumer warpgroup hh (0 / 1) accumulates sub-tile hh of every unit of the CTA's pass: acc[q] holds columns
-// [64 q, 64 q + 64) of the pass's accumulator, i.e. column block q % (uc / 64) of unit q / (uc / 64).  Every consumer
+// [64 q, 64 q + 64) of the pass's accumulator, i.e. column block q % (UC / 64) of unit q / (UC / 64).  Every consumer
 // warp arrives on the ring "empty" barriers (expected count 8).  After the CTA's last row tile it stores its partial dW
 // into its workspace slot: row (u * 128 + 64 hh + channel), column within the unit.
-template <int NSPLIT, bool CPASYNC>
+// Retire: one wgmma group stays in flight, as in the convolution consumer.  After committing slot n the warpgroup waits
+// for slot n - 1 (wait_group 1) and only then releases slot n - 1's A stage, and the row tile's gout buffer when slot
+// n - 1 was the tile's last unit.  The last slot is drained (wait_group 0) before the partial dW is stored.  Each slot's
+// MMA chain and its commit sit in one basic block (else ptxas commits an empty group and the wait drains the real MMAs).
+template <int NSPLIT, bool CPASYNC, int UC>
 __device__ __forceinline__ void wgrad_consumer(const WgradParams& p, const uint8_t* g_smem, const uint8_t* a_smem, int g_bytes, int a_bytes,
                                                uint64_t* full_bar, uint64_t* empty_bar, uint64_t* gfull_bar, uint64_t* gempty_bar,
                                                int unit0, int nunits, int cta_in_pass, int64_t num_rt, int hh, int wq, int lane) {
-  const int NB = p.Cout / 64, UNB = p.uc / 64, CB = p.Cin / 64;
+  constexpr int UNB = UC / 64;
   float acc[2][32];
 #pragma unroll
   for (int q = 0; q < 2; ++q)
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
-  int stage = 0;
-  uint32_t phase = 0;
-  int git = 0;
-  for (int64_t rt = cta_in_pass; rt < num_rt; rt += p.ctas_per_pass, ++git) {
-    const int gb = git & 1;
-    mbar_wait(smem_u32(gfull_bar + gb), (git >> 1) & 1);
+  int stage = 0, gb = 0;
+  uint32_t phase = 0, gphase = 0;
+  int held = -1, held_g = -1;     // A stage and gout buffer of the slot whose MMAs may still be in flight (-1: none)
+  auto release_held = [&]() {
+    __syncwarp();
+    if (lane == 0) {
+      if (held >= 0) mbar_arrive(smem_u32(empty_bar + held));
+      if (held_g >= 0) mbar_arrive(smem_u32(gempty_bar + held_g));
+    }
+    held = held_g = -1;
+  };
+  const uint32_t g_lo_off = p.gblocks * WG_SUB_BYTES;
+  for (int64_t rt = cta_in_pass; rt < num_rt; rt += p.ctas_per_pass) {
+    mbar_wait(smem_u32(gfull_bar + gb), gphase);
     if (CPASYNC) fence_proxy_async_smem();     // tiles were written by cp.async copies (generic proxy)
     const uint32_t g_hi = smem_u32(g_smem + (size_t)gb * g_bytes);
-    const uint32_t g_lo_off = NB * WG_SUB_BYTES;
     for (int u = 0; u < nunits; ++u) {
       mbar_wait(smem_u32(full_bar + stage), phase);
       if (CPASYNC) fence_proxy_async_smem();
       const uint32_t a_hi = smem_u32(a_smem + (size_t)stage * a_bytes) + (uint32_t)hh * WG_SUB_BYTES;
       const uint32_t a_lo = a_hi + 2 * WG_SUB_BYTES;
       const uint64_t da_hi = make_desc_sw128(a_hi, WG_SUB_BYTES, 1024), da_lo = make_desc_sw128(a_lo, WG_SUB_BYTES, 1024);
-      const int nb0 = ((unit0 + u) % p.ncr) * UNB;   // first 64-column block of gout that the unit covers
+      // the unit's first block in the gout tile: uc = 128 reads blocks 0-1, uc = 64 the block of unit u
+      const uint32_t b = g_hi + (uint32_t)(UC == 128 || p.ncr == 1 ? 0 : u) * WG_SUB_BYTES;
+      const uint64_t db_hi = make_desc_sw128(b, WG_SUB_BYTES, 1024), db_lo = make_desc_sw128(b + g_lo_off, WG_SUB_BYTES, 1024);
+      // k-step j (16 rows = 2048 bytes = 128 address units); every column adds hi·hi, lo·hi, hi·lo for j = 0, 1, ...
+      auto mma_chain = [&](auto& a) {
+#pragma unroll
+        for (int j = 0; j < WG_R / 16; ++j) {
+          if constexpr (UC == 128) {     // one MMA spans the unit's two gout blocks (LBO = the block distance)
+            wgmma_n128<1, 1>(a, da_hi + 128 * j, db_hi + 128 * j);
+            if (NSPLIT == 3) {
+              wgmma_n128<1, 1>(a, da_lo + 128 * j, db_hi + 128 * j);
+              wgmma_n128<1, 1>(a, da_hi + 128 * j, db_lo + 128 * j);
+            }
+          } else {
+            wgmma_n64<1, 1>(a, da_hi + 128 * j, db_hi + 128 * j);
+            if (NSPLIT == 3) {
+              wgmma_n64<1, 1>(a, da_lo + 128 * j, db_hi + 128 * j);
+              wgmma_n64<1, 1>(a, da_hi + 128 * j, db_lo + 128 * j);
+            }
+          }
+        }
+      };
       wg_fence();
+      if constexpr (UC == 128) {           // one unit per pass: the chain is unconditional
+        mma_chain(reinterpret_cast<float(&)[64]>(acc));
+        wg_commit();
+      } else {                             // unit u accumulates into acc[u]: each chain is committed in its own branch
 #pragma unroll
-      for (int q = 0; q < 2; ++q) {
-        if (q / UNB != u) continue;
-        const uint32_t b = g_hi + (uint32_t)(nb0 + q % UNB) * WG_SUB_BYTES;
-        const uint64_t db_hi = make_desc_sw128(b, WG_SUB_BYTES, 1024), db_lo = make_desc_sw128(b + g_lo_off, WG_SUB_BYTES, 1024);
-#pragma unroll
-        for (int j = 0; j < WG_R / 16; ++j) {          // 16 rows = 2048 bytes = 128 address units per k-step
-          wgmma_n64<1, 1>(acc[q], da_hi + 128 * j, db_hi + 128 * j);
-          if (NSPLIT == 3) {
-            wgmma_n64<1, 1>(acc[q], da_lo + 128 * j, db_hi + 128 * j);
-            wgmma_n64<1, 1>(acc[q], da_hi + 128 * j, db_lo + 128 * j);
+        for (int q = 0; q < 2; ++q) {
+          if (q == u) {
+            mma_chain(acc[q]);
+            wg_commit();
           }
         }
       }
-      wg_commit();
-      wg_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(empty_bar + stage));
+      wg_wait<1>();                        // the previous slot's MMAs are complete
+      release_held();
+      held = stage;
+      held_g = u == nunits - 1 ? gb : -1;  // the gout buffer is free after the row tile's last unit
       if (++stage == p.stages) {
         stage = 0;
         phase ^= 1;
       }
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(gempty_bar + gb));
+    if (++gb == p.gstages) {
+      gb = 0;
+      gphase ^= 1;
+    }
   }
-  (void)CB;
+  wg_wait<0>();
+  release_held();
   float* slot = p.part + (int64_t)blockIdx.x * p.slot;
 #pragma unroll
   for (int q = 0; q < 2; ++q) {
@@ -150,9 +196,26 @@ __device__ __forceinline__ void wgrad_consumer(const WgradParams& p, const uint8
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const int ch = frag_row(i, wq, lane), col = col0 + frag_col(i, lane);
-      *reinterpret_cast<float2*>(slot + (int64_t)(u * 128 + hh * 64 + ch) * p.uc + col) = make_float2(acc[q][i], acc[q][i + 1]);
+      *reinterpret_cast<float2*>(slot + (int64_t)(u * 128 + hh * 64 + ch) * UC + col) = make_float2(acc[q][i], acc[q][i + 1]);
     }
   }
+}
+
+template <int NSPLIT, bool CPASYNC>
+__device__ __forceinline__ void run_wgrad_consumer(const WgradParams& p, const uint8_t* g_smem, const uint8_t* a_smem, int g_bytes,
+                                                   int a_bytes, uint64_t* bars, int unit0, int nunits, int cta_in_pass,
+                                                   int64_t num_rt, int warp, int lane) {
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + MAX_STAGES;
+  uint64_t* gfull_bar = bars + 2 * MAX_STAGES;
+  uint64_t* gempty_bar = bars + 2 * MAX_STAGES + MAX_GSTAGES;
+  const int hh = (warp - CONS_WARP0) >> 2, wq = (warp - CONS_WARP0) & 3;
+  if (p.uc == 128)
+    wgrad_consumer<NSPLIT, CPASYNC, 128>(p, g_smem, a_smem, g_bytes, a_bytes, full_bar, empty_bar, gfull_bar, gempty_bar,
+                                         unit0, nunits, cta_in_pass, num_rt, hh, wq, lane);
+  else
+    wgrad_consumer<NSPLIT, CPASYNC, 64>(p, g_smem, a_smem, g_bytes, a_bytes, full_bar, empty_bar, gfull_bar, gempty_bar,
+                                        unit0, nunits, cta_in_pass, num_rt, hh, wq, lane);
 }
 
 // dW[k][ci][co] += Σ_c part[c * passes + pass][...] over the CTAs c of the pass that owns (k, ci, co), in CTA order
@@ -178,16 +241,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int n_op = (NSPLIT == 3) ? 2 : 1;
-  const int NB = p.Cout / 64;                    // 64-column blocks of gout
-  const int g_bytes = n_op * NB * WG_SUB_BYTES;  // one gout tile (hi [+ lo])
-  const int a_bytes = n_op * 2 * WG_SUB_BYTES;   // one stage: two sub-tiles (hi [+ lo])
-  uint8_t* g_smem = smem;                        // [2][g_bytes]
-  uint8_t* a_smem = smem + 2 * (size_t)g_bytes;  // [stages][a_bytes]
+  const int g_bytes = n_op * p.gblocks * WG_SUB_BYTES;   // one gout tile (hi blocks [+ lo blocks])
+  const int a_bytes = n_op * 2 * WG_SUB_BYTES;           // one stage: two sub-tiles (hi [+ lo])
+  uint8_t* g_smem = smem;                                // [gstages][g_bytes]
+  uint8_t* a_smem = smem + (size_t)p.gstages * g_bytes;  // [stages][a_bytes]
   uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + (size_t)p.stages * a_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + MAX_STAGES;
-  uint64_t* gfull_bar = bars + 2 * MAX_STAGES;       // [2]
-  uint64_t* gempty_bar = bars + 2 * MAX_STAGES + 2;  // [2]
+  uint64_t* gfull_bar = bars + 2 * MAX_STAGES;
+  uint64_t* gempty_bar = bars + 2 * MAX_STAGES + MAX_GSTAGES;
 
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
   const int CB = p.Cin / 64;
@@ -202,7 +264,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
       mbar_init(smem_u32(full_bar + s), NUM_GATHER_WARPS);
       mbar_init(smem_u32(empty_bar + s), NUM_CONS_WARPS);
     }
-    for (int b = 0; b < 2; ++b) {
+    for (int b = 0; b < p.gstages; ++b) {
       mbar_init(smem_u32(gfull_bar + b), NUM_GATHER_WARPS);
       mbar_init(smem_u32(gempty_bar + b), NUM_CONS_WARPS);
     }
@@ -210,18 +272,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
   }
   // slot descriptor table: [j][0]=type (0 gout, 1 unit), [1],[2]=column bases of the two sub-tiles (-1 = none),
   // [3],[4]=kernel offset of the two sub-tiles (-1 = padding)
-  int* idx_ring = reinterpret_cast<int*>(bars + 2 * MAX_STAGES + 4);   // [IDX_RING][2][WG_R]
-  int* desc = idx_ring + IDX_RING * 2 * WG_R;                        // [<=16][8]
+  int* idx_ring = reinterpret_cast<int*>(bars + 2 * (MAX_STAGES + MAX_GSTAGES));   // [IDX_RING][2][WG_R]
+  int* desc = idx_ring + IDX_RING * 2 * WG_R;                                    // [<=16][8]
   {
-    const int GSd = (NB + 1) / 2;
-    for (int j = threadIdx.x; j < GSd + nunits; j += NUM_THREADS) {
+    for (int j = threadIdx.x; j < 1 + nunits; j += NUM_THREADS) {
       int* dj = desc + j * 8;
-      if (j < GSd) {
-        dj[0] = 0; dj[1] = j * 2 * 64; dj[2] = (j * 2 + 1 < NB) ? (j * 2 + 1) * 64 : -1; dj[3] = -1; dj[4] = -1;
+      if (j == 0) {                          // the gout slot: the tile's one or two column blocks
+        dj[0] = 0; dj[1] = gout_block(p, unit0, 0) * 64;
+        dj[2] = gout_nblocks(p, nunits) > 1 ? gout_block(p, unit0, 1) * 64 : -1; dj[3] = -1; dj[4] = -1;
       } else {
         dj[0] = 1;
         for (int h = 0; h < 2; ++h) {
-          const int sub = ((unit0 + (j - GSd)) / p.ncr) * 2 + h;
+          const int sub = ((unit0 + (j - 1)) / p.ncr) * 2 + h;
           const bool ok = sub < p.num_subs;
           dj[1 + h] = ok ? (sub % CB) * 64 : 0;
           dj[3 + h] = ok ? sub / CB : -1;
@@ -230,12 +292,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
     }
   }
   __syncthreads();
-  const int GS = (NB + 1) / 2;
-  const int spr = GS + nunits;               // slots per row tile
+  const int spr = 1 + nunits;               // slots per row tile
 
   if (warp < NUM_GATHER_WARPS) {
-    // Flat slot sequence per row tile:  GS gout slots (two 64-column blocks each), then one slot per unit (two
-    // gathered sub-tiles).  Every slot = 2 x WLOADS float4 loads per lane; the loads of slot s+1 are in flight in
+    // Flat slot sequence per row tile:  one gout slot (the tile's one or two 64-column blocks), then one slot per unit
+    // (two gathered sub-tiles).  Every slot = 2 x WLOADS float4 loads per lane; the loads of slot s+1 are in flight in
     // registers while slot s is converted and stored; neighbour indices arrive through a cp.async ring PF_DIST slots
     // ahead.  Slot geometry comes from a small descriptor table in shared memory (no divisions in the loop).
     const int my_r = warp * WROWS + (lane & (WROWS - 1));          // this lane's row inside the 64-row tile
@@ -271,21 +332,22 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
         }
       }
     };
-    int stage = 0;
-    uint32_t phase = 0;
-    auto store = [&](int j, int git, SubRegs (&r)[2]) {
+    int stage = 0, gb = 0;
+    uint32_t phase = 0, gphase = 0;
+    auto store = [&](int j, SubRegs (&r)[2]) {
       const int* dj = desc + j * 8;
       if (dj[0] == 0) {
-        const int gb = git & 1;
-        if (j == 0) mbar_wait(smem_u32(gempty_bar + gb), ((git >> 1) & 1) ^ 1);
+        mbar_wait(smem_u32(gempty_bar + gb), gphase ^ 1);
         uint8_t* g = g_smem + (size_t)gb * g_bytes;
-        const int nb = j * 2;
-        sub_store<NSPLIT>(r[0], g + (size_t)nb * WG_SUB_BYTES, g + (size_t)(NB + nb) * WG_SUB_BYTES, warp, lane);
-        if (dj[2] >= 0) sub_store<NSPLIT>(r[1], g + (size_t)(nb + 1) * WG_SUB_BYTES, g + (size_t)(NB + nb + 1) * WG_SUB_BYTES, warp, lane);
-        if (j == GS - 1) {
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(gfull_bar + gb));
+        const int GB = p.gblocks;
+        sub_store<NSPLIT>(r[0], g, g + (size_t)GB * WG_SUB_BYTES, warp, lane);
+        if (dj[2] >= 0) sub_store<NSPLIT>(r[1], g + WG_SUB_BYTES, g + (size_t)(GB + 1) * WG_SUB_BYTES, warp, lane);
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(gfull_bar + gb));
+        if (++gb == p.gstages) {
+          gb = 0;
+          gphase ^= 1;
         }
       } else {
         mbar_wait(smem_u32(empty_bar + stage), phase ^ 1);
@@ -304,7 +366,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
 
     // three cursors over the same slot sequence: prefetch (PF_DIST ahead), load, store
     int64_t p_rt = cta_in_pass, l_rt = cta_in_pass, s_rt = cta_in_pass;
-    int p_j = 0, l_j = 0, s_j = 0, p_g = 0, l_g = 0, s_git = 0;
+    int p_j = 0, l_j = 0, s_j = 0, p_g = 0, l_g = 0;
 #define WG_ADV(rt, j) do { if (++(j) == spr) { (j) = 0; (rt) += stride_rt; } } while (0)
     if (l_rt < num_rt) {
       for (int a = 0; a < PF_DIST; ++a) {
@@ -322,11 +384,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
         WG_ADV(l_rt, l_j);
       };
       auto store_next = [&](SubRegs (&r)[2]) {
-        store(s_j, s_git, r);
+        store(s_j, r);
         if (++s_j == spr) {
           s_j = 0;
           s_rt += stride_rt;
-          ++s_git;
         }
       };
       issue_next(ra);
@@ -341,8 +402,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
 #undef WG_ADV
     cp_async_wait<0>();
   } else {
-    wgrad_consumer<NSPLIT, false>(p, g_smem, a_smem, g_bytes, a_bytes, full_bar, empty_bar, gfull_bar, gempty_bar, unit0, nunits,
-                                  cta_in_pass, num_rt, (warp - CONS_WARP0) >> 2, (warp - CONS_WARP0) & 3, lane);
+    run_wgrad_consumer<NSPLIT, false>(p, g_smem, a_smem, g_bytes, a_bytes, bars, unit0, nunits, cta_in_pass, num_rt, warp, lane);
   }
 }
 
@@ -360,16 +420,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int n_op = (NSPLIT == 3) ? 2 : 1;
-  const int NB = p.Cout / 64;                    // 64-column blocks of gout
-  const int g_bytes = n_op * NB * WG_SUB_BYTES;  // one gout tile (hi blocks [+ lo blocks])
-  const int a_bytes = n_op * 2 * WG_SUB_BYTES;   // one stage: two sub-tiles (hi, hi [, lo, lo])
-  uint8_t* g_smem = smem;                        // [2][g_bytes]
-  uint8_t* a_smem = smem + 2 * (size_t)g_bytes;  // [stages][a_bytes]
+  const int g_bytes = n_op * p.gblocks * WG_SUB_BYTES;   // one gout tile (hi blocks [+ lo blocks])
+  const int a_bytes = n_op * 2 * WG_SUB_BYTES;           // one stage: two sub-tiles (hi, hi [, lo, lo])
+  uint8_t* g_smem = smem;                                // [gstages][g_bytes]
+  uint8_t* a_smem = smem + (size_t)p.gstages * g_bytes;  // [stages][a_bytes]
   uint64_t* bars = reinterpret_cast<uint64_t*>(a_smem + (size_t)p.stages * a_bytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + MAX_STAGES;
-  uint64_t* gfull_bar = bars + 2 * MAX_STAGES;       // [2]
-  uint64_t* gempty_bar = bars + 2 * MAX_STAGES + 2;  // [2]
+  uint64_t* gfull_bar = bars + 2 * MAX_STAGES;
+  uint64_t* gempty_bar = bars + 2 * MAX_STAGES + MAX_GSTAGES;
 
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
   const int CB = p.Cin / 64;
@@ -384,7 +443,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
       mbar_init(smem_u32(full_bar + s), 32);    // one cp.async arrival per lane of the warp that fills the slot
       mbar_init(smem_u32(empty_bar + s), NUM_CONS_WARPS);
     }
-    for (int b = 0; b < 2; ++b) {
+    for (int b = 0; b < p.gstages; ++b) {
       mbar_init(smem_u32(gfull_bar + b), 32);
       mbar_init(smem_u32(gempty_bar + b), NUM_CONS_WARPS);
     }
@@ -394,8 +453,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
 
   if (warp < NUM_GATHER_WARPS) {
     // ONE WARP PER SLOT, ownership split by resource:
-    //   * warp 7 fills every gout tile (double buffer; consecutive fills by the same warp, so its parity wait on the
-    //     "gout empty" barrier is never more than one phase away from the barrier);
+    //   * warp 7 fills every gout tile (a ring of gstages buffers, filled in order by the same warp, so its parity wait
+    //     on a "gout empty" barrier is never more than one phase away from the barrier);
     //   * warps 0 .. Wu-1 (Wu = min(7, stages)) fill the unit slots ord = w, w + Wu, ... of the CTA's unit sequence
     //     (row tile major): the stride Wu <= stages keeps a warp within one revolution of the unit ring.
     // A warp waits only on barriers of slots it owns.  (Letting all 8 warps take slots round-robin across both rings, or
@@ -416,12 +475,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
     int Wu = 1;
     for (int c = 2; c <= NUM_GATHER_WARPS - 1; ++c)
       if (p.stages % c == 0) Wu = c;
-    if (warp == NUM_GATHER_WARPS - 1) {
-      // ---- gout tiles: [64 rows][Cout] per plane, contiguous rows ----
-      for (int64_t rti = 0; rti < my_rts; ++rti) {
+    // gout producers: the last Wg warps, Wg = the largest divisor of `gstages` that the unit producers leave free; warp
+    // 8 - Wg + i fills the row tiles i, i + Wg, ... and so always the same gout buffers
+    int Wg = 1;
+    for (int c = 2; c <= NUM_GATHER_WARPS - Wu; ++c)
+      if (p.gstages % c == 0) Wg = c;
+    if (warp >= NUM_GATHER_WARPS - Wg) {
+      // ---- gout tiles: [64 rows][the units' 64-column blocks] per plane, contiguous rows ----
+      const int GB = p.gblocks, gn = gout_nblocks(p, nunits);
+      const int64_t gcol0 = gout_block(p, unit0, 0) * 64 * 2, gcol1 = gout_block(p, unit0, gn - 1) * 64 * 2;   // bytes
+      int gb = warp - (NUM_GATHER_WARPS - Wg);     // < Wg <= gstages
+      uint32_t gphase = 0;
+      for (int64_t rti = gb; rti < my_rts; rti += Wg) {
         const int64_t rt = cta_in_pass + rti * stride_rt;
-        const int gb = (int)(rti & 1);
-        mbar_wait(smem_u32(gempty_bar + gb), (uint32_t)(((rti >> 1) & 1) ^ 1));
+        mbar_wait(smem_u32(gempty_bar + gb), gphase ^ 1);
         const uint32_t g0 = smem_u32(g_smem + (size_t)gb * g_bytes) + (uint32_t)sub * 128u;
 #pragma unroll 4
         for (int i = 0; i < WG_R / 4; ++i) {
@@ -429,12 +496,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
           const uint32_t nbytes = row < p.n_out ? 16u : 0u;
           const int64_t boff = ((row < p.n_out ? row : 0) * p.gout_pitch + ch * 8) * 2;
           const uint32_t off = (uint32_t)i * 512u + (((uint32_t)ch ^ (((uint32_t)(i & 1) << 2) + (uint32_t)sub)) << 4);
-          for (int nb = 0; nb < NB; ++nb) {
-            cp_async16_zfill(g0 + (uint32_t)nb * WG_SUB_BYTES + off, gp_hi + boff + nb * 128, nbytes);
-            if (NSPLIT == 3) cp_async16_zfill(g0 + (uint32_t)(NB + nb) * WG_SUB_BYTES + off, gp_lo + boff + nb * 128, nbytes);
+          for (int b = 0; b < gn; ++b) {
+            const int64_t src = boff + (b == 0 ? gcol0 : gcol1);
+            cp_async16_zfill(g0 + (uint32_t)b * WG_SUB_BYTES + off, gp_hi + src, nbytes);
+            if (NSPLIT == 3) cp_async16_zfill(g0 + (uint32_t)(GB + b) * WG_SUB_BYTES + off, gp_lo + src, nbytes);
           }
         }
         cp_async_mbar_arrive_noinc(smem_u32(gfull_bar + gb));
+        gb += Wg;                                   // at most one wrap: Wg <= gstages
+        if (gb >= p.gstages) {
+          gb -= p.gstages;
+          gphase ^= 1;
+        }
       }
     } else if (warp < Wu) {
       // ---- units: two gathered [64 rows][64 ch] sub-tiles each ----
@@ -494,8 +567,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
     cp_async_commit();
     cp_async_wait<0>();
   } else {
-    wgrad_consumer<NSPLIT, true>(p, g_smem, a_smem, g_bytes, a_bytes, full_bar, empty_bar, gfull_bar, gempty_bar, unit0, nunits,
-                                 cta_in_pass, num_rt, (warp - CONS_WARP0) >> 2, (warp - CONS_WARP0) & 3, lane);
+    run_wgrad_consumer<NSPLIT, true>(p, g_smem, a_smem, g_bytes, a_bytes, bars, unit0, nunits, cta_in_pass, num_rt, warp, lane);
   }
 }
 
@@ -541,17 +613,31 @@ int wgrad_launch(const char* fn, WgradParams& p, int64_t n_out, int32_t K, int32
   int dev = 0, smem_optin = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  // shared memory: two gout tiles, the unit stages, barriers and, for k_wgrad_tc, its index ring and slot descriptors
+  unit_plan(p, K, Cin, Cout);
+  p.gblocks = p.uc == 128 ? 2 : (p.ncr > 1 ? p.units_per_pass : 1);
+  // shared memory: the gout ring, the unit ring, barriers and, for k_wgrad_tc, its index ring and slot descriptors.
+  // With one wgmma group in flight the consumers hold one buffer of each ring, so gstages - 1 gout tiles and stages - 1
+  // unit slots (units_per_pass per row tile) can be filled ahead of the MMAs: the two depths are picked together for
+  // the most row tiles filled ahead, then for the most unit stages.
   const int n_op = precision == 3 ? 2 : 1;
-  const int g_bytes = n_op * (Cout / 64) * WG_SUB_BYTES;
+  const int g_bytes = n_op * p.gblocks * WG_SUB_BYTES;
   const int a_bytes = n_op * 2 * WG_SUB_BYTES;
-  const int fixed = 1024 + (2 * MAX_STAGES + 4) * 8 + (planes ? 0 : IDX_RING * 2 * WG_R * 4 + 16 * 8 * 4);
-  int stages = (smem_optin - fixed - 2 * g_bytes) / a_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  PASCO_CHECK_ARG(stages >= 2, "%s: not enough shared memory", fn);
+  const int fixed = 1024 + 2 * (MAX_STAGES + MAX_GSTAGES) * 8 + (planes ? 0 : IDX_RING * 2 * WG_R * 4 + 16 * 8 * 4);
+  const int upr = p.units_per_pass;
+  int stages = 0, gstages = 0, best = -1;
+  for (int gs = 2; gs <= MAX_GSTAGES; ++gs) {
+    const int st = std::min(MAX_STAGES, (smem_optin - fixed - gs * g_bytes) / a_bytes);
+    const int ahead = std::min((gs - 1) * upr, st - 1);     // row tiles filled ahead, times units_per_pass
+    if (st >= 3 && ahead > best) {
+      best = ahead;
+      stages = st;
+      gstages = gs;
+    }
+  }
+  PASCO_CHECK_ARG(stages >= 3, "%s: not enough shared memory", fn);   // a stage is filled, one multiplied, one held back
   if (planes) {   // the stage count with the largest divisor <= 7 (= the number of unit producer warps, see k_wgrad_pl)
     int pick = stages, pick_w = 0;
-    for (int st = stages; st >= 2; --st) {
+    for (int st = stages; st >= 3; --st) {
       int w = 1;
       for (int c = 2; c <= 7; ++c)
         if (st % c == 0) w = c;
@@ -561,10 +647,10 @@ int wgrad_launch(const char* fn, WgradParams& p, int64_t n_out, int32_t K, int32
   }
   p.n_out = n_out; p.K = K; p.Cin = Cin; p.Cout = Cout;
   p.stages = stages;
-  unit_plan(p, K, Cin, Cout);
+  p.gstages = gstages;
   p.ctas_per_pass = ctas_per_pass((n_out + WG_R - 1) / WG_R, p.passes);
   p.slot = (int64_t)p.units_per_pass * 128 * p.uc;
-  const size_t smem = (size_t)2 * g_bytes + (size_t)stages * a_bytes + fixed;
+  const size_t smem = (size_t)gstages * g_bytes + (size_t)stages * a_bytes + fixed;
   const int grid = p.passes * p.ctas_per_pass;
   const cudaStream_t st = (cudaStream_t)s;
   cudaError_t e = ws_alloc((void**)&p.part, (size_t)grid * p.slot * sizeof(float), st);

@@ -1,6 +1,10 @@
 """Micro-benchmark of the map-building and convolution kernels on BASELINE-shaped synthetic scenes.
 
-    python tools/conv_microbench.py [--occ 0.1] [--channels 64] [--out gpurun_out/micro.jsonl]
+    python tools/conv_microbench.py [--occ 0.1] [--channels 64] [--stride 1] [--out FILE.jsonl]
+
+--stride S times the level-S coordinate set of the same synthetic grid (coordinates divided by S, duplicates merged),
+so that a kernel runs at the size it has at the network's stride-S level: the network convolves 64 channels at stride
+1, 128 at stride 2 and 256 at strides 4 and 8.
 
 Times each kernel with CUDA events (3 warm-ups, 10 timed launches, L2 flushed between launches by
 writing a 256 MB buffer) and prints achieved algorithmic GB/s / TFLOP/s per SURVEY.md §8d formulas.
@@ -41,6 +45,7 @@ def main():
     ap.add_argument("--grid", type=int, nargs=3, default=[256, 256, 32])
     ap.add_argument("--occ", type=float, nargs="+", default=[0.1, 0.5])
     ap.add_argument("--channels", type=int, nargs="+", default=[64, 128])
+    ap.add_argument("--stride", type=int, default=1)
     ap.add_argument("--out", default="gpurun_out/micro.jsonl")
     a = ap.parse_args()
     os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
@@ -57,6 +62,8 @@ def main():
         g = torch.Generator(device="cpu").manual_seed(0)
         o = torch.rand(*a.grid, generator=g) < occ
         c = torch.nonzero(o).int()
+        if a.stride > 1:
+            c = torch.unique(torch.div(c, a.stride, rounding_mode="floor"), dim=0)
         C = torch.cat([torch.zeros(c.shape[0], 1, dtype=torch.int32), c], 1).to(dev)
         N = C.shape[0]
         t_ins = timed(lambda: ops.hash_insert(C), flush=flush)
@@ -64,7 +71,7 @@ def main():
         t_probe = timed(lambda: ops.kernel_map_probe(C, table, 3, (1, 1, 1)), flush=flush)
         nbr = ops.kernel_map_probe(C, table, 3, (1, 1, 1))
         pairs = int((nbr >= 0).sum())
-        emit(kind="maps", occ=occ, N=N, pairs=pairs, insert_ms=t_ins, probe_ms=t_probe,
+        emit(kind="maps", occ=occ, stride=a.stride, N=N, pairs=pairs, insert_ms=t_ins, probe_ms=t_probe,
              insert_GBs=16 * N / t_ins / 1e6, probe_GBs=(16 + 4 * 27) * N / t_probe / 1e6)
         for ch in a.channels:
             F = torch.randn(N, ch, device=dev)
@@ -88,7 +95,7 @@ def main():
                 flops = 2.0 * pairs * ch * ch
                 issued = 2.0 * N * 27 * ch * ch * (3 if prec == "fp32" else 1)
                 bytes_min = 4.0 * (2 * N * ch) + 4.0 * 27 * ch * ch + 8.0 * pairs
-                emit(kind="conv3", occ=occ, N=N, C=ch, pairs=pairs, precision=prec, split_ms=split,
+                emit(kind="conv3", occ=occ, stride=a.stride, N=N, C=ch, pairs=pairs, precision=prec, split_ms=split,
                      fwd_planes_ms=fwd_pl, dgrad_planes_ms=dgr_pl, wgrad_planes_ms=wgr_pl,
                      fwd_regs_ms=fwd, dgrad_regs_ms=dgr, wgrad_regs_ms=wgr,
                      fwd_planes_useful_TFLOPs=flops / fwd_pl / 1e9, fwd_planes_issued_TFLOPs=issued / fwd_pl / 1e9,
