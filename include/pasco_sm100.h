@@ -7,7 +7,10 @@
  * as pasco/<file>:<line> (paths relative to /root/reference).
  *
  * Conventions
- *   - plain C types, raw DEVICE pointers, caller-owned memory (the library never allocates);
+ *   - plain C types, raw DEVICE pointers; inputs and outputs are caller-owned memory;
+ *   - scratch a call needs for itself comes from a stream-ordered memory pool of the library's own and is released
+ *     on the call's stream; the one exception is the split-K convolution, whose caller passes its workspace
+ *     (pasco_conv_splitk_workspace_bytes also tells the caller whether a shape is split at all);
  *   - every call takes the CUDA stream to launch on (pass torch's current stream);
  *   - returns 0 on success, negative on error; pasco_last_error() gives the message of the
  *     last failure on the calling thread;
@@ -219,12 +222,10 @@ int pasco_bn_bwd_apply(const float* dy, const float* x, int64_t n, int32_t C, co
  *      transformer_predictor_v2.py:220-289): Q <= 128 queries against all P voxels, H heads of width D <= 64 ------
  * q [Q, H*D], k / v [P, H*D] float32 (already projected); logits = scale * q.k; mask = bit rows
  * uint32 [Q, 2*ceil(P/64)] (bit j of word 2t + j/32 set = key 64t + j masked) or NULL; out [Q, H*D] is overwritten
- * (the key chunks' shares are summed in a fixed order); lse [H, Q] receives log-sum-exp per row (needed by the backward).  Two streaming passes over K (row
- * statistics, then output), wgmma for both GEMMs, bf16x3 split operands.                                          */
-int64_t pasco_xattn_workspace_bytes(int32_t Q, int64_t P, int32_t H, int32_t D);
+ * (the key chunks' shares are summed in a fixed order); lse [H, Q] receives log-sum-exp per row (needed by the
+ * backward).  Two streaming passes over K (row statistics, then output), wgmma for both GEMMs, bf16x3 split operands. */
 int pasco_xattn_forward(const float* q, const float* k, const float* v, const uint32_t* mask, int32_t Q, int64_t P,
-                        int32_t H, int32_t D, float scale, float* out, float* lse, float* workspace,
-                        int64_t workspace_bytes, pasco_stream_t s);
+                        int32_t H, int32_t D, float scale, float* out, float* lse, pasco_stream_t s);
 /* backward of the above: recomputes the probabilities from lse; dq [Q, H*D] is overwritten (chunk shares, fixed order),
  * dk / dv [P, H*D] are fully overwritten (every row written exactly once, no atomics).                            */
 int pasco_xattn_backward(const float* q, const float* k, const float* v, const uint32_t* mask, const float* lse,

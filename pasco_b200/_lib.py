@@ -56,8 +56,7 @@ PROTOTYPES = {
     "pasco_bn_finalize": (C.c_int, [_p, _p, C.c_double, _i32, _p, _p, C.c_float, C.c_float, _p, _p, _p, _p, _p, _p, _p]),
     "pasco_bn_bwd_coefs": (C.c_int, [_p, _p, C.c_double, _i32, _p, _p, _p, C.c_float, _p, _p, _p, _p, _p, _p]),
     "pasco_bn_bwd_reduce": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i32, _p, _p]),
-    "pasco_xattn_workspace_bytes": (_i64, [_i32, _i64, _i32, _i32]),
-    "pasco_xattn_forward": (C.c_int, [_p, _p, _p, _p, _i32, _i64, _i32, _i32, C.c_float, _p, _p, _p, _i64, _p]),
+    "pasco_xattn_forward": (C.c_int, [_p, _p, _p, _p, _i32, _i64, _i32, _i32, C.c_float, _p, _p, _p]),
     "pasco_xattn_backward": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, C.c_float, _p, _p, _p, _p]),
     "pasco_bn_bwd_apply": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i32, _p, _p, _p, _p, _p]),
 }

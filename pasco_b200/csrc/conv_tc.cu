@@ -101,7 +101,7 @@ __global__ void k_pack_weights(const float* __restrict__ W, int K, int Cin, int 
     hi = make_uint4(h0.x, h0.y, h1.x, h1.y);
     lo = make_uint4(l0.x, l0.y, l1.x, l1.y);
     int64_t tile = ((int64_t)k * KB + kb) * (int64_t)N * 256;  // hi image then lo image
-    int64_t off = (int64_t)n * 128 + ((c ^ (n & 7)) << 4);
+    const int64_t off = sw128_off<int64_t>(n, c);
     *reinterpret_cast<uint4*>(packed + tile + off) = hi;
     *reinterpret_cast<uint4*>(packed + tile + (int64_t)N * 128 + off) = lo;
   }
@@ -493,7 +493,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
       for (int i = 0; i < LOADS_PER_SLOT; ++i) {
         const float4 x = v[i];
         const uint32_t trow = row_base + i * 2;
-        const uint32_t off = trow * 128u + ((((uint32_t)chunk >> 1) ^ (trow & 7u)) << 4) + (((uint32_t)chunk & 1u) << 3);
+        const uint32_t off = sw128_half_off(trow, chunk);
         if (NSPLIT == 3) {
           uint2 hi, lo;
           split4(x, hi, lo);
@@ -656,7 +656,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
         const int idx = __shfl_sync(0xffffffffu, q0.v[i >> 3], ((i & 7) << 2) + sub);
         const uint32_t nbytes = idx >= 0 ? 16u : 0u;
         const int64_t boff = (int64_t)(idx >= 0 ? idx : 0) * pitch_b + coff_b;
-        // byte offset of (row r, chunk ch) in the swizzled tile: r*128 + ((ch ^ (r & 7)) << 4), r & 7 = 4 (i & 1) + sub
+        // sw128_off(r, ch) with r*128 = i*512 + sub*128 (the latter folded into dst0) and r & 7 = 4 (i & 1) + sub
         const uint32_t off = (uint32_t)i * 512u + (((uint32_t)ch ^ (((uint32_t)(i & 1) << 2) + (uint32_t)sub)) << 4);
         cp_async16_zfill(dst0 + off, base_hi + boff, nbytes);
         if (NSPLIT == 3) cp_async16_zfill(dst0 + A_TILE_BYTES + off, base_lo + boff, nbytes);

@@ -108,6 +108,13 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t
   d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
 }
+// byte offset of 16-byte chunk `chunk` of row `row` in such a tile (T = int64_t where the offset joins a 64-bit one),
+// and of 8-byte half-chunk `half` (= 2 chunk + 0/1)
+template <typename T>
+__device__ __forceinline__ T sw128_off(T row, uint32_t chunk) { return row * 128 + ((chunk ^ ((uint32_t)row & 7u)) << 4); }
+__device__ __forceinline__ uint32_t sw128_half_off(uint32_t row, uint32_t half) {
+  return sw128_off(row, half >> 1) + ((half & 1u) << 3);
+}
 
 // ---- wgmma ---------------------------------------------------------------------------------------------------
 // Issued by a whole warpgroup (4 consecutive warps starting at a multiple of 4).  D[64 x N] fp32 lives in registers:

@@ -16,7 +16,7 @@ void set_error(const char* fmt, ...) {
 using namespace pasco;
 
 extern "C" const char* pasco_last_error(void) { return pasco::g_err; }
-extern "C" int pasco_abi_version(void) { return 2; }
+extern "C" int pasco_abi_version(void) { return 3; }
 extern "C" int pasco_device_info(int* sm_count, int* smem_optin, int* cc) {
   int dev = 0, v = 0, maj = 0, min = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) {

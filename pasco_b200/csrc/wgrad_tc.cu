@@ -73,7 +73,7 @@ __device__ __forceinline__ void sub_store(const SubRegs& r, uint8_t* dst_hi, uin
   for (int i = 0; i < WLOADS; ++i) {
     const float4 x = r.v[i];
     const uint32_t trow = (uint32_t)(warp * WROWS + i * 2 + rsub);
-    const uint32_t off = trow * 128u + ((((uint32_t)chunk >> 1) ^ (trow & 7u)) << 4) + (((uint32_t)chunk & 1u) << 3);
+    const uint32_t off = sw128_half_off(trow, chunk);
     if (NSPLIT == 3) {
       uint2 hi, lo;
       split4(x, hi, lo);

@@ -17,7 +17,9 @@
 // A CTA = (head, key chunk); warps 0-3 (one warpgroup): issue the MMAs, pass each result through a [64 col][128 row]
 // fp32 scratch so that thread t then holds query row t (mask, exp, row statistics); warps 4-7: K/V tile gather (16
 // lanes per 256-byte padded row segment, fp32 → bf16 hi/lo split, 128-byte swizzle).  Operands are split bf16x3 like
-// the convolution ("fp32" mode).
+// the convolution ("fp32" mode).  The backward (below) shares the CTAs, the warp roles, the K/V producer, the operand
+// staging and the mask bits with the forward; only the consumer bodies differ.
+#include <initializer_list>
 #include <math_constants.h>
 #include "common.cuh"
 #include "gmma.cuh"
@@ -35,15 +37,19 @@ constexpr int TILE_K = BK * 128;            // 8 KB : [64 keys][64] bf16
 constexpr int NTHREADS = 8 * 32;
 constexpr int SCRATCH = 64 * QM * 4;        // 32 KB: one [64 col][128 row] fp32 accumulator, row-contiguous per column
 
+// arguments of both forward passes and of the backward; the fields a kernel does not use are null
 struct XParams {
-  const float* q;      // [Q, H*D]
-  const float* k;      // [P, H*D]
-  const float* v;      // [P, H*D]
+  const float* q;       // [Q, H*D]
+  const float* k;       // [P, H*D]
+  const float* v;       // [P, H*D]
   const uint32_t* mask; // bit rows [Q, 2*ceil(P/64)]: bit j of word 2t + j/32 = key 64t + j masked; nullptr = none
-  const float* lse;    // [H, Q]            (pass 1)
-  float* out;          // [Q, H*D]          (written by k_xattn_osum)
-  float* ws;           // [chunks, H, Q, 2] (pass 0)
-  float* opart;        // [chunks, Q, H*D]  (pass 1: this chunk's share of O)
+  const float* lse;     // [H, Q]            (forward pass 1, backward)
+  const float* out;     // [Q, H*D]          (backward: the forward's output)
+  const float* dout;    // [Q, H*D]          (backward)
+  float* dk;            // [P, H*D]          (backward)
+  float* dv;            // [P, H*D]          (backward)
+  float* ws;            // [chunks, H, Q, 2] (forward pass 0: row statistics of each chunk)
+  float* part;          // [chunks, Q, H*D]  (this chunk's share of O in forward pass 1, of dQ in the backward)
   int Q, H, D;
   int64_t P;
   int chunks;
@@ -62,8 +68,6 @@ constexpr int OFF_P = OFF_KV + 2 * KV_STAGE;
 constexpr int OFF_SCR = OFF_P + 2 * TILE_Q;
 constexpr int OFF_BAR = OFF_SCR + SCRATCH;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-
-__device__ __forceinline__ uint32_t sw_off(uint32_t row, uint32_t chunk16) { return row * 128u + ((chunk16 ^ (row & 7u)) << 4); }
 
 // D[128 rows][64] (+)= A[128 rows][16 k-steps of K-major smem, 64 K] · B[64 K][64 N], bf16x3; A K-major, B K-major (TB = 0)
 // with 16-element k-steps of 32 bytes, or MN-major (TB = 1) with 16-row k-steps of 2048 bytes
@@ -101,6 +105,127 @@ __device__ __forceinline__ void acc_to_rows(const float (&d)[2][32], float* scr,
   for (int j = 0; j < 64; ++j) v[j] = scr[j * QM + row];
 }
 
+// this CTA's head, key chunk, and its key tiles [t0, t0 + my_tiles) out of the n_tiles that cover P
+struct CtaTiles {
+  int h, chunk;
+  int64_t n_tiles, t0, my_tiles;
+};
+__device__ __forceinline__ CtaTiles cta_tiles(const XParams& p) {
+  CtaTiles c;
+  c.h = blockIdx.x % p.H;
+  c.chunk = blockIdx.x / p.H;
+  c.n_tiles = (p.P + BK - 1) / BK;
+  const int64_t tiles_per_chunk = (c.n_tiles + p.chunks - 1) / p.chunks;
+  c.t0 = (int64_t)c.chunk * tiles_per_chunk;
+  const int64_t t1 = c.t0 + tiles_per_chunk < c.n_tiles ? c.t0 + tiles_per_chunk : c.n_tiles;
+  c.my_tiles = t1 > c.t0 ? t1 - c.t0 : 0;
+  return c;
+}
+
+// the two-stage K/V ring: full[s] takes one arrival per gather warp, empty[s] one per MMA warp
+__device__ __forceinline__ void init_kv_ring(uint64_t* kv_full, uint64_t* kv_empty) {
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(smem_u32(kv_full + i), 4);
+      mbar_init(smem_u32(kv_empty + i), 4);
+    }
+    fence_barrier_init();
+  }
+}
+
+// f[0..7] → bf16 hi / lo of 16-byte chunk c of row `row` in a [128 rows][64] tile pair (hi at `tile`, lo TILE_Q on)
+__device__ __forceinline__ void store_split8(uint8_t* tile, uint32_t row, uint32_t c, const float* f) {
+  uint2 h0, l0, h1, l1;
+  split4(make_float4(f[0], f[1], f[2], f[3]), h0, l0);
+  split4(make_float4(f[4], f[5], f[6], f[7]), h1, l1);
+  const uint32_t off = sw128_off(row, c);
+  *reinterpret_cast<uint4*>(tile + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
+  *reinterpret_cast<uint4*>(tile + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
+}
+
+// resident operand, all threads: head h's columns of the [Q, H*D] matrix `src` times `factor` → bf16 hi / lo
+// [128 rows][64] at `tile`; rows >= Q and columns >= D are zero
+__device__ __forceinline__ void stage_rows(uint8_t* tile, const float* src, float factor, const XParams& p, int h) {
+  const int HD = p.H * p.D;
+  for (int t = threadIdx.x; t < QM * 8; t += NTHREADS) {       // one 16-byte output chunk (8 bf16) per iteration
+    const int row = t >> 3, c = t & 7;
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int d = c * 8 + j;
+      f[j] = (row < p.Q && d < p.D) ? __ldg(src + (int64_t)row * HD + h * p.D + d) * factor : 0.f;
+    }
+    store_split8(tile, row, c, f);
+  }
+}
+
+// warps 4-7 (16 keys per warp): the CTA's K tiles, and V tiles when WITH_V, into the two-stage ring at `ring`
+template <bool WITH_V>
+__device__ __forceinline__ void produce_kv(const XParams& p, const CtaTiles& ct, uint8_t* ring, uint64_t* kv_full,
+                                           uint64_t* kv_empty, int warp, int lane) {
+  const int HD = p.H * p.D;
+  const int gw = warp - 4;
+  const int chunk4 = lane & 15, rsub = lane >> 4;
+  uint32_t phase = 0;
+  for (int64_t it = 0; it < ct.my_tiles; ++it) {
+    const int st = (int)(it & 1);
+    const int64_t key0 = (ct.t0 + it) * BK;
+    // loads first (before the stage is free)
+    float4 kv[2][8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int r = gw * 16 + i * 2 + rsub;
+      const int64_t key = key0 + r;
+      const bool ok = key < p.P && chunk4 * 4 < p.D;
+      kv[0][i] = ok ? __ldg(reinterpret_cast<const float4*>(p.k + key * HD + ct.h * p.D + chunk4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      if (WITH_V)
+        kv[1][i] = ok ? __ldg(reinterpret_cast<const float4*>(p.v + key * HD + ct.h * p.D + chunk4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    mbar_wait(smem_u32(kv_empty + st), phase ^ 1);
+    uint8_t* base = ring + st * KV_STAGE;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const uint32_t off = sw128_half_off((uint32_t)(gw * 16 + i * 2 + rsub), (uint32_t)chunk4);
+      uint2 hi, lo;
+      split4(kv[0][i], hi, lo);
+      *reinterpret_cast<uint2*>(base + off) = hi;
+      *reinterpret_cast<uint2*>(base + TILE_K + off) = lo;
+      if (WITH_V) {
+        split4(kv[1][i], hi, lo);
+        *reinterpret_cast<uint2*>(base + 2 * TILE_K + off) = hi;
+        *reinterpret_cast<uint2*>(base + 3 * TILE_K + off) = lo;
+      }
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(kv_full + st));
+    if (st == 1) phase ^= 1;
+  }
+}
+
+// mask bits of query row `qrow` for the 64 keys of `tile` (bit set = masked); keys >= P and rows >= Q are masked
+__device__ __forceinline__ void tile_mask_bits(uint32_t (&mbits)[2], const XParams& p, int qrow, int64_t n_tiles,
+                                               int64_t tile) {
+  mbits[0] = mbits[1] = 0xffffffffu;
+  if (qrow >= p.Q) return;
+  if (p.mask) {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.mask + ((int64_t)qrow * n_tiles + tile) * 2));
+    mbits[0] = w.x;
+    mbits[1] = w.y;
+  } else {
+    mbits[0] = mbits[1] = 0u;
+  }
+  const int64_t left = p.P - tile * BK;
+  if (left < 64) {
+    if (left <= 32) {
+      mbits[1] = 0xffffffffu;
+      if (left < 32) mbits[0] |= ~0u << left;
+    } else {
+      mbits[1] |= ~0u << (left - 32);
+    }
+  }
+}
+
 template <int PASS>
 __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant__ XParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -111,81 +236,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
   float* scr = reinterpret_cast<float*>(smem + OFF_SCR);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int h = blockIdx.x % p.H;
-  const int chunk = blockIdx.x / p.H;
-  const int64_t n_tiles = (p.P + BK - 1) / BK;
-  const int64_t tiles_per_chunk = (n_tiles + p.chunks - 1) / p.chunks;
-  const int64_t t0 = (int64_t)chunk * tiles_per_chunk;
-  const int64_t t1 = t0 + tiles_per_chunk < n_tiles ? t0 + tiles_per_chunk : n_tiles;
-  const int64_t my_tiles = t1 > t0 ? t1 - t0 : 0;
+  const CtaTiles ct = cta_tiles(p);
+  const int h = ct.h;
   const int HD = p.H * p.D;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(kv_full + i), 4);
-      mbar_init(smem_u32(kv_empty + i), 4);
-    }
-    fence_barrier_init();
-  }
-  // ---- resident query operand: Q_h * scale → bf16 hi/lo, rows >= Q and columns >= D are zero ----
-  for (int t = threadIdx.x; t < QM * 8; t += NTHREADS) {       // one 16-byte output chunk (8 bf16) per iteration
-    const int row = t >> 3, c = t & 7;
-    float f[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int d = c * 8 + j;
-      f[j] = (row < p.Q && d < p.D) ? __ldg(p.q + (int64_t)row * HD + h * p.D + d) * p.scale : 0.f;
-    }
-    uint2 h0, l0, h1, l1;
-    split4(make_float4(f[0], f[1], f[2], f[3]), h0, l0);
-    split4(make_float4(f[4], f[5], f[6], f[7]), h1, l1);
-    const uint32_t off = sw_off(row, c);
-    *reinterpret_cast<uint4*>(smem + OFF_Q + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-    *reinterpret_cast<uint4*>(smem + OFF_Q + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-  }
+  init_kv_ring(kv_full, kv_empty);
+  stage_rows(smem + OFF_Q, p.q, p.scale, p, h);      // resident query operand Q_h * scale
   fence_proxy_async_smem();
   __syncthreads();
 
   if (warp >= 4) {
-    // ===================================== K / V tile gather =====================================
-    const int gw = warp - 4;                 // 16 keys per warp
-    const int chunk4 = lane & 15, rsub = lane >> 4;
-    uint32_t phase = 0;
-    for (int64_t it = 0; it < my_tiles; ++it) {
-      const int st = (int)(it & 1);
-      const int64_t key0 = (t0 + it) * BK;
-      // loads first (before the stage is free)
-      float4 kv[2][8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int r = gw * 16 + i * 2 + rsub;
-        const int64_t key = key0 + r;
-        const bool ok = key < p.P && chunk4 * 4 < p.D;
-        kv[0][i] = ok ? __ldg(reinterpret_cast<const float4*>(p.k + key * HD + h * p.D + chunk4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        if (PASS == 1)
-          kv[1][i] = ok ? __ldg(reinterpret_cast<const float4*>(p.v + key * HD + h * p.D + chunk4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      mbar_wait(smem_u32(kv_empty + st), phase ^ 1);
-      uint8_t* base = smem + OFF_KV + st * KV_STAGE;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const uint32_t r = (uint32_t)(gw * 16 + i * 2 + rsub);
-        const uint32_t off = r * 128u + ((((uint32_t)chunk4 >> 1) ^ (r & 7u)) << 4) + (((uint32_t)chunk4 & 1u) << 3);
-        uint2 hi, lo;
-        split4(kv[0][i], hi, lo);
-        *reinterpret_cast<uint2*>(base + off) = hi;
-        *reinterpret_cast<uint2*>(base + TILE_K + off) = lo;
-        if (PASS == 1) {
-          split4(kv[1][i], hi, lo);
-          *reinterpret_cast<uint2*>(base + 2 * TILE_K + off) = hi;
-          *reinterpret_cast<uint2*>(base + 3 * TILE_K + off) = lo;
-        }
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(kv_full + st));
-      if (st == 1) phase ^= 1;
-    }
+    produce_kv<PASS == 1>(p, ct, smem + OFF_KV, kv_full, kv_empty, warp, lane);
   } else {
     // ===================================== MMA + softmax rows (warps 0-3) =====================================
     const int qrow = warp * 32 + lane;
@@ -196,29 +257,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
     const float my_lse = (PASS == 1 && qok) ? __ldg(p.lse + (int64_t)h * p.Q + qrow) : 0.f;
     float oacc[2][32];
     zero_acc(oacc);
-    for (int64_t it = 0; it < my_tiles; ++it) {
+    for (int64_t it = 0; it < ct.my_tiles; ++it) {
       const int st = (int)(it & 1);
-      const int64_t key0 = (t0 + it) * BK;
-      // mask bytes of this row for the 64 keys of the tile
-      uint32_t mbits[2] = {0xffffffffu, 0xffffffffu};
-      if (qok) {
-        if (p.mask) {
-          const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.mask + ((int64_t)qrow * n_tiles + (t0 + it)) * 2));
-          mbits[0] = w.x;
-          mbits[1] = w.y;
-        } else {
-          mbits[0] = mbits[1] = 0u;
-        }
-        const int64_t left = p.P - key0;          // keys beyond P are masked
-        if (left < 64) {
-          if (left <= 32) {
-            mbits[1] = 0xffffffffu;
-            if (left < 32) mbits[0] |= ~0u << left;
-          } else {
-            mbits[1] |= ~0u << (left - 32);
-          }
-        }
-      }
+      uint32_t mbits[2];
+      tile_mask_bits(mbits, p, qrow, ct.n_tiles, ct.t0 + it);
       mbar_wait(smem_u32(kv_full + st), (uint32_t)((it >> 1) & 1));
       const uint32_t k_hi = smem_u32(smem + OFF_KV + st * KV_STAGE), k_lo = k_hi + TILE_K;
       float s[BK];
@@ -247,7 +289,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
           m_run = mx;
         }
       } else {
-        uint8_t* ph = smem + OFF_P;
 #pragma unroll
         for (int c = 0; c < 8; ++c) {       // 8 probabilities per 16-byte chunk
           float f[8];
@@ -256,12 +297,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
             const int col = c * 8 + j;
             f[j] = ((mbits[col >> 5] >> (col & 31)) & 1u) ? 0.f : __expf(s[col] - my_lse);
           }
-          uint2 h0, l0, h1, l1;
-          split4(make_float4(f[0], f[1], f[2], f[3]), h0, l0);
-          split4(make_float4(f[4], f[5], f[6], f[7]), h1, l1);
-          const uint32_t off = sw_off((uint32_t)qrow, (uint32_t)c);
-          *reinterpret_cast<uint4*>(ph + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-          *reinterpret_cast<uint4*>(ph + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
+          store_split8(smem + OFF_P, (uint32_t)qrow, (uint32_t)c, f);
         }
         fence_proxy_async_smem();
         named_sync(1, 128);                 // the whole P tile is written
@@ -276,7 +312,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
     }
     if (PASS == 0) {
       if (qok) {
-        float* w = p.ws + (((int64_t)chunk * p.H + h) * p.Q + qrow) * 2;
+        float* w = p.ws + (((int64_t)ct.chunk * p.H + h) * p.Q + qrow) * 2;
         w[0] = m_run;
         w[1] = l_run;
       }
@@ -284,7 +320,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
       float o[DP];
       acc_to_rows(oacc, scr, o, warp, lane);
       if (qok) {
-        float* orow = p.opart + ((int64_t)chunk * p.Q + qrow) * HD + h * p.D;
+        float* orow = p.part + ((int64_t)ct.chunk * p.Q + qrow) * HD + h * p.D;
 #pragma unroll
         for (int d = 0; d < DP; ++d)
           if (d < p.D) orow[d] = o[d];
@@ -322,37 +358,53 @@ int pick_chunks(int64_t P, int H) {
   return c < 1 ? 1 : c;
 }
 
-}  // namespace
-
-extern "C" int64_t pasco_xattn_workspace_bytes(int32_t Q, int64_t P, int32_t H, int32_t D) {
-  return (int64_t)pick_chunks(P, H) * Q * H * (2 + D) * sizeof(float);   // row statistics + per-chunk shares of O
-}
-
-extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* v, const uint32_t* mask, int32_t Q,
-                                   int64_t P, int32_t H, int32_t D, float scale, float* out, float* lse, float* workspace,
-                                   int64_t workspace_bytes, pasco_stream_t s) {
-  PASCO_CHECK_ARG(Q >= 1 && Q <= QM, "pasco_xattn_forward: Q (%d) must be in [1,128]", Q);
-  PASCO_CHECK_ARG(D >= 4 && D <= DP && D % 4 == 0, "pasco_xattn_forward: head dim (%d) must be a multiple of 4, <= 64", D);
-  PASCO_CHECK_ARG((H * D) % 4 == 0 && P >= 1, "pasco_xattn_forward: bad shape");
-  PASCO_CHECK_ARG(workspace_bytes >= pasco_xattn_workspace_bytes(Q, P, H, D), "pasco_xattn_forward: workspace too small");
-  PASCO_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) == 0, "pasco_xattn_forward: pointers must be 16-byte aligned");
-  XParams p;
-  p.q = q; p.k = k; p.v = v; p.mask = mask; p.lse = lse; p.out = out; p.ws = workspace;
+// What both entry points do before their launches: check the shape, fill in the shape fields and the chunk count of
+// `p`, opt the kernels in to `smem` bytes of shared memory, and take the chunks' shares `part` [chunks, Q, H*D] (with
+// row_stats, the forward's `ws` [chunks, H, Q, 2] behind them) from the library's stream-ordered pool.  The caller
+// frees p.part on the same stream after its launches.
+int xattn_setup(const char* fn, XParams& p, int32_t Q, int64_t P, int32_t H, int32_t D, float scale, int smem,
+                std::initializer_list<const void*> kernels, bool row_stats, cudaStream_t st) {
+  PASCO_CHECK_ARG(Q >= 1 && Q <= QM, "%s: Q (%d) must be in [1,128]", fn, Q);
+  PASCO_CHECK_ARG(D >= 4 && D <= DP && D % 4 == 0, "%s: head dim (%d) must be a multiple of 4, <= 64", fn, D);
+  PASCO_CHECK_ARG(H >= 1 && P >= 1, "%s: bad shape (H = %d, P = %lld)", fn, H, (long long)P);
   p.Q = Q; p.H = H; p.D = D; p.P = P; p.scale = scale;
   p.chunks = pick_chunks(P, H);
-  p.opart = workspace + (int64_t)p.chunks * H * Q * 2;
-  cudaStream_t st = (cudaStream_t)s;
-  const int grid = p.chunks * H;
-  cudaError_t e = cudaFuncSetAttribute(k_xattn_fwd<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_xattn_fwd<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+  for (const void* k : kernels) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) {
+      set_error("%s: cudaFuncSetAttribute(%d) failed: %s", fn, smem, cudaGetErrorString(e));
+      return -1;
+    }
+  }
+  const int64_t n = (int64_t)p.chunks * Q * H * D, stats = row_stats ? (int64_t)p.chunks * H * Q * 2 : 0;
+  const cudaError_t e = ws_alloc((void**)&p.part, (size_t)(n + stats) * sizeof(float), st);
   if (e != cudaSuccess) {
-    set_error("pasco_xattn_forward: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+    set_error("%s: workspace of %lld bytes: %s", fn, (long long)(n + stats) * 4, cudaGetErrorString(e));
     return -1;
   }
+  p.ws = row_stats ? p.part + n : nullptr;
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* v, const uint32_t* mask, int32_t Q,
+                                   int64_t P, int32_t H, int32_t D, float scale, float* out, float* lse,
+                                   pasco_stream_t s) {
+  PASCO_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) == 0, "pasco_xattn_forward: pointers must be 16-byte aligned");
+  XParams p = {};
+  p.q = q; p.k = k; p.v = v; p.mask = mask; p.lse = lse;
+  cudaStream_t st = (cudaStream_t)s;
+  const int rc = xattn_setup("pasco_xattn_forward", p, Q, P, H, D, scale, SMEM_BYTES,
+                             {(const void*)k_xattn_fwd<0>, (const void*)k_xattn_fwd<1>}, true, st);
+  if (rc != 0) return rc;
+  const int grid = p.chunks * H;
+  const int64_t n = (int64_t)Q * H * D;
   k_xattn_fwd<0><<<grid, NTHREADS, SMEM_BYTES, st>>>(p);
-  k_xattn_lse<<<(H * Q + 127) / 128, 128, 0, st>>>(workspace, p.chunks, H * Q, lse);
+  k_xattn_lse<<<(H * Q + 127) / 128, 128, 0, st>>>(p.ws, p.chunks, H * Q, lse);
   k_xattn_fwd<1><<<grid, NTHREADS, SMEM_BYTES, st>>>(p);
-  k_xattn_osum<<<grid_for((int64_t)Q * H * D, 256), 256, 0, st>>>(p.opart, p.chunks, (int64_t)Q * H * D, out);
+  k_xattn_osum<<<grid_for(n, 256), 256, 0, st>>>(p.part, p.chunks, n, out);
+  cudaFreeAsync(p.part, st);
   PASCO_CHECK_LAUNCH("pasco_xattn_forward");
   return 0;
 }
@@ -370,17 +422,6 @@ extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* 
 // every dK/dV row is written exactly once (no atomics); each chunk stores its share of dQ, k_xattn_osum adds them in order.
 // ==================================================================================================================
 namespace {
-
-struct XBwdParams {
-  const float* q; const float* k; const float* v; const uint32_t* mask; const float* lse;
-  const float* out; const float* dout;
-  float* dq; float* dk; float* dv;
-  float* dqpart;       // [chunks, Q, H*D]: this chunk's share of dQ (summed in chunk order by k_xattn_osum)
-  int Q, H, D;
-  int64_t P;
-  int chunks;
-  float scale;
-};
 
 constexpr int B_OFF_Q = 0;                          // Qs hi | lo           2 x 16 KB
 constexpr int B_OFF_DO = 2 * TILE_Q;                // dO hi | lo           2 x 16 KB
@@ -403,7 +444,7 @@ __device__ __forceinline__ void mma_t64(float (&d)[32], uint32_t a_hi, uint32_t 
   }
 }
 
-__global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant__ XBwdParams p) {
+__global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant__ XParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B_OFF_BAR);
@@ -412,83 +453,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
   float* scr = reinterpret_cast<float*>(smem + B_OFF_SCR);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int h = blockIdx.x % p.H;
-  const int chunk = blockIdx.x / p.H;
-  const int64_t n_tiles = (p.P + BK - 1) / BK;
-  const int64_t tiles_per_chunk = (n_tiles + p.chunks - 1) / p.chunks;
-  const int64_t t0 = (int64_t)chunk * tiles_per_chunk;
-  const int64_t t1 = t0 + tiles_per_chunk < n_tiles ? t0 + tiles_per_chunk : n_tiles;
-  const int64_t my_tiles = t1 > t0 ? t1 - t0 : 0;
+  const CtaTiles ct = cta_tiles(p);
+  const int h = ct.h;
   const int HD = p.H * p.D;
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(kv_full + i), 4);
-      mbar_init(smem_u32(kv_empty + i), 4);
-    }
-    fence_barrier_init();
-  }
-  // resident operands: Qs = scale*Q_h and dO_h as bf16 hi/lo [128 rows][64]
-  for (int t = threadIdx.x; t < QM * 8; t += NTHREADS) {
-    const int row = t >> 3, c = t & 7;
-    float f[8], g[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int d = c * 8 + j;
-      const bool ok = row < p.Q && d < p.D;
-      f[j] = ok ? __ldg(p.q + (int64_t)row * HD + h * p.D + d) * p.scale : 0.f;
-      g[j] = ok ? __ldg(p.dout + (int64_t)row * HD + h * p.D + d) : 0.f;
-    }
-    uint2 h0, l0, h1, l1;
-    const uint32_t off = sw_off(row, c);
-    split4(make_float4(f[0], f[1], f[2], f[3]), h0, l0);
-    split4(make_float4(f[4], f[5], f[6], f[7]), h1, l1);
-    *reinterpret_cast<uint4*>(smem + B_OFF_Q + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-    *reinterpret_cast<uint4*>(smem + B_OFF_Q + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-    split4(make_float4(g[0], g[1], g[2], g[3]), h0, l0);
-    split4(make_float4(g[4], g[5], g[6], g[7]), h1, l1);
-    *reinterpret_cast<uint4*>(smem + B_OFF_DO + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-    *reinterpret_cast<uint4*>(smem + B_OFF_DO + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-  }
+  init_kv_ring(kv_full, kv_empty);
+  stage_rows(smem + B_OFF_Q, p.q, p.scale, p, h);    // resident operands: Qs = scale*Q_h and dO_h
+  stage_rows(smem + B_OFF_DO, p.dout, 1.f, p, h);
   fence_proxy_async_smem();
   __syncthreads();
 
   if (warp >= 4) {
-    // ===================================== K / V tile gather (as forward pass 1) =====================================
-    const int gw = warp - 4;
-    const int chunk4 = lane & 15, rsub = lane >> 4;
-    uint32_t phase = 0;
-    for (int64_t it = 0; it < my_tiles; ++it) {
-      const int st = (int)(it & 1);
-      const int64_t key0 = (t0 + it) * BK;
-      float4 kv[2][8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int r = gw * 16 + i * 2 + rsub;
-        const int64_t key = key0 + r;
-        const bool ok = key < p.P && chunk4 * 4 < p.D;
-        kv[0][i] = ok ? __ldg(reinterpret_cast<const float4*>(p.k + key * HD + h * p.D + chunk4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        kv[1][i] = ok ? __ldg(reinterpret_cast<const float4*>(p.v + key * HD + h * p.D + chunk4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      mbar_wait(smem_u32(kv_empty + st), phase ^ 1);
-      uint8_t* base = smem + B_OFF_KV + st * KV_STAGE;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const uint32_t r = (uint32_t)(gw * 16 + i * 2 + rsub);
-        const uint32_t off = r * 128u + ((((uint32_t)chunk4 >> 1) ^ (r & 7u)) << 4) + (((uint32_t)chunk4 & 1u) << 3);
-        uint2 hi, lo;
-        split4(kv[0][i], hi, lo);
-        *reinterpret_cast<uint2*>(base + off) = hi;
-        *reinterpret_cast<uint2*>(base + TILE_K + off) = lo;
-        split4(kv[1][i], hi, lo);
-        *reinterpret_cast<uint2*>(base + 2 * TILE_K + off) = hi;
-        *reinterpret_cast<uint2*>(base + 3 * TILE_K + off) = lo;
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(kv_full + st));
-      if (st == 1) phase ^= 1;
-    }
+    produce_kv<true>(p, ct, smem + B_OFF_KV, kv_full, kv_empty, warp, lane);
   } else {
     // ===================================== MMA + query rows (warps 0-3) =====================================
     const int qrow = warp * 32 + lane;
@@ -505,28 +481,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
     }
     float dq[2][32];
     zero_acc(dq);
-    for (int64_t it = 0; it < my_tiles; ++it) {
+    for (int64_t it = 0; it < ct.my_tiles; ++it) {
       const int st = (int)(it & 1);
-      const int64_t key0 = (t0 + it) * BK;
-      uint32_t mbits[2] = {0xffffffffu, 0xffffffffu};
-      if (qok) {
-        if (p.mask) {
-          const uint2 w = __ldg(reinterpret_cast<const uint2*>(p.mask + ((int64_t)qrow * n_tiles + (t0 + it)) * 2));
-          mbits[0] = w.x;
-          mbits[1] = w.y;
-        } else {
-          mbits[0] = mbits[1] = 0u;
-        }
-        const int64_t left = p.P - key0;
-        if (left < 64) {
-          if (left <= 32) {
-            mbits[1] = 0xffffffffu;
-            if (left < 32) mbits[0] |= ~0u << left;
-          } else {
-            mbits[1] |= ~0u << (left - 32);
-          }
-        }
-      }
+      const int64_t key0 = (ct.t0 + it) * BK;
+      uint32_t mbits[2];
+      tile_mask_bits(mbits, p, qrow, ct.n_tiles, ct.t0 + it);
       mbar_wait(smem_u32(kv_full + st), (uint32_t)((it >> 1) & 1));
       const uint32_t k_hi = smem_u32(smem + B_OFF_KV + st * KV_STAGE), k_lo = k_hi + TILE_K;
       const uint32_t v_hi = k_hi + 2 * TILE_K, v_lo = v_hi + TILE_K;
@@ -552,16 +511,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
       }
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
-        uint2 h0, l0, h1, l1;
-        const uint32_t off = sw_off((uint32_t)qrow, (uint32_t)c);
-        split4(make_float4(pr[c * 8], pr[c * 8 + 1], pr[c * 8 + 2], pr[c * 8 + 3]), h0, l0);
-        split4(make_float4(pr[c * 8 + 4], pr[c * 8 + 5], pr[c * 8 + 6], pr[c * 8 + 7]), h1, l1);
-        *reinterpret_cast<uint4*>(smem + B_OFF_P + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-        *reinterpret_cast<uint4*>(smem + B_OFF_P + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-        split4(make_float4(ds[c * 8], ds[c * 8 + 1], ds[c * 8 + 2], ds[c * 8 + 3]), h0, l0);
-        split4(make_float4(ds[c * 8 + 4], ds[c * 8 + 5], ds[c * 8 + 6], ds[c * 8 + 7]), h1, l1);
-        *reinterpret_cast<uint4*>(smem + B_OFF_DS + off) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-        *reinterpret_cast<uint4*>(smem + B_OFF_DS + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
+        store_split8(smem + B_OFF_P, (uint32_t)qrow, (uint32_t)c, pr + c * 8);
+        store_split8(smem + B_OFF_DS, (uint32_t)qrow, (uint32_t)c, ds + c * 8);
       }
       fence_proxy_async_smem();
       named_sync(1, 128);                               // the whole P / dS tiles are written
@@ -592,7 +543,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
       float a[DP];
       acc_to_rows(dq, scr, a, warp, lane);
       if (qok) {
-        float* row = p.dqpart + ((int64_t)chunk * p.Q + qrow) * HD + h * p.D;
+        float* row = p.part + ((int64_t)ct.chunk * p.Q + qrow) * HD + h * p.D;
 #pragma unroll
         for (int d = 0; d < DP; ++d)
           if (d < p.D) row[d] = a[d] * p.scale;
@@ -606,30 +557,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
 extern "C" int pasco_xattn_backward(const float* q, const float* k, const float* v, const uint32_t* mask, const float* lse,
                                     const float* out, const float* dout, int32_t Q, int64_t P, int32_t H, int32_t D,
                                     float scale, float* dq, float* dk, float* dv, pasco_stream_t s) {
-  PASCO_CHECK_ARG(Q >= 1 && Q <= QM, "pasco_xattn_backward: Q (%d) must be in [1,128]", Q);
-  PASCO_CHECK_ARG(D >= 4 && D <= DP && D % 4 == 0, "pasco_xattn_backward: head dim (%d) must be a multiple of 4, <= 64", D);
   PASCO_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)dq | (uintptr_t)dk | (uintptr_t)dv) & 15) == 0,
                   "pasco_xattn_backward: pointers must be 16-byte aligned");
-  XBwdParams p;
-  p.q = q; p.k = k; p.v = v; p.mask = mask; p.lse = lse; p.out = out; p.dout = dout;
-  p.dq = dq; p.dk = dk; p.dv = dv;
-  p.Q = Q; p.H = H; p.D = D; p.P = P; p.scale = scale;
-  p.chunks = pick_chunks(P, H);
-  cudaError_t e = cudaFuncSetAttribute(k_xattn_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, B_SMEM_BYTES);
-  if (e != cudaSuccess) {
-    set_error("pasco_xattn_backward: cudaFuncSetAttribute(%d) failed: %s", B_SMEM_BYTES, cudaGetErrorString(e));
-    return -1;
-  }
+  XParams p = {};
+  p.q = q; p.k = k; p.v = v; p.mask = mask; p.lse = lse; p.out = out; p.dout = dout; p.dk = dk; p.dv = dv;
   cudaStream_t st = (cudaStream_t)s;
+  const int rc = xattn_setup("pasco_xattn_backward", p, Q, P, H, D, scale, B_SMEM_BYTES, {(const void*)k_xattn_bwd},
+                             false, st);
+  if (rc != 0) return rc;
   const int64_t n = (int64_t)Q * H * D;
-  e = ws_alloc((void**)&p.dqpart, (size_t)p.chunks * n * sizeof(float), st);
-  if (e != cudaSuccess) {
-    set_error("pasco_xattn_backward: workspace of %lld bytes: %s", (long long)p.chunks * n * 4, cudaGetErrorString(e));
-    return -1;
-  }
   k_xattn_bwd<<<p.chunks * H, NTHREADS, B_SMEM_BYTES, st>>>(p);
-  k_xattn_osum<<<grid_for(n, 256), 256, 0, st>>>(p.dqpart, p.chunks, n, dq);
-  cudaFreeAsync(p.dqpart, st);
+  k_xattn_osum<<<grid_for(n, 256), 256, 0, st>>>(p.part, p.chunks, n, dq);
+  cudaFreeAsync(p.part, st);
   PASCO_CHECK_LAUNCH("pasco_xattn_backward");
   return 0;
 }

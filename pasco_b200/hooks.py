@@ -9,10 +9,11 @@ PaSCo's transformer are plain torch in the reference and therefore outside that 
     [1, 100, X/s, Y/s, Z/s] volume (839 MB at scale 1) built only to be sampled at the key voxels.
 
 `install()` replaces those two methods — at run time, on the imported classes, without touching the reference's files —
-with calls into the engine: the K/V projections on the wgmma GEMM (ops.linear), the masked softmax·V as
-`pasco_xattn_forward/backward` (ops.MaskedCrossAttention: streaming two-pass softmax, bit-packed mask rows, no [Q, P]
-score volume in HBM) and the mask as a sparse max-pool + hash look-up.  Same parameters, same state_dict, same results
-within the fp32 tolerance (tests/test_dropin_reference.py runs the reference with and without the hooks).
+with calls into the engine: the attention through ops.cross_attention, which net3d's own decoder uses too (K/V
+projections on the wgmma GEMM, the masked softmax·V as `pasco_xattn_forward/backward`: streaming two-pass softmax,
+bit-packed mask rows, no [Q, P] score volume in HBM) and the mask as a sparse max-pool + hash look-up.  Same
+parameters, same state_dict, same results within the fp32 tolerance (tests/test_dropin_reference.py runs the reference
+with and without the hooks).
 
     import pasco_b200.hooks; pasco_b200.hooks.install()        # after `pasco` is importable, before building Net
     PASCO_B200_HOOKS=1 python scripts/train.py ...              # compat/MinkowskiEngine calls install() lazily
@@ -20,7 +21,6 @@ within the fp32 tolerance (tests/test_dropin_reference.py runs the reference wit
 from __future__ import annotations
 
 import torch
-import torch.nn.functional as F
 
 from . import me as ME
 from . import ops
@@ -33,20 +33,14 @@ def _cross_attention_forward(self, q_embed, bb_feat, attn_mask=None, padding_mas
     bool [B*heads, Q, P] (True = masked; the reference repeats one [Q, P] mask over the heads)."""
     if padding_mask is not None or not bb_feat.is_cuda:
         return self._pasco_b200_orig_forward(q_embed, bb_feat, attn_mask, padding_mask, pos, query_pos)
-    mha = self.multihead_attn
-    d, h = q_embed.shape[-1], mha.num_heads
+    h = self.multihead_attn.num_heads
     q_embed = self.norm(q_embed)
-    wq, wk, wv = mha.in_proj_weight.split(d, 0)
-    bq, bk, bv = mha.in_proj_bias.split(d, 0)
     outs = []
     for b in range(q_embed.shape[0]):
         qb = q_embed[b] if query_pos is None else q_embed[b] + query_pos[b]
         kv = bb_feat[b] if pos is None else bb_feat[b] + pos[b]
-        Q = F.linear(qb, wq, bq)
-        K = ops.linear(kv.contiguous(), wk, bk)                    # wgmma GEMM over all voxels
-        V = ops.linear(kv.contiguous(), wv, bv)
         m = attn_mask[b * h] if attn_mask is not None else None    # all heads of an item share one mask
-        outs.append(mha.out_proj(ops.MaskedCrossAttention.apply(Q, K, V, m, h)))
+        outs.append(ops.cross_attention(self.multihead_attn, qb, kv, m))
     return q_embed + self.dropout(torch.stack(outs, 0))
 
 

@@ -775,8 +775,11 @@ def pack_mask_bits(mask: torch.Tensor) -> torch.Tensor:
 
 class MaskedCrossAttention(torch.autograd.Function):
     """out[q] = concat_h softmax_v(scale·q_h·k_h[v] | mask[q,v]) · v_h[v]  — blocks.py:73-92 with the mask of
-    transformer_predictor_v2.py:220-289.  Forward: two streaming wgmma passes; backward: one streaming pass with
-    five wgmma GEMMs per 64-key tile that recomputes the probabilities from the saved log-sum-exp (xattn.cu)."""
+    transformer_predictor_v2.py:220-289.  q [Q, H*D] with Q <= 128, k / v [P, H*D], D <= 64 and a multiple of 4,
+    mask bool [Q, P] (True = masked) or None.  Forward: two streaming wgmma passes (row statistics, then output);
+    backward: one streaming pass with five wgmma GEMMs per 64-key tile that recomputes the probabilities from the
+    saved log-sum-exp (xattn.cu).  Each pass splits the keys into chunks whose shares of out / dq are added in a fixed
+    order; the per-chunk scratch comes from the library's own stream-ordered pool."""
 
     @staticmethod
     def forward(ctx, q, k, v, mask, heads: int):
@@ -788,10 +791,8 @@ class MaskedCrossAttention(torch.autograd.Function):
         bits = pack_mask_bits(mask) if mask is not None else None
         out = torch.zeros(Q, HD, dtype=torch.float32, device=q.device)
         lse = torch.empty(heads, Q, dtype=torch.float32, device=q.device)
-        nbytes = _lib.load().pasco_xattn_workspace_bytes(Q, P, heads, D)
-        ws = torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=q.device)
         call("pasco_xattn_forward", ptr(q), ptr(k), ptr(v), ptr(bits), Q, P, heads, D, C.c_float(scale), ptr(out),
-             ptr(lse), ptr(ws), nbytes)
+             ptr(lse))
         ctx.save_for_backward(q, k, v, bits, out, lse)
         ctx.heads, ctx.scale = heads, scale
         return out
@@ -808,6 +809,20 @@ class MaskedCrossAttention(torch.autograd.Function):
         call("pasco_xattn_backward", ptr(q), ptr(k), ptr(v), ptr(bits), ptr(lse), ptr(out), ptr(go), Q, P, H, HD // H,
              C.c_float(scale), ptr(dq), ptr(dk), ptr(dv))
         return dq, dk, dv, None, None
+
+
+def cross_attention(mha: torch.nn.MultiheadAttention, q: torch.Tensor, kv: torch.Tensor,
+                    mask: Optional[torch.Tensor]) -> torch.Tensor:
+    """`mha(q, kv, kv, attn_mask=mask)` of blocks.py:73-92 for one scene: q [Q, d] (query position already added),
+    kv [P, d] (key position already added), mask bool [Q, P] (True = masked) or None → [Q, d].  The K / V projections
+    over all voxels run on the wgmma GEMM, the masked softmax·V on MaskedCrossAttention."""
+    d = q.shape[-1]
+    wq, wk, wv = mha.in_proj_weight.split(d, 0)
+    bq, bk, bv = mha.in_proj_bias.split(d, 0)
+    kv = kv.contiguous()
+    o = MaskedCrossAttention.apply(torch.nn.functional.linear(q, wq, bq), linear(kv, wk, bk), linear(kv, wv, bv), mask,
+                                   mha.num_heads)
+    return mha.out_proj(o)
 
 
 # ----------------------------------------------------------------------------------------------

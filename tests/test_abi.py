@@ -35,8 +35,8 @@ def test_header_symbols_are_exported_and_typed(lib):
     assert sorted(_lib.PROTOTYPES) == names, "ctypes prototypes and header disagree"
 
 
-def test_abi_version_2_and_error_string(lib):
-    assert lib.pasco_abi_version() == 2
+def test_abi_version_3_and_error_string(lib):
+    assert lib.pasco_abi_version() == 3
     assert isinstance(lib.pasco_last_error(), bytes)
     assert lib.pasco_conv_packed_bytes(27, 64, 64) == 27 * 64 * 64 * 4
 

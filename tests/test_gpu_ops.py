@@ -512,10 +512,13 @@ def test_linear_tensor_core_matches_fp64(ME, n, cin, cout, bias):
 # ------------------------------------------------------------------------------------------------
 # masked cross-attention kernel
 # ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("P,Q,masked", [(3000, 100, True), (64, 100, True), (37, 5, False), (20011, 100, True)])
-def test_masked_cross_attention_matches_reference(ME, P, Q, masked):
+@pytest.mark.parametrize("P,Q,H,D,masked", [
+    (3000, 100, 8, 48, True), (64, 100, 8, 48, True), (37, 5, 8, 48, False), (20011, 100, 8, 48, True),
+    (3000, 128, 6, 64, True),          # no query or head-dim padding
+    (1000, 100, 4, 20, True),          # a head that ends inside a 16-byte chunk of the bf16 operand tiles
+])
+def test_masked_cross_attention_matches_reference(ME, P, Q, H, D, masked):
     from pasco_b200 import ops
-    H, D = 8, 48
     g = torch.Generator().manual_seed(P)
     q, k, v = (torch.randn(n, H * D, generator=g) for n in (Q, P, P))
     mask = None
@@ -541,7 +544,7 @@ def test_masked_cross_attention_matches_reference(ME, P, Q, masked):
     (yg * up.cuda()).sum().backward()
     e = relerr(yg, yr)
     eg = max(relerr(qg.grad, qr.grad), relerr(kg.grad, kr.grad), relerr(vg.grad, vr.grad))
-    print(f"xattn P={P} Q={Q}: fwd {e:.2e} grads {eg:.2e}")
+    print(f"xattn P={P} Q={Q} H={H} D={D}: fwd {e:.2e} grads {eg:.2e}")
     assert e <= 1e-4 and eg <= 5e-4      # backward = fp32 library GEMMs against an fp64 reference
 
 
