@@ -219,7 +219,8 @@ int pasco_bn_bwd_apply(const float* dy, const float* x, int64_t n, int32_t C, co
                        const float* coef_c, float* dx, pasco_stream_t s);
 
 /* ---- MaskPLS masked cross-attention (pasco/models/transformer/blocks.py:73-92 with the attention mask of
- *      transformer_predictor_v2.py:220-289): Q <= 128 queries against all P voxels, H heads of width D <= 64 ------
+ *      transformer_predictor_v2.py:220-289): Q queries against all P voxels, H heads of width D <= 64 ----------
+ * Any Q >= 1: the kernels work in blocks of 128 queries and stream K and V once per block (Q <= 128 is one block).
  * q [Q, H*D], k / v [P, H*D] float32 (already projected); logits = scale * q.k; mask = bit rows
  * uint32 [Q, 2*ceil(P/64)] (bit j of word 2t + j/32 set = key 64t + j masked) or NULL; out [Q, H*D] is overwritten
  * (the key chunks' shares are summed in a fixed order); lse [H, Q] receives log-sum-exp per row (needed by the
@@ -227,7 +228,8 @@ int pasco_bn_bwd_apply(const float* dy, const float* x, int64_t n, int32_t C, co
 int pasco_xattn_forward(const float* q, const float* k, const float* v, const uint32_t* mask, int32_t Q, int64_t P,
                         int32_t H, int32_t D, float scale, float* out, float* lse, pasco_stream_t s);
 /* backward of the above: recomputes the probabilities from lse; dq [Q, H*D] is overwritten (chunk shares, fixed order),
- * dk / dv [P, H*D] are fully overwritten (every row written exactly once, no atomics).                            */
+ * dk / dv [P, H*D] are fully overwritten (no atomics; at Q > 128 the query blocks' partials are added in block order,
+ * through a workspace of (ceil(Q/128) - 1) * 2 * P * H * D floats from the library's pool).                       */
 int pasco_xattn_backward(const float* q, const float* k, const float* v, const uint32_t* mask, const float* lse,
                          const float* out, const float* dout, int32_t Q, int64_t P, int32_t H, int32_t D, float scale,
                          float* dq, float* dk, float* dv, pasco_stream_t s);

@@ -1,4 +1,4 @@
-// Masked cross-attention of a handful of queries (≤128) over ALL voxels of a scale, sm_90a (wgmma).
+// Masked cross-attention of a few hundred queries over ALL voxels of a scale, sm_90a (wgmma).
 //
 //   O[q, h, :] = Σ_v softmax_v( Q[q,h,:]·K[v,h,:]·scale + mask[q,v] ) · V[v,h,:]
 //
@@ -14,7 +14,8 @@
 //           V tile as MN-major B operand), accumulated in registers over all tiles of the CTA; `k_xattn_osum` adds
 //           the chunks' shares in chunk order (deterministic: the attention mask of the next layer thresholds O-derived
 //           logits, so run-to-run rounding differences could flip mask bits).
-// A CTA = (head, key chunk); warps 0-3 (one warpgroup): issue the MMAs, pass each result through a [64 col][128 row]
+// A CTA = (query block of 128 rows, head, key chunk); Q <= 128 is one query block, and each further block of 128 queries
+// streams K and V once more.  Warps 0-3 (one warpgroup): issue the MMAs, pass each result through a [64 col][128 row]
 // fp32 scratch so that thread t then holds query row t (mask, exp, row statistics); warps 4-7: K/V tile gather (16
 // lanes per 256-byte padded row segment, fp32 → bf16 hi/lo split, 128-byte swizzle).  Operands are split bf16x3 like
 // the convolution ("fp32" mode).  The backward (below) shares the CTAs, the warp roles, the K/V producer, the operand
@@ -30,7 +31,7 @@ using namespace gmma;
 namespace {
 
 constexpr int BK = 64;                      // keys per tile
-constexpr int QM = 128;                     // query rows (padded) = 2 x wgmma M
+constexpr int QM = 128;                     // query rows of a query block (padded) = 2 x wgmma M
 constexpr int DP = 64;                      // padded head dim = one 128-byte swizzle row of bf16
 constexpr int TILE_Q = QM * 128;            // 16 KB: [128 rows][64] bf16
 constexpr int TILE_K = BK * 128;            // 8 KB : [64 keys][64] bf16
@@ -50,6 +51,7 @@ struct XParams {
   float* dv;            // [P, H*D]          (backward)
   float* ws;            // [chunks, H, Q, 2] (forward pass 0: row statistics of each chunk)
   float* part;          // [chunks, Q, H*D]  (this chunk's share of O in forward pass 1, of dQ in the backward)
+  float* dkv;           // [nqb-1, 2, P, H*D] (backward, Q > 128: dK then dV of query blocks 1..; block 0 writes dk, dv)
   int Q, H, D;
   int64_t P;
   int chunks;
@@ -105,13 +107,16 @@ __device__ __forceinline__ void acc_to_rows(const float (&d)[2][32], float* scr,
   for (int j = 0; j < 64; ++j) v[j] = scr[j * QM + row];
 }
 
-// this CTA's head, key chunk, and its key tiles [t0, t0 + my_tiles) out of the n_tiles that cover P
+// this CTA's query block (rows [q0, q0 + 128) of Q), head, key chunk, and its key tiles [t0, t0 + my_tiles) out of the
+// n_tiles that cover P
 struct CtaTiles {
-  int h, chunk;
+  int qb, q0, h, chunk;
   int64_t n_tiles, t0, my_tiles;
 };
 __device__ __forceinline__ CtaTiles cta_tiles(const XParams& p) {
   CtaTiles c;
+  c.qb = blockIdx.y;
+  c.q0 = c.qb * QM;
   c.h = blockIdx.x % p.H;
   c.chunk = blockIdx.x / p.H;
   c.n_tiles = (p.P + BK - 1) / BK;
@@ -143,9 +148,9 @@ __device__ __forceinline__ void store_split8(uint8_t* tile, uint32_t row, uint32
   *reinterpret_cast<uint4*>(tile + TILE_Q + off) = make_uint4(l0.x, l0.y, l1.x, l1.y);
 }
 
-// resident operand, all threads: head h's columns of the [Q, H*D] matrix `src` times `factor` → bf16 hi / lo
-// [128 rows][64] at `tile`; rows >= Q and columns >= D are zero
-__device__ __forceinline__ void stage_rows(uint8_t* tile, const float* src, float factor, const XParams& p, int h) {
+// resident operand, all threads: head h's columns of rows [q0, q0 + 128) of the [Q, H*D] matrix `src` times `factor`
+// → bf16 hi / lo [128 rows][64] at `tile`; rows >= Q and columns >= D are zero
+__device__ __forceinline__ void stage_rows(uint8_t* tile, const float* src, float factor, const XParams& p, int q0, int h) {
   const int HD = p.H * p.D;
   for (int t = threadIdx.x; t < QM * 8; t += NTHREADS) {       // one 16-byte output chunk (8 bf16) per iteration
     const int row = t >> 3, c = t & 7;
@@ -153,7 +158,7 @@ __device__ __forceinline__ void stage_rows(uint8_t* tile, const float* src, floa
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int d = c * 8 + j;
-      f[j] = (row < p.Q && d < p.D) ? __ldg(src + (int64_t)row * HD + h * p.D + d) * factor : 0.f;
+      f[j] = (q0 + row < p.Q && d < p.D) ? __ldg(src + (int64_t)(q0 + row) * HD + h * p.D + d) * factor : 0.f;
     }
     store_split8(tile, row, c, f);
   }
@@ -203,7 +208,7 @@ __device__ __forceinline__ void produce_kv(const XParams& p, const CtaTiles& ct,
   }
 }
 
-// mask bits of query row `qrow` for the 64 keys of `tile` (bit set = masked); keys >= P and rows >= Q are masked
+// mask bits of (global) query row `qrow` for the 64 keys of `tile` (bit set = masked); keys >= P and rows >= Q are masked
 __device__ __forceinline__ void tile_mask_bits(uint32_t (&mbits)[2], const XParams& p, int qrow, int64_t n_tiles,
                                                int64_t tile) {
   mbits[0] = mbits[1] = 0xffffffffu;
@@ -241,7 +246,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
   const int HD = p.H * p.D;
 
   init_kv_ring(kv_full, kv_empty);
-  stage_rows(smem + OFF_Q, p.q, p.scale, p, h);      // resident query operand Q_h * scale
+  stage_rows(smem + OFF_Q, p.q, p.scale, p, ct.q0, h);   // resident query operand Q_h * scale
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -249,7 +254,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
     produce_kv<PASS == 1>(p, ct, smem + OFF_KV, kv_full, kv_empty, warp, lane);
   } else {
     // ===================================== MMA + softmax rows (warps 0-3) =====================================
-    const int qrow = warp * 32 + lane;
+    const int row = warp * 32 + lane, qrow = ct.q0 + row;    // tile row, query row
     const bool qok = qrow < p.Q;
     const uint32_t q_hi = smem_u32(smem + OFF_Q), q_lo = q_hi + TILE_Q;
     const uint32_t p_hi = smem_u32(smem + OFF_P), p_lo = p_hi + TILE_Q;
@@ -297,7 +302,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_fwd(const __grid_constant
             const int col = c * 8 + j;
             f[j] = ((mbits[col >> 5] >> (col & 31)) & 1u) ? 0.f : __expf(s[col] - my_lse);
           }
-          store_split8(smem + OFF_P, (uint32_t)qrow, (uint32_t)c, f);
+          store_split8(smem + OFF_P, (uint32_t)row, (uint32_t)c, f);
         }
         fence_proxy_async_smem();
         named_sync(1, 128);                 // the whole P tile is written
@@ -351,24 +356,42 @@ __global__ void k_xattn_osum(const float* __restrict__ opart, int chunks, int64_
   }
 }
 
-int pick_chunks(int64_t P, int H) {
+// dk[i] (i < n) / dv[i - n] (i >= n) += dkv[b, i] for the query blocks b = 1.. in block order; n is a multiple of 4
+__global__ void k_xattn_dkv_sum(const float4* __restrict__ dkv, int parts, int64_t n, float4* __restrict__ dk,
+                                float4* __restrict__ dv) {
+  const int64_t n4 = n / 4;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < 2 * n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4* dst = i < n4 ? dk + i : dv + (i - n4);
+    float4 acc = *dst;
+    for (int b = 0; b < parts; ++b) {
+      const float4 w = __ldg(dkv + b * 2 * n4 + i);
+      acc.x += w.x; acc.y += w.y; acc.z += w.z; acc.w += w.w;
+    }
+    *dst = acc;
+  }
+}
+
+// key chunks per (query block, head): ~one CTA per SM over the nqb x H x chunks grid
+int pick_chunks(int64_t P, int H, int nqb) {
   int64_t tiles = (P + BK - 1) / BK;
-  int c = (num_sms() + H - 1) / H;        // ~one CTA per SM
+  int c = (num_sms() + H * nqb - 1) / (H * nqb);
   if (c > tiles) c = (int)tiles;
   return c < 1 ? 1 : c;
 }
 
 // What both entry points do before their launches: check the shape, fill in the shape fields and the chunk count of
-// `p`, opt the kernels in to `smem` bytes of shared memory, and take the chunks' shares `part` [chunks, Q, H*D] (with
-// row_stats, the forward's `ws` [chunks, H, Q, 2] behind them) from the library's stream-ordered pool.  The caller
-// frees p.part on the same stream after its launches.
+// `p`, opt the kernels in to `smem` bytes of shared memory, and take the chunks' shares `part` [chunks, Q, H*D] from the
+// library's stream-ordered pool.  Behind them lie the forward's row statistics `ws` [chunks, H, Q, 2], or for the
+// backward at Q > 128 the dK / dV partials `dkv` [nqb-1, 2, P, H*D].  Returns the number of query blocks nqb (< 0 on
+// error); the caller frees p.part on the same stream after its launches.
 int xattn_setup(const char* fn, XParams& p, int32_t Q, int64_t P, int32_t H, int32_t D, float scale, int smem,
-                std::initializer_list<const void*> kernels, bool row_stats, cudaStream_t st) {
-  PASCO_CHECK_ARG(Q >= 1 && Q <= QM, "%s: Q (%d) must be in [1,128]", fn, Q);
+                std::initializer_list<const void*> kernels, bool forward, cudaStream_t st) {
+  PASCO_CHECK_ARG(Q >= 1 && Q <= 65535 * QM, "%s: Q (%d) must be in [1,%d]", fn, Q, 65535 * QM);
   PASCO_CHECK_ARG(D >= 4 && D <= DP && D % 4 == 0, "%s: head dim (%d) must be a multiple of 4, <= 64", fn, D);
   PASCO_CHECK_ARG(H >= 1 && P >= 1, "%s: bad shape (H = %d, P = %lld)", fn, H, (long long)P);
   p.Q = Q; p.H = H; p.D = D; p.P = P; p.scale = scale;
-  p.chunks = pick_chunks(P, H);
+  const int nqb = (Q + QM - 1) / QM;
+  p.chunks = pick_chunks(P, H, nqb);
   for (const void* k : kernels) {
     const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) {
@@ -376,14 +399,16 @@ int xattn_setup(const char* fn, XParams& p, int32_t Q, int64_t P, int32_t H, int
       return -1;
     }
   }
-  const int64_t n = (int64_t)p.chunks * Q * H * D, stats = row_stats ? (int64_t)p.chunks * H * Q * 2 : 0;
-  const cudaError_t e = ws_alloc((void**)&p.part, (size_t)(n + stats) * sizeof(float), st);
+  const int64_t n = (int64_t)p.chunks * Q * H * D;
+  const int64_t extra = forward ? (int64_t)p.chunks * H * Q * 2 : (int64_t)(nqb - 1) * 2 * P * H * D;
+  const cudaError_t e = ws_alloc((void**)&p.part, (size_t)(n + extra) * sizeof(float), st);
   if (e != cudaSuccess) {
-    set_error("%s: workspace of %lld bytes: %s", fn, (long long)(n + stats) * 4, cudaGetErrorString(e));
+    set_error("%s: workspace of %lld bytes: %s", fn, (long long)(n + extra) * 4, cudaGetErrorString(e));
     return -1;
   }
-  p.ws = row_stats ? p.part + n : nullptr;
-  return 0;
+  p.ws = forward ? p.part + n : nullptr;
+  p.dkv = !forward && nqb > 1 ? p.part + n : nullptr;
+  return nqb;
 }
 
 }  // namespace
@@ -395,10 +420,10 @@ extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* 
   XParams p = {};
   p.q = q; p.k = k; p.v = v; p.mask = mask; p.lse = lse;
   cudaStream_t st = (cudaStream_t)s;
-  const int rc = xattn_setup("pasco_xattn_forward", p, Q, P, H, D, scale, SMEM_BYTES,
-                             {(const void*)k_xattn_fwd<0>, (const void*)k_xattn_fwd<1>}, true, st);
-  if (rc != 0) return rc;
-  const int grid = p.chunks * H;
+  const int nqb = xattn_setup("pasco_xattn_forward", p, Q, P, H, D, scale, SMEM_BYTES,
+                              {(const void*)k_xattn_fwd<0>, (const void*)k_xattn_fwd<1>}, true, st);
+  if (nqb < 0) return nqb;
+  const dim3 grid(p.chunks * H, nqb);
   const int64_t n = (int64_t)Q * H * D;
   k_xattn_fwd<0><<<grid, NTHREADS, SMEM_BYTES, st>>>(p);
   k_xattn_lse<<<(H * Q + 127) / 128, 128, 0, st>>>(p.ws, p.chunks, H * Q, lse);
@@ -415,11 +440,14 @@ extern "C" int pasco_xattn_forward(const float* q, const float* k, const float* 
 //   P = exp(S − lse) (masked → 0),  dP = dO·Vᵀ,  dS = P ∘ (dP − rowsum(dO ∘ O)),
 //   dV = Pᵀ·dO,  dK = dSᵀ·Qs,  dQ = scale · dS·K                       (Qs = scale·Q)
 //
-// Same CTA = (head, key chunk) decomposition, warp roles and 64-key tiles as the forward.  Five wgmma GEMMs per tile:
+// Same CTA = (query block, head, key chunk) decomposition, warp roles and 64-key tiles as the forward.  Five wgmma GEMMs
+// per tile:
 //   S  [128q x 64k] = Qs(K-major) · K(K-major)            dP [128q x 64k] = dO(K-major) · V(K-major)
 //   dVᵀ[ 64d x 64k] = dOᵀ(MN-major) · P(MN-major)          dKᵀ[ 64d x 64k] = Qsᵀ(MN-major) · dS(MN-major)
 //   dQ [128q x 64d] += dS(K-major) · K(MN-major)              (accumulates in registers over the CTA's tiles)
-// every dK/dV row is written exactly once (no atomics); each chunk stores its share of dQ, k_xattn_osum adds them in order.
+// every dK/dV row is written exactly once per query block (no atomics): block 0 into dk / dv, blocks 1.. into a workspace
+// that k_xattn_dkv_sum adds to dk / dv in block order.  Each (block, chunk) stores its share of dQ, k_xattn_osum adds
+// the chunks' shares in order.
 // ==================================================================================================================
 namespace {
 
@@ -458,8 +486,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
   const int HD = p.H * p.D;
 
   init_kv_ring(kv_full, kv_empty);
-  stage_rows(smem + B_OFF_Q, p.q, p.scale, p, h);    // resident operands: Qs = scale*Q_h and dO_h
-  stage_rows(smem + B_OFF_DO, p.dout, 1.f, p, h);
+  stage_rows(smem + B_OFF_Q, p.q, p.scale, p, ct.q0, h);    // resident operands: Qs = scale*Q_h and dO_h
+  stage_rows(smem + B_OFF_DO, p.dout, 1.f, p, ct.q0, h);
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -467,7 +495,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
     produce_kv<true>(p, ct, smem + B_OFF_KV, kv_full, kv_empty, warp, lane);
   } else {
     // ===================================== MMA + query rows (warps 0-3) =====================================
-    const int qrow = warp * 32 + lane;
+    const int row = warp * 32 + lane, qrow = ct.q0 + row;    // tile row, query row
     const bool qok = qrow < p.Q;
     const uint32_t q_hi = smem_u32(smem + B_OFF_Q), q_lo = q_hi + TILE_Q;
     const uint32_t o_hi = smem_u32(smem + B_OFF_DO), o_lo = o_hi + TILE_Q;
@@ -479,6 +507,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
       for (int d = 0; d < p.D; ++d)
         my_delta += __ldg(p.dout + (int64_t)qrow * HD + h * p.D + d) * __ldg(p.out + (int64_t)qrow * HD + h * p.D + d);
     }
+    // query block 0 writes its dK / dV straight into dk / dv, blocks 1.. their partials into p.dkv
+    float* dk = ct.qb == 0 ? p.dk : p.dkv + (int64_t)(ct.qb - 1) * 2 * p.P * HD;
+    float* dv = ct.qb == 0 ? p.dv : dk + p.P * HD;
     float dq[2][32];
     zero_acc(dq);
     for (int64_t it = 0; it < ct.my_tiles; ++it) {
@@ -511,8 +542,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
       }
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
-        store_split8(smem + B_OFF_P, (uint32_t)qrow, (uint32_t)c, pr + c * 8);
-        store_split8(smem + B_OFF_DS, (uint32_t)qrow, (uint32_t)c, ds + c * 8);
+        store_split8(smem + B_OFF_P, (uint32_t)row, (uint32_t)c, pr + c * 8);
+        store_split8(smem + B_OFF_DS, (uint32_t)row, (uint32_t)c, ds + c * 8);
       }
       fence_proxy_async_smem();
       named_sync(1, 128);                               // the whole P / dS tiles are written
@@ -533,8 +564,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_xattn_bwd(const __grid_constant
           const int d = frag_row(i, warp, lane);
           const int64_t key = key0 + frag_col(i, lane);
           if (d < p.D && key < p.P) {
-            p.dv[key * HD + h * p.D + d] = dvt[i];
-            p.dk[key * HD + h * p.D + d] = dkt[i];
+            dv[key * HD + h * p.D + d] = dvt[i];
+            dk[key * HD + h * p.D + d] = dkt[i];
           }
         }
       }
@@ -562,12 +593,17 @@ extern "C" int pasco_xattn_backward(const float* q, const float* k, const float*
   XParams p = {};
   p.q = q; p.k = k; p.v = v; p.mask = mask; p.lse = lse; p.out = out; p.dout = dout; p.dk = dk; p.dv = dv;
   cudaStream_t st = (cudaStream_t)s;
-  const int rc = xattn_setup("pasco_xattn_backward", p, Q, P, H, D, scale, B_SMEM_BYTES, {(const void*)k_xattn_bwd},
-                             false, st);
-  if (rc != 0) return rc;
+  const int nqb = xattn_setup("pasco_xattn_backward", p, Q, P, H, D, scale, B_SMEM_BYTES, {(const void*)k_xattn_bwd},
+                              false, st);
+  if (nqb < 0) return nqb;
   const int64_t n = (int64_t)Q * H * D;
-  k_xattn_bwd<<<p.chunks * H, NTHREADS, B_SMEM_BYTES, st>>>(p);
+  k_xattn_bwd<<<dim3(p.chunks * H, nqb), NTHREADS, B_SMEM_BYTES, st>>>(p);
   k_xattn_osum<<<grid_for(n, 256), 256, 0, st>>>(p.part, p.chunks, n, dq);
+  if (nqb > 1) {
+    const int64_t nkv = P * H * D;
+    k_xattn_dkv_sum<<<grid_for(2 * nkv / 4, 256), 256, 0, st>>>((const float4*)p.dkv, nqb - 1, nkv, (float4*)dk,
+                                                                 (float4*)dv);
+  }
   cudaFreeAsync(p.part, st);
   PASCO_CHECK_LAUNCH("pasco_xattn_backward");
   return 0;

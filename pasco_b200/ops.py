@@ -775,11 +775,14 @@ def pack_mask_bits(mask: torch.Tensor) -> torch.Tensor:
 
 class MaskedCrossAttention(torch.autograd.Function):
     """out[q] = concat_h softmax_v(scale·q_h·k_h[v] | mask[q,v]) · v_h[v]  — blocks.py:73-92 with the mask of
-    transformer_predictor_v2.py:220-289.  q [Q, H*D] with Q <= 128, k / v [P, H*D], D <= 64 and a multiple of 4,
+    transformer_predictor_v2.py:220-289.  q [Q, H*D] with any Q >= 1, k / v [P, H*D], D <= 64 and a multiple of 4,
     mask bool [Q, P] (True = masked) or None.  Forward: two streaming wgmma passes (row statistics, then output);
     backward: one streaming pass with five wgmma GEMMs per 64-key tile that recomputes the probabilities from the
     saved log-sum-exp (xattn.cu).  Each pass splits the keys into chunks whose shares of out / dq are added in a fixed
-    order; the per-chunk scratch comes from the library's own stream-ordered pool."""
+    order; the per-chunk scratch comes from the library's own stream-ordered pool.  The kernels hold 128 queries at a
+    time: above 128 every block of 128 queries streams K and V again, and the backward adds the blocks' dk / dv
+    partials in block order (a workspace of (ceil(Q/128) - 1) * 2 * P * H*D floats), so results stay run-to-run
+    identical."""
 
     @staticmethod
     def forward(ctx, q, k, v, mask, heads: int):
