@@ -127,11 +127,14 @@ int pasco_dense_occupancy(const float* dense, int32_t B, int32_t C, int64_t cell
  * Tensor-core path (wgmma, bf16 split operands, fp32 accumulate in registers):
  *   precision 1 = bf16 operands (1 MMA / k-step), 3 = bf16x3 split (hi·hi + lo·hi + hi·lo,
  *   ~2^-16 relative: the "fp32" mode of BASELINE.json configs[1]).
- *   Requires Cin % 64 == 0, Cout % 16 == 0, 16 <= Cout <= 256.
+ *   Requires Cin % 16 == 0 (Cin >= 16), Cout % 16 == 0, 16 <= Cout <= 512 (forward, input gradient, planes and weight
+ *   gradient alike).  The contraction runs in blocks of 64 channels; a last block past Cin is zero-padded in the
+ *   kernels and never read from memory.
  * Weights are first packed into the swizzled shared-memory operand image:
  *   transpose=0: B[n=co][k=ci] = W[k][ci][co]      (forward)
  *   transpose=1: B[n=ci][k=co] = W[k][ci][co]      (input gradient; swap Cin/Cout in the conv call)
- * packed size in bytes = pasco_conv_packed_bytes(K, Cin, Cout).                                 */
+ * packed size in bytes = pasco_conv_packed_bytes(K, Cin, Cout): K x Cout x Cin x 4 with the contraction rounded up to
+ * a multiple of 64, large enough for either transpose (= K * Cin * Cout * 4 when both are multiples of 64).         */
 int64_t pasco_conv_packed_bytes(int32_t K, int32_t Cin, int32_t Cout);
 int pasco_conv_pack_weights(const float* W, int32_t K, int32_t Cin, int32_t Cout, int32_t transpose, void* packed,
                             pasco_stream_t s);
@@ -161,7 +164,8 @@ int pasco_conv_forward_splitk(const float* in, int64_t n_in, const int32_t* nbr,
  * planes x = hi + lo (lo = NULL for precision 1) by pasco_split_planes — optionally fused with y = act(x*scale + shift),
  * the BatchNorm + activation of the producing layer — and the convolution / weight-gradient producers move plane rows
  * with 16-byte cp.async copies straight into the swizzled operand tiles (missing neighbours are zero-fill copies that touch
- * no memory).  Planes are bf16 [N, C] with a row pitch in ELEMENTS (0 = C); C % 8 == 0.
+ * no memory).  Planes are bf16 [N, C] with a row pitch in ELEMENTS (0 = C); C % 8 == 0.  The convolutions read only the
+ * C channels of a row: channels past C up to the next multiple of 64 are zero-fill copies.
  * pasco_conv_forward_planes: forward and input gradient (same contract as pasco_conv_forward_tc: koff_map, bias, fused
  * BatchNorm statistics of `out` in `stats`);  pasco_conv_wgrad_planes: dW (zeroed by the caller) from the planes of the
  * layer input and of the output gradient.                                                                          */
@@ -175,7 +179,8 @@ int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int64_t n_in, 
                             int64_t n_out, int32_t Cin, int32_t Cout, const void* g_hi, const void* g_lo, float* dW,
                             int32_t precision, int64_t in_pitch, int64_t gout_pitch, pasco_stream_t s);
 
-/* dW[k] = sum_o in[nbr[k,o],:]^T @ gout[o,:]   (wgmma, MN-major operands); dW float32 [K,Cin,Cout] zeroed by caller */
+/* dW[k] = sum_o in[nbr[k,o],:]^T @ gout[o,:]   (wgmma, MN-major operands); dW float32 [K,Cin,Cout] zeroed by caller.
+ * Cin % 16 == 0, Cout % 16 == 0, Cout <= 512 (this function and pasco_conv_wgrad_planes).                         */
 int pasco_conv_wgrad_tc(const float* in, int64_t n_in, const int32_t* nbr, int32_t K, int64_t n_out, int32_t Cin,
                         int32_t Cout, const float* gout, float* dW, int32_t precision, int64_t in_pitch,
                         int64_t gout_pitch, pasco_stream_t s);

@@ -1,6 +1,6 @@
 // CUDA-core fp32 path of the sparse-conv contraction  out[o,:] = Σ_k in[nbr[k,o],:] @ W[k].
 // Any Cin/Cout.  This is the in-library cross-check for the tensor-core path (conv_tc.cu) and serves the
-// shapes the tensor-core kernel does not take (channel counts that are not multiples of 64/16).
+// shapes the tensor-core kernels do not take (channel counts that are not multiples of 16, or more than 512 outputs).
 #include "common.cuh"
 
 using namespace pasco;

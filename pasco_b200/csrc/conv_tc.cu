@@ -5,7 +5,9 @@
 // One persistent CTA per SM walks work items of 128-row output tiles.  A work item is a GROUP of T consecutive tiles
 // (T x the item's columns <= 128 accumulator columns) and walks offset k → 64-channel block → tile, so every weight
 // slice W[k] is fetched from L2 once per group instead of once per tile.  Outputs wider than 128 channels are cut into
-// column ranges, one work item each.  Warp roles:
+// up to four column ranges of 128 (the last one may be narrower), one work item each.  Cin and Cout are multiples of 16;
+// the 64-channel operand blocks keep their layout when Cin is not a multiple of 64: the channels of the last block past
+// Cin are zeros in A (zero-fill copies / zero stores) and in the packed weights.  Warp roles:
 //   warps 0-7   gather: load the neighbour rows of a tile (coalesced 16-byte loads, 16 lanes per 256-byte row
 //               segment; neighbour indices arrive through a cp.async ring one offset ahead), split fp32 → bf16
 //               hi (+ lo), and store the 128x64 tile into shared memory in the 128-byte-swizzled K-major layout.
@@ -48,6 +50,7 @@ constexpr int LOADS_PER_SLOT = ROWS_PER_WARP / 2;               // float4 per la
 constexpr int TILES_PER_IDX_STEP = 32 / ROWS_PER_WARP;          // tiles whose indices one warp-wide cp.async covers
 constexpr int MAX_STAGES = 8;
 constexpr int ACC_COLS = 128;               // accumulator columns per consumer warpgroup (64 fp32 registers per thread)
+constexpr int MAX_COUT = 4 * ACC_COLS;      // output channels: at most four column ranges
 
 struct ConvParams {
   const float* in;     // k_conv_tc: the fp32 input rows
@@ -73,13 +76,15 @@ struct ConvParams {
 };
 
 // ------------------------------------------------------------------------------------------------------------
-// weight packing: fp32 [K, Cin, Cout] → per (k, kb): [hi image | lo image], image = N rows x 128 B, swizzled
+// weight packing: fp32 [K, Cin, Cout] → per (k, kb): [hi image | lo image], image = N rows x 128 B, swizzled.  The
+// contraction is cut into ceil(Kc / 64) blocks; in the last block of a contraction that is not a multiple of 64 the
+// channels past Kc are packed as zeros.
 // ------------------------------------------------------------------------------------------------------------
 __global__ void k_pack_weights(const float* __restrict__ W, int K, int Cin, int Cout, int transpose,
                                uint8_t* __restrict__ packed) {
   const int N = transpose ? Cin : Cout;   // B rows
   const int Kc = transpose ? Cout : Cin;  // contraction length
-  const int KB = Kc / KBLK;
+  const int KB = (Kc + KBLK - 1) / KBLK;
   int64_t total = (int64_t)K * KB * N * 8;  // one thread per 16-byte chunk (8 bf16)
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     int c = (int)(t & 7);
@@ -92,7 +97,7 @@ __global__ void k_pack_weights(const float* __restrict__ W, int K, int Cin, int 
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       int kc = kb * KBLK + c * 8 + j;
-      v[j] = transpose ? __ldg(W + ((int64_t)k * Cin + n) * Cout + kc) : __ldg(W + ((int64_t)k * Cin + kc) * Cout + n);
+      v[j] = kc >= Kc ? 0.f : transpose ? __ldg(W + ((int64_t)k * Cin + n) * Cout + kc) : __ldg(W + ((int64_t)k * Cin + kc) * Cout + n);
     }
     uint4 hi, lo;
     uint2 h0, l0, h1, l1;
@@ -156,7 +161,7 @@ __device__ __forceinline__ Pipe pipe_setup(const ConvParams& p, uint8_t* smem_ra
   pl.bfull = bars + 2 * MAX_STAGES;
   pl.bempty = bars + 3 * MAX_STAGES;
   pl.stat_acc = p.stats ? reinterpret_cast<double*>(bars + 4 * MAX_STAGES) : nullptr;
-  pl.KB = p.Cin / KBLK;
+  pl.KB = (p.Cin + KBLK - 1) / KBLK;   // the last block of a Cin that is not a multiple of 64 is zero past Cin
   pl.T = p.tiles_per_group;
   const int64_t num_tiles = (p.n_out + BLOCK_M - 1) / BLOCK_M;
   pl.num_items = (num_tiles + pl.T - 1) / pl.T * p.ksplit * p.nsplit;
@@ -473,9 +478,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
       }
       const int* irow = idx_ring + (it.gk % IDX_RING) * T * BLOCK_M + it.t * BLOCK_M + warp * ROWS_PER_WARP;
       const int cbase = it.kb * KBLK + chunk * 4;
+      const bool cok = cbase < p.Cin;    // chunks past Cin (Cin % 64 != 0) are stored as zeros
       int srcs[LOADS_PER_SLOT];
 #pragma unroll
-      for (int i = 0; i < LOADS_PER_SLOT; ++i) srcs[i] = irow[i * 2 + rsub];
+      for (int i = 0; i < LOADS_PER_SLOT; ++i) srcs[i] = cok ? irow[i * 2 + rsub] : -1;
 #pragma unroll
       for (int i = 0; i < LOADS_PER_SLOT; ++i) {
         v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -649,12 +655,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
       const Idx4 q2 = load_idx(it2);                // indices of this warp's slot after next
       observe();
       const uint32_t dst0 = smem_u32(pl.a_smem + (size_t)stage * pl.a_stage_bytes) + (uint32_t)sub * 128u;
-      const int64_t coff_b = ((int64_t)it0.kb * KBLK + ch * 8) * 2;
+      // chunks past Cin (Cin % 64 != 0) are zero-fill copies from the start of the row
+      const int cin = it0.kb * KBLK + ch * 8;
+      const int64_t coff_b = cin < p.Cin ? (int64_t)cin * 2 : 0;
+      const uint32_t nfull = cin < p.Cin ? 16u : 0u;
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         // tile row r = 4i + sub; its index lives in register (i / 8) of lane (4 (i % 8) + sub)
         const int idx = __shfl_sync(0xffffffffu, q0.v[i >> 3], ((i & 7) << 2) + sub);
-        const uint32_t nbytes = idx >= 0 ? 16u : 0u;
+        const uint32_t nbytes = idx >= 0 ? nfull : 0u;
         const int64_t boff = (int64_t)(idx >= 0 ? idx : 0) * pitch_b + coff_b;
         // sw128_off(r, ch) with r*128 = i*512 + sub*128 (the latter folded into dst0) and r & 7 = 4 (i & 1) + sub
         const uint32_t off = (uint32_t)i * 512u + (((uint32_t)ch ^ (((uint32_t)(i & 1) << 2) + (uint32_t)sub)) << 4);
@@ -680,16 +689,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
 
 }  // namespace
 
+// room for either orientation: the contraction (Cin, or Cout when transposed) is rounded up to 64 channels
 extern "C" int64_t pasco_conv_packed_bytes(int32_t K, int32_t Cin, int32_t Cout) {
-  return (int64_t)K * Cin * Cout * 4;
+  const int64_t fwd = (int64_t)(Cin + KBLK - 1) / KBLK * KBLK * Cout, tr = (int64_t)(Cout + KBLK - 1) / KBLK * KBLK * Cin;
+  return (int64_t)K * (fwd > tr ? fwd : tr) * 4;
 }
 
 extern "C" int pasco_conv_pack_weights(const float* W, int32_t K, int32_t Cin, int32_t Cout, int32_t transpose,
                                        void* packed, pasco_stream_t s) {
   const int N = transpose ? Cin : Cout, Kc = transpose ? Cout : Cin;
-  PASCO_CHECK_ARG(Kc % KBLK == 0, "pasco_conv_pack_weights: contraction channels (%d) must be a multiple of 64", Kc);
-  PASCO_CHECK_ARG(N % 16 == 0 && N >= 16 && N <= 256, "pasco_conv_pack_weights: output channels (%d) must be a multiple of 16 in [16,256]", N);
-  int64_t total = (int64_t)K * (Kc / KBLK) * N * 8;
+  PASCO_CHECK_ARG(Kc % 16 == 0 && Kc >= 16, "pasco_conv_pack_weights: contraction channels (%d) must be a positive multiple of 16", Kc);
+  PASCO_CHECK_ARG(N % 16 == 0 && N >= 16 && N <= MAX_COUT, "pasco_conv_pack_weights: output channels (%d) must be a multiple of 16 in [16,512]", N);
+  int64_t total = (int64_t)K * ((Kc + KBLK - 1) / KBLK) * N * 8;
   k_pack_weights<<<grid_for(total, 256), 256, 0, (cudaStream_t)s>>>(W, K, Cin, Cout, transpose, (uint8_t*)packed);
   PASCO_CHECK_LAUNCH("pasco_conv_pack_weights");
   return 0;
@@ -697,7 +708,8 @@ extern "C" int pasco_conv_pack_weights(const float* W, int32_t K, int32_t Cin, i
 
 namespace {
 
-// output column ranges: up to 128 columns (the register accumulators of a consumer warpgroup) per work item, and
+// output column ranges: up to 128 columns (the register accumulators of a consumer warpgroup) per work item, up to four
+// ranges (Cout <= 512, the last range takes the remainder), and
 // the tiles per group whose accumulators fit beside each other; small inputs spread tiles over more SMs instead
 void column_plan(int Cout, int64_t tiles, int& nsplit, int& ncols, int& T) {
   nsplit = (Cout + ACC_COLS - 1) / ACC_COLS;
@@ -743,8 +755,8 @@ int conv_launch(const char* fn, const float* in, const void* hi, const void* lo,
                 float* workspace, pasco_stream_t s) {
   const bool planes = hi != nullptr;
   PASCO_CHECK_ARG(precision == 1 || precision == 3, "%s: precision must be 1 (bf16) or 3 (bf16x3)", fn);
-  PASCO_CHECK_ARG(Cin % KBLK == 0, "%s: Cin (%d) must be a multiple of 64", fn, Cin);
-  PASCO_CHECK_ARG(Cout % 16 == 0 && Cout >= 16 && Cout <= 256, "%s: Cout (%d) must be a multiple of 16 in [16,256]", fn, Cout);
+  PASCO_CHECK_ARG(Cin % 16 == 0 && Cin >= 16, "%s: Cin (%d) must be a positive multiple of 16", fn, Cin);
+  PASCO_CHECK_ARG(Cout % 16 == 0 && Cout >= 16 && Cout <= MAX_COUT, "%s: Cout (%d) must be a multiple of 16 in [16,512]", fn, Cout);
   PASCO_CHECK_ARG(K >= 1 && K <= 1024, "%s: K (%d) out of range", fn, K);
   if (in_pitch <= 0) in_pitch = Cin;
   if (out_pitch <= 0) out_pitch = Cout;

@@ -5,9 +5,11 @@
 // MMA view: D[M = 64 input channels][N = columns of gout] += A^T · G with the voxel rows as the contraction dimension,
 // so both operands are MN-major: the very same gathered [rows][64 ch] swizzled tiles the forward kernel builds serve
 // as A and the gout tile as B.  "sub-tile" s = (offset k, 64-channel block cb); a unit = two consecutive sub-tiles x
-// one range of UC output columns (UC = Cout up to 128); consumer warpgroup h accumulates sub-tile h of the CTA's units
-// in registers (at most 128 columns per thread set), walks its share of 64-row tiles, and finally stores its partial
-// dW into its own workspace slot; k_wgrad_sum adds the slots of a pass in CTA order (deterministic, no atomics).
+// one range of UC output columns (UC = 64 or 128, see unit_plan); consumer warpgroup h accumulates sub-tile h of the
+// CTA's units in registers (at most 128 columns per thread set), walks its share of 64-row tiles, and finally stores its
+// partial dW into its own workspace slot; k_wgrad_sum adds the slots of a pass in CTA order (deterministic, no atomics).
+// Cin and Cout are multiples of 16.  The channels of a sub-tile past Cin and the gout columns past Cout are gathered as
+// zeros, so those rows and columns of the partial dW are zero; k_wgrad_sum never reads them.
 #include "common.cuh"
 #include "gmma.cuh"
 
@@ -42,7 +44,8 @@ struct WgradParams {
   int stages, gstages;            // depths of the unit ring and of the gout ring
   int gblocks;                    // 64-column blocks of gout per gout tile (see gout_block)
   int units_per_pass, num_units, num_subs, passes, ctas_per_pass;
-  int uc, ncr;                    // columns per unit, column ranges (unit u = sub-tile pair u / ncr, columns of range u % ncr)
+  int uc, ncr;                    // columns per unit, column ranges (unit u = sub-tile pair u / ncr, columns of range u % ncr;
+                                  // the last range is zero past Cout)
   float* part;                    // [grid][slot]: partial dW of CTA b = cta_in_pass * passes + pass
   int64_t slot;                   // units_per_pass * 128 * uc floats
 };
@@ -55,14 +58,16 @@ struct SubRegs {
   float4 v[WLOADS];
 };
 
-__device__ __forceinline__ void sub_load(SubRegs& r, const float* __restrict__ src, int ld, int cbase_blk, int idx, int lane) {
+// columns >= ncol (past Cin / Cout) load as zeros
+__device__ __forceinline__ void sub_load(SubRegs& r, const float* __restrict__ src, int ld, int cbase_blk, int ncol, int idx, int lane) {
   const int chunk = lane & 15, rsub = lane >> 4;
   const int cbase = cbase_blk + chunk * 4;
+  const bool cok = cbase < ncol;
 #pragma unroll
   for (int i = 0; i < WLOADS; ++i) {
     const int s = __shfl_sync(0xffffffffu, idx, i * 2 + rsub);
     r.v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (s >= 0) r.v[i] = __ldg(reinterpret_cast<const float4*>(src + (int64_t)s * ld + cbase));
+    if (s >= 0 && cok) r.v[i] = __ldg(reinterpret_cast<const float4*>(src + (int64_t)s * ld + cbase));
   }
 }
 
@@ -220,7 +225,7 @@ __device__ __forceinline__ void run_wgrad_consumer(const WgradParams& p, const u
 
 // dW[k][ci][co] += Σ_c part[c * passes + pass][...] over the CTAs c of the pass that owns (k, ci, co), in CTA order
 __global__ void k_wgrad_sum(const WgradParams p, float* __restrict__ dW) {
-  const int CB = p.Cin / 64;
+  const int CB = (p.Cin + 63) / 64;
   const int64_t total = (int64_t)p.K * p.Cin * p.Cout;
   for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t kc = e / p.Cout;
@@ -252,7 +257,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
   uint64_t* gempty_bar = bars + 2 * MAX_STAGES + MAX_GSTAGES;
 
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
-  const int CB = p.Cin / 64;
+  const int CB = (p.Cin + 63) / 64;
   const int pass = blockIdx.x % p.passes;
   const int cta_in_pass = blockIdx.x / p.passes;
   const int unit0 = pass * p.units_per_pass;
@@ -321,14 +326,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_tc(const __grid_consta
       const int64_t row = rt * WG_R + my_r;
       if (dj[0] == 0) {                                            // gout slot: identity rows
         int gidx = row < p.n_out ? (int)row : -1;
-        sub_load(r[0], p.gout, (int)p.gout_pitch, dj[1], gidx, lane);
-        if (dj[2] >= 0) sub_load(r[1], p.gout, (int)p.gout_pitch, dj[2], gidx, lane);
+        sub_load(r[0], p.gout, (int)p.gout_pitch, dj[1], p.Cout, gidx, lane);
+        if (dj[2] >= 0) sub_load(r[1], p.gout, (int)p.gout_pitch, dj[2], p.Cout, gidx, lane);
       } else {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           int idx = idx_ring[((g & (IDX_RING - 1)) * 2 + h) * WG_R + my_r];
           if (!p.nbr && idx >= 0) idx = (int)row;
-          sub_load(r[h], p.in, (int)p.in_pitch, dj[1 + h], idx, lane);
+          sub_load(r[h], p.in, (int)p.in_pitch, dj[1 + h], p.Cin, idx, lane);
         }
       }
     };
@@ -431,7 +436,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
   uint64_t* gempty_bar = bars + 2 * MAX_STAGES + MAX_GSTAGES;
 
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
-  const int CB = p.Cin / 64;
+  const int CB = (p.Cin + 63) / 64;
   const int pass = blockIdx.x % p.passes;
   const int cta_in_pass = blockIdx.x / p.passes;
   const int unit0 = pass * p.units_per_pass;
@@ -483,7 +488,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
     if (warp >= NUM_GATHER_WARPS - Wg) {
       // ---- gout tiles: [64 rows][the units' 64-column blocks] per plane, contiguous rows ----
       const int GB = p.gblocks, gn = gout_nblocks(p, nunits);
-      const int64_t gcol0 = gout_block(p, unit0, 0) * 64 * 2, gcol1 = gout_block(p, unit0, gn - 1) * 64 * 2;   // bytes
+      // byte offsets of the first and the last block from this lane's chunk, and the copy size of the chunk: a chunk
+      // past Cout is a zero-fill copy from the start of the row
+      const int gc0 = gout_block(p, unit0, 0) * 64, gc1 = gout_block(p, unit0, gn - 1) * 64;
+      const bool ok0 = gc0 + ch * 8 < p.Cout, ok1 = gc1 + ch * 8 < p.Cout;
+      const int64_t gcol0 = ok0 ? gc0 * 2 : -ch * 16, gcol1 = ok1 ? gc1 * 2 : -ch * 16;
+      const uint32_t nb0 = ok0 ? 16u : 0u, nb1 = ok1 ? 16u : 0u;
       int gb = warp - (NUM_GATHER_WARPS - Wg);     // < Wg <= gstages
       uint32_t gphase = 0;
       for (int64_t rti = gb; rti < my_rts; rti += Wg) {
@@ -493,11 +503,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
 #pragma unroll 4
         for (int i = 0; i < WG_R / 4; ++i) {
           const int64_t row = rt * WG_R + i * 4 + sub;
-          const uint32_t nbytes = row < p.n_out ? 16u : 0u;
-          const int64_t boff = ((row < p.n_out ? row : 0) * p.gout_pitch + ch * 8) * 2;
+          const bool rok = row < p.n_out;
+          const int64_t boff = ((rok ? row : 0) * p.gout_pitch + ch * 8) * 2;
           const uint32_t off = (uint32_t)i * 512u + (((uint32_t)ch ^ (((uint32_t)(i & 1) << 2) + (uint32_t)sub)) << 4);
           for (int b = 0; b < gn; ++b) {
             const int64_t src = boff + (b == 0 ? gcol0 : gcol1);
+            const uint32_t nbytes = rok ? (b == 0 ? nb0 : nb1) : 0u;
             cp_async16_zfill(g0 + (uint32_t)b * WG_SUB_BYTES + off, gp_hi + src, nbytes);
             if (NSPLIT == 3) cp_async16_zfill(g0 + (uint32_t)(GB + b) * WG_SUB_BYTES + off, gp_lo + src, nbytes);
           }
@@ -544,11 +555,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_wgrad_pl(const __grid_consta
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int sbi = sb0 + h;
-          const int64_t coff_b = ((int64_t)(sbi < p.num_subs ? sbi % CB : 0) * 64 + ch * 8) * 2;
+          // channels past Cin (Cin % 64 != 0) are zero-fill copies from the start of the row
+          const int cin = (sbi < p.num_subs ? sbi % CB : 0) * 64 + ch * 8;
+          const int64_t coff_b = cin < p.Cin ? (int64_t)cin * 2 : 0;
+          const uint32_t nfull = cin < p.Cin ? 16u : 0u;
 #pragma unroll
           for (int i = 0; i < WG_R / 4; ++i) {
             const int idx = __shfl_sync(0xffffffffu, q0.v[h * 2 + (i >> 3)], ((i & 7) << 2) + sub);
-            const uint32_t nbytes = idx >= 0 ? 16u : 0u;
+            const uint32_t nbytes = idx >= 0 ? nfull : 0u;
             const int64_t boff = (int64_t)(idx >= 0 ? idx : 0) * p.in_pitch * 2 + coff_b;
             const uint32_t off = (uint32_t)i * 512u + (((uint32_t)ch ^ (((uint32_t)(i & 1) << 2) + (uint32_t)sub)) << 4);
             cp_async16_zfill(a0 + (uint32_t)h * WG_SUB_BYTES + off, in_hi + boff, nbytes);
@@ -582,11 +596,14 @@ int ctas_per_pass(int64_t num_rt, int passes) {
   return cpp < 1 ? 1 : (int)cpp;
 }
 
-// unit geometry: uc columns per unit (the consumers' 128 accumulator columns hold 128 / uc units), ncr column ranges
+// unit geometry: uc columns per unit (the consumers' 128 accumulator columns hold 128 / uc units), ncr column ranges.
+// 64-column units for Cout <= 64 and for Cout = 192 (three full ranges instead of two with a zero half), 128-column
+// units otherwise, up to four of them (Cout <= 512); the last range of a Cout that is not a multiple of uc is zero
+// past Cout.
 void unit_plan(WgradParams& p, int K, int Cin, int Cout) {
-  p.uc = Cout <= ACC_COLS ? Cout : (Cout % ACC_COLS == 0 ? ACC_COLS : 64);
-  p.ncr = Cout / p.uc;
-  p.num_subs = K * (Cin / 64);
+  p.uc = Cout <= 64 || Cout == 192 ? 64 : ACC_COLS;
+  p.ncr = (Cout + p.uc - 1) / p.uc;
+  p.num_subs = K * ((Cin + 63) / 64);
   p.num_units = (p.num_subs + 1) / 2 * p.ncr;
   p.units_per_pass = ACC_COLS / p.uc;
   if (p.units_per_pass > p.num_units) p.units_per_pass = p.num_units;
@@ -601,8 +618,8 @@ int wgrad_launch(const char* fn, WgradParams& p, int64_t n_out, int32_t K, int32
                  int32_t precision, pasco_stream_t s) {
   const bool planes = p.in_hi != nullptr;
   PASCO_CHECK_ARG(precision == 1 || precision == 3, "%s: precision must be 1 or 3", fn);
-  PASCO_CHECK_ARG(Cin % 64 == 0 && Cout % 64 == 0 && Cout <= 256,
-                  "%s: Cin (%d) and Cout (%d) must be multiples of 64, Cout <= 256", fn, Cin, Cout);
+  PASCO_CHECK_ARG(Cin % 16 == 0 && Cin >= 16 && Cout % 16 == 0 && Cout >= 16 && Cout <= 4 * ACC_COLS,
+                  "%s: Cin (%d) and Cout (%d) must be positive multiples of 16, Cout <= 512", fn, Cin, Cout);
   if (p.in_pitch <= 0) p.in_pitch = Cin;
   if (p.gout_pitch <= 0) p.gout_pitch = Cout;
   if (planes)

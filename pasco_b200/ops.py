@@ -368,16 +368,17 @@ def conv_path(kind: str, c_contract: int, c_out: int, K: int, nbr, n_rows: int) 
     """The kernels one convolution launch runs on: 'planes' (pasco_conv_forward_planes / pasco_conv_wgrad_planes),
     'splitk' (pasco_conv_forward_splitk), 'regs' (pasco_conv_forward_tc / pasco_conv_wgrad_tc) or 'simt' (CUDA cores).
     kind 'fwd' / 'dgrad': c_contract gathered channels → c_out channels of n_rows output rows through K offsets of the
-    neighbour table nbr (None: identity rows); 'wgrad': c_contract = Cin, c_out = Cout (never split, n_rows unused)."""
-    if _FORCE_SIMT or (_SIMT_KINDS is not None and kind in _SIMT_KINDS) or c_contract % 64:
+    neighbour table nbr (None: identity rows); 'wgrad': c_contract = Cin, c_out = Cout (never split, n_rows unused).
+    The tensor-core kernels take both channel counts as multiples of 16 and c_out <= 512."""
+    if _FORCE_SIMT or (_SIMT_KINDS is not None and kind in _SIMT_KINDS):
         return "simt"
-    if kind == "wgrad":
-        if c_out % 64 or c_out > 256:
+    if c_contract % 16 or c_contract < 16 or c_out % 16 or not 16 <= c_out <= 512:
+        return "simt"
+    if kind != "wgrad":
+        if K > 1024:
             return "simt"
-    elif c_out % 16 or not 16 <= c_out <= 256 or K > 1024:
-        return "simt"
-    elif _SPLIT_K and load().pasco_conv_splitk_workspace_bytes(K, n_rows, c_out) > 0:
-        return "splitk"
+        if _SPLIT_K and load().pasco_conv_splitk_workspace_bytes(K, n_rows, c_out) > 0:
+            return "splitk"
     return "planes" if _USE_PLANES and nbr is not None and K > 1 else "regs"
 
 
