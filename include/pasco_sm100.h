@@ -175,6 +175,22 @@ int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t n_in, cons
                               int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map, const float* bias,
                               double* stats, float* out, int32_t precision, int64_t plane_pitch, int64_t out_pitch,
                               pasco_stream_t s);
+/* Inference form of pasco_conv_forward_planes (eval-mode forward without gradients): the same convolution with an
+ * epilogue that, per element of row r < n_out and column c,
+ *   v = acc + bias[c]
+ *   residual != NULL:  v = act_out(residual[r][c] + v)             (a residual block's ReLU(skip + y))
+ *   out != NULL:       out[r][c] = v
+ *   next_hi != NULL:   z = act_next(v * next_scale[c] + next_shift[c])  (one fused multiply-add; no affine when next_scale
+ *                      is NULL), next_hi[r][c] = bf16(z), next_lo[r][c] = bf16(z - hi) (next_lo in precision 3 only)
+ * i.e. the next layer's eval-mode BatchNorm + activation written as the planes the next convolution gathers.  The
+ * arithmetic is that of pasco_affine_act and pasco_split_planes, so the result is bit for bit the unfused sequence.
+ * residual, out and the next planes are contiguous [n_out, Cout]; act_* as in pasco_affine_act (0 none, 1 ReLU,
+ * 2 LeakyReLU 0.01).  At least one of out / next_hi is set.  No statistics are computed.                          */
+int pasco_conv_forward_planes_infer(const void* hi, const void* lo, int64_t n_in, const int32_t* nbr, int32_t K,
+                                    int64_t n_out, int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
+                                    const float* bias, const float* residual, int32_t act_out, float* out,
+                                    const float* next_scale, const float* next_shift, int32_t act_next, void* next_hi,
+                                    void* next_lo, int32_t precision, int64_t plane_pitch, pasco_stream_t s);
 int pasco_conv_wgrad_planes(const void* in_hi, const void* in_lo, int64_t n_in, const int32_t* nbr, int32_t K,
                             int64_t n_out, int32_t Cin, int32_t Cout, const void* g_hi, const void* g_lo, float* dW,
                             int32_t precision, int64_t in_pitch, int64_t gout_pitch, pasco_stream_t s);

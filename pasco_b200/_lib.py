@@ -45,6 +45,8 @@ PROTOTYPES = {
     "pasco_conv_forward_splitk": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _i32, _i64, _i64, _p, _i64, _p]),
     "pasco_split_planes": (C.c_int, [_p, _i64, _i32, _i64, _p, _p, _i32, _p, _p, _p]),
     "pasco_conv_forward_planes": (C.c_int, [_p, _p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _p, _i32, _i64, _i64, _p]),
+    "pasco_conv_forward_planes_infer": (C.c_int, [_p, _p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _p, _i32, _p, _p, _p,
+                                                  _i32, _p, _p, _i32, _i64, _p]),
     "pasco_conv_wgrad_planes": (C.c_int, [_p, _p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _p, _i32, _i64, _i64, _p]),
     "pasco_conv_wgrad_tc": (C.c_int, [_p, _i64, _p, _i32, _i64, _i32, _i32, _p, _p, _i32, _i64, _i64, _p]),
     "pasco_conv_forward_simt": (C.c_int, [_p, _p, _i32, _i64, _i32, _i32, _p, _i32, _p, _p, _p, _p]),

@@ -55,6 +55,14 @@ __device__ __forceinline__ int table_find(const uint64_t* __restrict__ keys, con
   }
 }
 
+// activations: 0 none, 1 ReLU, 2 LeakyReLU(0.01) — the row kernels (reduce.cu) and the convolution's inference epilogue
+// (conv_tc.cu) share this one definition, so a fused epilogue computes bit for bit what the row pass computes
+__device__ __forceinline__ float act_fwd(float z, int act) {
+  if (act == 1) return fmaxf(z, 0.f);
+  if (act == 2) return z > 0.f ? z : 0.01f * z;
+  return z;
+}
+
 __host__ __device__ __forceinline__ int floor_div(int a, int s) {
   int q = a / s;
   return (a % s != 0 && ((a < 0) != (s < 0))) ? q - 1 : q;

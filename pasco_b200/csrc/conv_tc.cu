@@ -20,6 +20,7 @@
 //
 // precision 3 (the "fp32" mode): operands split as x = hi + lo (bf16 each) and three MMAs
 // hi·hi + lo·hi + hi·lo accumulate in fp32 — ~2^-16 relative error, well inside the 1e-3 parity bound.
+#include <type_traits>
 #include "common.cuh"
 #include "gmma.cuh"
 
@@ -73,6 +74,20 @@ struct ConvParams {
   int nsplit, ncols;          // output columns in ranges of ncols (the last one may be narrower), one work item each
   int koff_base, koff_step;   // weight slice of table row k = koff_base + koff_step * k
   int ksplit;                 // offset ranges (1: no split)
+};
+
+// Operands of the inference epilogue (k_conv_pl<NSPLIT, true>, see infer_epilogue).  Rows are [n_out, Cout], contiguous.
+struct InferEpilogue {
+  const float* residual;      // added before act_out (nullptr: none)
+  const float* next_scale;    // the next layer's eval BatchNorm as a per-channel affine (nullptr: none)
+  const float* next_shift;
+  uint16_t* next_hi;          // bf16 planes of act_next(affine(v)) (nullptr: not written)
+  uint16_t* next_lo;          // bf16x3 mode only
+  int act_out, act_next;
+};
+// The training instantiations keep ConvParams as their kernel parameter; the inference ones append the epilogue.
+struct InferParams : ConvParams {
+  InferEpilogue e;
 };
 
 // ------------------------------------------------------------------------------------------------------------
@@ -228,11 +243,16 @@ __device__ __forceinline__ void role_weight_loader(const ConvParams& p, const Pi
 // The epilogue adds the bias, stores fp32 rows and optionally accumulates the per-channel sum and sum of squares of
 // what was stored (the BatchNorm statistics of the next layer): per warp over its rows with shuffles, then in fp64 in
 // shared memory, one global fp64 atomic per channel and CTA.
-template <int NSPLIT, bool CPASYNC_A, int CH>
+// INFER (k_conv_pl<NSPLIT, true>) replaces that epilogue by infer_epilogue: no statistics.
+template <int CH, int NCH>
+__device__ __forceinline__ void infer_epilogue(const InferParams& q, const Pipe& pl, float (&acc)[NCH][CH / 2], int64_t v,
+                                               int g, int wq, int lane);
+
+template <int NSPLIT, bool CPASYNC_A, int CH, bool INFER>
 __device__ __forceinline__ void role_consumer(const ConvParams& p, const Pipe& pl, int g, int wq, int lane) {
   constexpr int NCH = ACC_COLS / CH;
   float acc[NCH][CH / 2];
-  const bool want_stats = pl.stat_acc != nullptr;
+  const bool want_stats = !INFER && pl.stat_acc != nullptr;
   int sa = 0, sb = 0;
   uint32_t pa = 0, pb = 0;
   int held_a = -1, held_b = -1;     // stages of the slot whose MMAs may still be in flight (-1: none)
@@ -323,6 +343,10 @@ __device__ __forceinline__ void role_consumer(const ConvParams& p, const Pipe& p
     wg_wait<0>();
     release_held();
     // ---- epilogue ----
+    if constexpr (INFER) {
+      infer_epilogue<CH, NCH>(static_cast<const InferParams&>(p), pl, acc, v, g, wq, lane);
+      continue;
+    }
     float* out_part = p.out + item_ks(p, v) * p.n_out * p.out_pitch;    // this split's partial output
     const int n0 = item_n0(p, v);
 #pragma unroll
@@ -373,13 +397,70 @@ __device__ __forceinline__ void role_consumer(const ConvParams& p, const Pipe& p
   }
 }
 
+// Inference epilogue of work item v.  Per element (row < n_out, column c):
+//   v = acc + bias[c]
+//   residual:  v = act_out(residual[row][c] + v)                  (a residual block's relu(skip + y))
+//   out:       out[row][c] = v
+//   next_hi:   z = act_next(fmaf(v, next_scale[c], next_shift[c]))  (the next layer's eval BatchNorm + activation; no
+//              affine when next_scale is null), hi = bf16(z), lo = bf16(z - hi) (lo in bf16x3 mode only)
+// The arithmetic is that of k_affine_act (residual + act) and k_split_planes (affine + act + split), so the fused result
+// is bit for bit the unfused sequence.  Inference items never split the offsets (ksplit = 1).
+template <int CH, int NCH>
+__device__ __forceinline__ void infer_epilogue(const InferParams& q, const Pipe& pl, float (&acc)[NCH][CH / 2], int64_t v,
+                                               int g, int wq, int lane) {
+  const InferEpilogue& e = q.e;
+  const int64_t group = item_group(q, v);
+  const int n0 = item_n0(q, v), ncols = item_ncols(q, v);
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+    const int t = (c * CH) / q.ncols, col0 = c * CH - t * q.ncols;
+    if (t >= pl.T || col0 >= ncols) continue;
+    const int64_t rbase = (group * pl.T + t) * BLOCK_M + g * 64;
+#pragma unroll
+    for (int i4 = 0; i4 < CH / 8; ++i4) {
+      const int col = n0 + col0 + frag_col(i4 * 4, lane);
+      float2 b = make_float2(0.f, 0.f), sc = b, sh = b;
+      if (q.bias) b = __ldg(reinterpret_cast<const float2*>(q.bias + col));
+      if (e.next_scale) {
+        sc = __ldg(reinterpret_cast<const float2*>(e.next_scale + col));
+        sh = __ldg(reinterpret_cast<const float2*>(e.next_shift + col));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {              // rows r and r + 8
+        const int64_t row = rbase + frag_row(i4 * 4 + 2 * h, wq, lane);
+        if (row >= q.n_out) continue;
+        float v0 = acc[c][i4 * 4 + 2 * h] + b.x, v1 = acc[c][i4 * 4 + 2 * h + 1] + b.y;
+        const int64_t off = row * q.Cout + col;
+        if (e.residual) {
+          const float2 r = __ldg(reinterpret_cast<const float2*>(e.residual + off));
+          v0 = act_fwd(r.x + v0, e.act_out);
+          v1 = act_fwd(r.y + v1, e.act_out);
+        }
+        if (q.out) *reinterpret_cast<float2*>(q.out + row * q.out_pitch + col) = make_float2(v0, v1);
+        if (e.next_hi) {
+          if (e.next_scale) {
+            v0 = fmaf(v0, sc.x, sh.x);
+            v1 = fmaf(v1, sc.y, sh.y);
+          }
+          v0 = act_fwd(v0, e.act_next);
+          v1 = act_fwd(v1, e.act_next);
+          uint32_t hi, lo;
+          split2(v0, v1, hi, lo);
+          *reinterpret_cast<uint32_t*>(e.next_hi + off) = hi;
+          if (e.next_lo) *reinterpret_cast<uint32_t*>(e.next_lo + off) = lo;
+        }
+      }
+    }
+  }
+}
+
 // the consumer role of warp `warp` (CONS_WARP0 <= warp < LOAD_WARP), dispatched on the chunk width
-template <int NSPLIT, bool CPASYNC_A>
+template <int NSPLIT, bool CPASYNC_A, bool INFER>
 __device__ __forceinline__ void run_consumer(const ConvParams& p, const Pipe& pl, int warp, int lane) {
   const int g = (warp - CONS_WARP0) >> 2, wq = (warp - CONS_WARP0) & 3;
-  if (p.Cout % 128 == 0) role_consumer<NSPLIT, CPASYNC_A, 128>(p, pl, g, wq, lane);   // column ranges of exactly 128
-  else if (p.Cout % 64 == 0) role_consumer<NSPLIT, CPASYNC_A, 64>(p, pl, g, wq, lane);
-  else role_consumer<NSPLIT, CPASYNC_A, 16>(p, pl, g, wq, lane);
+  if (p.Cout % 128 == 0) role_consumer<NSPLIT, CPASYNC_A, 128, INFER>(p, pl, g, wq, lane);   // column ranges of exactly 128
+  else if (p.Cout % 64 == 0) role_consumer<NSPLIT, CPASYNC_A, 64, INFER>(p, pl, g, wq, lane);
+  else role_consumer<NSPLIT, CPASYNC_A, 16, INFER>(p, pl, g, wq, lane);
 }
 
 template <int NSPLIT>
@@ -543,7 +624,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
     if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, NSPLIT == 3 ? 2 : 1);
   } else {
     reg_alloc<TC_CONS_REGS>();
-    run_consumer<NSPLIT, false>(p, pl, warp, lane);
+    run_consumer<NSPLIT, false, false>(p, pl, warp, lane);
   }
 }
 
@@ -561,8 +642,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_tc(const __grid_constan
 // cp.async.mbarrier.arrive.noinc on the slot's "full" barrier (expected count = 32), so the barrier completes when the
 // last copy has landed — no wait_group, no software publish step, and the producers run up to `sa` slots ahead of the
 // MMA.  The consumers add a generic→async proxy fence after their barrier wait.
-template <int NSPLIT>
-__global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constant__ ConvParams p) {
+// INFER: the inference epilogue (infer_epilogue) instead of the training one; everything else is the same kernel.
+template <int NSPLIT, bool INFER>
+__global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constant__ std::conditional_t<INFER, InferParams, ConvParams> p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const Pipe pl = pipe_setup<NSPLIT>(p, smem_raw, 0, 32);
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x, 0) >> 5, lane = threadIdx.x & 31;   // provably warp-uniform, else ptxas serializes the wgmma
@@ -683,7 +765,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) k_conv_pl(const __grid_constan
     if (warp == LOAD_WARP && lane == 0) role_weight_loader(p, pl, NSPLIT == 3 ? 2 : 1);
   } else {
     reg_alloc<PL_CONS_REGS>();
-    run_consumer<NSPLIT, true>(p, pl, warp, lane);
+    run_consumer<NSPLIT, true, INFER>(p, pl, warp, lane);
   }
 }
 
@@ -748,12 +830,26 @@ __global__ void k_splitk_reduce(const float* __restrict__ part, int ksplit, int6
 
 // The host half of every forward / input-gradient launch.  The gathered operand is either fp32 rows `in` (register
 // gather, k_conv_tc; split over the offsets when ksplit > 1) or, when `hi` is set, bf16 planes hi [+ lo] (plane gather,
-// k_conv_pl); in_pitch is its row stride in floats or plane elements (0 = Cin).  Error messages name the entry point fn.
+// k_conv_pl); in_pitch is its row stride in floats or plane elements (0 = Cin).  epi (plane gather only, no statistics,
+// no split) selects the inference epilogue; nullptr = the training one.  Error messages name the entry point fn.
+template <class P>
+int launch_conv(const char* fn, void (*kern)(P), int grid, size_t smem, pasco_stream_t s, const P& p) {
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) {
+    set_error("%s: cudaFuncSetAttribute(%zu bytes) failed: %s", fn, smem, cudaGetErrorString(e));
+    return -1;
+  }
+  kern<<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
+  PASCO_CHECK_LAUNCH(fn);
+  return 0;
+}
+
 int conv_launch(const char* fn, const float* in, const void* hi, const void* lo, int64_t in_pitch, const int32_t* nbr,
                 int32_t K, int64_t n_out, int32_t Cin, int32_t Cout, const void* packed_w, const int32_t* koff_map,
                 const float* bias, double* stats, float* out, int32_t precision, int64_t out_pitch, int ksplit,
-                float* workspace, pasco_stream_t s) {
+                float* workspace, pasco_stream_t s, const InferEpilogue* epi = nullptr) {
   const bool planes = hi != nullptr;
+  PASCO_CHECK_ARG(!epi || (planes && !stats && ksplit == 1), "%s: the inference epilogue is plane-gather only", fn);
   PASCO_CHECK_ARG(precision == 1 || precision == 3, "%s: precision must be 1 (bf16) or 3 (bf16x3)", fn);
   PASCO_CHECK_ARG(Cin % 16 == 0 && Cin >= 16, "%s: Cin (%d) must be a positive multiple of 16", fn, Cin);
   PASCO_CHECK_ARG(Cout % 16 == 0 && Cout >= 16 && Cout <= MAX_COUT, "%s: Cout (%d) must be a multiple of 16 in [16,512]", fn, Cout);
@@ -813,15 +909,16 @@ int conv_launch(const char* fn, const float* in, const void* hi, const void* lo,
   const size_t smem = (size_t)sa * a_stage + (size_t)sb * b_stage + fixed;
   const int64_t items = (tiles + T - 1) / T * p.ksplit * nsplit;
   const int grid = (int)(items < num_sms() ? items : num_sms());
-  void (*kern)(ConvParams) = planes ? (precision == 3 ? k_conv_pl<3> : k_conv_pl<1>)
-                                    : (precision == 3 ? k_conv_tc<3> : k_conv_tc<1>);
-  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) {
-    set_error("%s: cudaFuncSetAttribute(%zu bytes) failed: %s", fn, smem, cudaGetErrorString(e));
-    return -1;
+  if (epi) {
+    InferParams q;
+    static_cast<ConvParams&>(q) = p;
+    q.e = *epi;
+    return launch_conv(fn, precision == 3 ? k_conv_pl<3, true> : k_conv_pl<1, true>, grid, smem, s, q);
   }
-  kern<<<grid, NUM_THREADS, smem, (cudaStream_t)s>>>(p);
-  PASCO_CHECK_LAUNCH(fn);
+  void (*kern)(ConvParams) = planes ? (precision == 3 ? k_conv_pl<3, false> : k_conv_pl<1, false>)
+                                    : (precision == 3 ? k_conv_tc<3> : k_conv_tc<1>);
+  const int rc = launch_conv(fn, kern, grid, smem, s, p);
+  if (rc != 0) return rc;
   if (p.ksplit > 1) {
     k_splitk_reduce<<<grid_for(n_out * (Cout / 4), 256), 256, 0, (cudaStream_t)s>>>(workspace, p.ksplit, n_out, Cout, bias, out,
                                                                                 out_pitch);
@@ -847,6 +944,30 @@ extern "C" int pasco_conv_forward_planes(const void* hi, const void* lo, int64_t
   PASCO_CHECK_ARG(hi != nullptr && (precision == 1 || lo != nullptr), "pasco_conv_forward_planes: missing plane (precision 3 needs hi and lo)");
   return conv_launch("pasco_conv_forward_planes", nullptr, hi, lo, plane_pitch, nbr, K, n_out, Cin, Cout, packed_w, koff_map,
                      bias, stats, out, precision, out_pitch, 1, nullptr, s);
+}
+
+extern "C" int pasco_conv_forward_planes_infer(const void* hi, const void* lo, int64_t /*n_in*/, const int32_t* nbr, int32_t K,
+                                               int64_t n_out, int32_t Cin, int32_t Cout, const void* packed_w,
+                                               const int32_t* koff_map, const float* bias, const float* residual,
+                                               int32_t act_out, float* out, const float* next_scale, const float* next_shift,
+                                               int32_t act_next, void* next_hi, void* next_lo, int32_t precision,
+                                               int64_t plane_pitch, pasco_stream_t s) {
+  const char* fn = "pasco_conv_forward_planes_infer";
+  PASCO_CHECK_ARG(hi != nullptr && (precision == 1 || lo != nullptr), "%s: missing plane (precision 3 needs hi and lo)", fn);
+  PASCO_CHECK_ARG(out != nullptr || next_hi != nullptr, "%s: nothing to write (out and next_hi are both null)", fn);
+  PASCO_CHECK_ARG(act_out >= 0 && act_out <= 2 && act_next >= 0 && act_next <= 2, "%s: act must be 0, 1 or 2", fn);
+  PASCO_CHECK_ARG((next_scale == nullptr) == (next_shift == nullptr), "%s: next_scale and next_shift come together", fn);
+  PASCO_CHECK_ARG(next_hi != nullptr || (next_scale == nullptr && next_lo == nullptr), "%s: next-layer operands without next_hi", fn);
+  PASCO_CHECK_ARG(next_hi == nullptr || (next_lo != nullptr) == (precision == 3),
+                  "%s: next_lo is written in bf16x3 mode (precision 3) only, and then required", fn);
+  PASCO_CHECK_ARG((((uintptr_t)residual | (uintptr_t)next_scale | (uintptr_t)next_shift | (uintptr_t)bias) & 7) == 0 &&
+                  (((uintptr_t)next_hi | (uintptr_t)next_lo) & 3) == 0, "%s: misaligned residual, coefficient or plane pointer", fn);
+  InferEpilogue e;
+  e.residual = residual; e.next_scale = next_scale; e.next_shift = next_shift;
+  e.next_hi = (uint16_t*)next_hi; e.next_lo = (uint16_t*)next_lo;
+  e.act_out = act_out; e.act_next = act_next;
+  return conv_launch(fn, nullptr, hi, lo, plane_pitch, nbr, K, n_out, Cin, Cout, packed_w, koff_map, bias, nullptr, out,
+                     precision, 0, 1, nullptr, s, &e);
 }
 
 extern "C" int64_t pasco_conv_splitk_workspace_bytes(int32_t K, int64_t n_out, int32_t Cout) {

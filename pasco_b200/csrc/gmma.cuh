@@ -190,6 +190,11 @@ __device__ __forceinline__ void split4(const float4& x, uint2& hi, uint2& lo) {
   lo.x = pack_bf16x2(r0, r1);
   lo.y = pack_bf16x2(r2, r3);
 }
+// the same split for two values (one packed bf16x2 word per plane)
+__device__ __forceinline__ void split2(float x, float y, uint32_t& hi, uint32_t& lo) {
+  hi = pack_bf16x2(x, y);
+  lo = pack_bf16x2(x - __uint_as_float(hi << 16), y - __uint_as_float(hi & 0xffff0000u));
+}
 __device__ __forceinline__ uint2 to_bf16x4(const float4& x) { return make_uint2(pack_bf16x2(x.x, x.y), pack_bf16x2(x.z, x.w)); }
 
 }  // namespace gmma

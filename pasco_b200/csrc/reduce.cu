@@ -6,13 +6,8 @@
 using namespace pasco;
 
 // ------------------------------------------------------------------------------------------------
-// activation helpers: 0 none, 1 ReLU, 2 LeakyReLU(0.01)
+// activation helpers: 0 none, 1 ReLU, 2 LeakyReLU(0.01) (act_fwd: common.cuh)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float act_fwd(float z, int act) {
-  if (act == 1) return fmaxf(z, 0.f);
-  if (act == 2) return z > 0.f ? z : 0.01f * z;
-  return z;
-}
 __device__ __forceinline__ float act_grad(float z, int act) {
   if (act == 1) return z > 0.f ? 1.f : 0.f;
   if (act == 2) return z > 0.f ? 1.f : 0.01f;

@@ -250,8 +250,9 @@ def _maybe_install_hooks() -> None:
 
 class _LazyRows:
     """Deferred act(BatchNorm(x)) over rows — what MinkowskiBatchNorm (+ a following MinkowskiReLU / LeakyReLU) returns in
-    training mode.  If the consumer is a stride-1 k>1 MinkowskiConvolution the three run as ONE fused node whose
-    BatchNorm apply pass writes the bf16 planes the convolution gathers (ops.BNActConv); any other consumer reading `.F`
+    training mode, and in eval mode without gradients.  If the consumer is a stride-1 k>1 MinkowskiConvolution the three
+    run as ONE fused node whose BatchNorm apply pass writes the bf16 planes the convolution gathers (ops.BNActConv; in eval
+    mode one split pass with the running statistics, ops.bn_act_conv); any other consumer reading `.F`
     materialises it through the fused row kernels (ops.batchnorm_rows).  Results are identical either way; this only
     removes one full read+write of the activations per BatchNorm → convolution pair of the UNMODIFIED reference model
     (pre-activation residual blocks, pasco/maskpls/mink.py:618-658)."""
@@ -523,9 +524,12 @@ class MinkowskiBatchNorm(MinkowskiModuleBase):
 
     def forward(self, x):
         # training-mode statistics + apply run in the fused row kernels (ops.BatchNormAct; the convolution that produced
-        # x already left its column sums); same parameters, buffers and running-statistics update as nn.BatchNorm1d
+        # x already left its column sums); same parameters, buffers and running-statistics update as nn.BatchNorm1d.  In
+        # eval mode without gradients the deferred form lets a following stride-1 convolution take bn_act_conv's
+        # split fusion (the running-statistics affine + activation written straight into its planes)
         xf = x.F
-        if self.bn.training and self.bn.running_mean is not None and xf.is_cuda and xf.dtype == torch.float32:
+        if (self.bn.running_mean is not None and xf.is_cuda and xf.dtype == torch.float32
+                and (self.bn.training or ops.inference_fusion_active(self.bn))):
             return _like(x, _LazyRows(self.bn, xf, ops.ACT_NONE, self._group()))      # see _LazyRows
         return _like(x, ops.batchnorm_rows(self.bn, xf, ops.ACT_NONE, self._group()))
 

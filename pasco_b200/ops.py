@@ -27,6 +27,8 @@ _SPLIT_K = True          # few-tile / many-offset convs (dense bottleneck) are s
 _PENDING_STATS = None
 _USE_PLANES = True      # gathered convs (K > 1) read pre-split bf16 planes with zero-fill cp.async copies (k_conv_pl /
                         # k_wgrad_pl); False = the round-1 register-gather kernels (kept for cross-checks)
+_INFER_FUSION = True    # eval mode without gradients: BatchNorm + activation fused into the planes / the convolution's
+                        # inference epilogue (inference_fusion_active); False = the row passes (bit-identical cross-check)
 PROFILE = None          # bench.py sets this to a list: (kind, start_event, end_event, meta) per conv launch
 PAIR_COUNTS = {}        # nbr.data_ptr() → 0-dim device tensor with the number of valid pairs (profiling only)
 CALLS = 0               # number of C-ABI compute calls (each launches >= 1 kernel of ours)
@@ -443,6 +445,48 @@ def conv_apply(feats: torch.Tensor, weight: torch.Tensor, nbr: Optional[torch.Te
     return out
 
 
+def conv_infer(planes, weight: torch.Tensor, bias: Optional[torch.Tensor], kmap: KernelMap,
+               packs: Optional[PackedWeights] = None, residual: Optional[torch.Tensor] = None, act_out: int = 0,
+               want_out: bool = True, next_coefs=None, next_act: int = 0, want_next: bool = False):
+    """Grad-free forward of a stride-1 plane-path convolution on the inference epilogue
+    (pasco_conv_forward_planes_infer): from the planes (hi, lo) of the gathered input,
+        v = conv + bias;  v = act_out(residual + v) when a residual is given
+    and returns (out, next_planes): out = v as fp32 [n_out, Cout] when want_out (else None), next_planes = the bf16 planes
+    of act_next(v * scale + shift) with (scale, shift) = next_coefs (the next layer's eval BatchNorm, bn_eval_coefs; None =
+    no affine) when want_next (else None).  Bit for bit what conv_apply, affine_act and split_planes compute in turn, in
+    one launch and without the fp32 intermediates or the statistics."""
+    if torch.is_grad_enabled():
+        raise RuntimeError("ops.conv_infer records no autograd graph: call it under torch.no_grad()")
+    K, Cin, Cout = weight.shape
+    if conv_path("fwd", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) != "planes":
+        raise RuntimeError(f"ops.conv_infer: a {Cin}->{Cout} convolution over {kmap.K} offsets is not on the plane-gather path")
+    hi, lo = planes
+    n, dev = kmap.n_out, hi.device
+    out = torch.empty(n, Cout, dtype=torch.float32, device=dev) if want_out else None
+    nhi = torch.empty(n, Cout, dtype=torch.bfloat16, device=dev) if want_next else None
+    nlo = torch.empty(n, Cout, dtype=torch.bfloat16, device=dev) if want_next and _PRECISION == 3 else None
+    scale, shift = (c.contiguous() for c in next_coefs) if next_coefs is not None else (None, None)
+    if residual is not None:
+        residual = residual.contiguous()
+        assert residual.shape == (n, Cout) and residual.dtype == torch.float32
+    prof = PROFILE
+    if prof is not None:
+        ev0 = torch.cuda.Event(enable_timing=True)
+        ev0.record()
+    global _PENDING_STATS
+    _PENDING_STATS = None
+    call("pasco_conv_forward_planes_infer", ptr(hi), ptr(lo), hi.shape[0], ptr(kmap.nbr), kmap.K, n, Cin, Cout,
+         ptr((packs or PackedWeights()).get(weight, False)), None, ptr(bias.view(-1).contiguous() if bias is not None else None),
+         ptr(residual), act_out, ptr(out), ptr(scale), ptr(shift), next_act, ptr(nhi), ptr(nlo), _PRECISION, 0)
+    if prof is not None:
+        ev1 = torch.cuda.Event(enable_timing=True)
+        ev1.record()
+        prof.append(("fwd", ev0, ev1, dict(n_in=hi.shape[0], n_out=n, K=kmap.K, Cin=Cin, Cout=Cout,
+                                           pairs=PAIR_COUNTS.get(kmap.nbr.data_ptr()), tc=True, precision=_PRECISION,
+                                           path="planes_infer")))
+    return out, ((nhi, nlo) if want_next else None)
+
+
 def take_pending_stats(x: torch.Tensor) -> Optional[torch.Tensor]:
     """Column statistics a convolution epilogue produced for exactly this tensor (same storage, shape and version —
     any in-place change since bumps the version), or None.  Consumed once."""
@@ -707,15 +751,57 @@ class BNActConv(torch.autograd.Function):
         return gx, gg, gbeta, gw, gb, None, None, None, None, None, None, None, None
 
 
+def inference_fusion(flag: bool) -> None:
+    global _INFER_FUSION
+    _INFER_FUSION = bool(flag)
+
+
+def inference_fusion_active(module) -> bool:
+    """True when `module` (a BatchNorm or a network) runs in eval mode with gradients disabled and the inference fusions
+    are on: nothing is recorded for a backward pass, so a BatchNorm with running statistics is a per-channel affine that
+    can be folded into the planes a convolution gathers and into the epilogue of the convolution before it.  With
+    gradients enabled, eval mode keeps its differentiable path (frozen-BatchNorm fine-tuning)."""
+    return _INFER_FUSION and not module.training and not torch.is_grad_enabled()
+
+
+def bn_eval_coefs(bn) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(scale, shift) of an eval-mode BatchNorm from its running statistics: BN(x) = x*scale + shift.  The one place these
+    coefficients are computed (batchnorm_rows, bn_act_conv and the inference epilogue all use it)."""
+    w = bn.weight if bn.weight is not None else 1.0
+    scale = w * torch.rsqrt(bn.running_var + bn.eps)
+    shift = (bn.bias if bn.bias is not None else 0.0) - bn.running_mean * scale
+    return scale, shift
+
+
+def bn_act_conv_route(bn, x, weight, kmap: "KernelMap") -> str:
+    """How bn_act_conv runs conv(act(BatchNorm(x))): 'fused' (training, BNActConv: the BatchNorm apply pass writes the
+    planes the convolution gathers), 'eval_split' (eval mode without gradients: one split_planes pass applies the
+    running-statistics affine + activation and writes the planes; no autograd node) or 'unfused' (batchnorm_rows, then
+    SparseConv).  The fused forms need the plane-gather tensor-core path."""
+    K, Cin, Cout = weight.shape
+    if bn.running_mean is None or not x.is_cuda:
+        return "unfused"
+    if bn.training:
+        ok = (conv_path("fwd", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) == "planes"
+              and conv_path("dgrad", Cout, Cin, kmap.K, kmap.nbr, kmap.n_in) == "planes"
+              and conv_path("wgrad", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) == "planes")
+        return "fused" if ok else "unfused"
+    if inference_fusion_active(bn) and conv_path("fwd", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) == "planes":
+        return "eval_split"
+    return "unfused"
+
+
 def bn_act_conv(bn, x: torch.Tensor, act: int, group, weight, bias, kmap: "KernelMap", packs=None) -> torch.Tensor:
     """conv(act(BatchNorm(x))) — fused (BNActConv) when the layer runs on the plane-gather tensor-core path in training
-    mode, the two separate nodes otherwise."""
-    K, Cin, Cout = weight.shape
-    fused = (bn.training and bn.running_mean is not None and x.is_cuda
-             and conv_path("fwd", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) == "planes"
-             and conv_path("dgrad", Cout, Cin, kmap.K, kmap.nbr, kmap.n_in) == "planes"
-             and conv_path("wgrad", Cin, Cout, kmap.K, kmap.nbr, kmap.n_out) == "planes")
-    if not fused:
+    mode, one split pass + the convolution in eval mode without gradients, the two separate nodes otherwise
+    (bn_act_conv_route)."""
+    route = bn_act_conv_route(bn, x, weight, kmap)
+    if route == "eval_split":
+        scale, shift = bn_eval_coefs(bn)
+        planes = split_planes(x.contiguous(), scale.contiguous(), shift.contiguous(), act)
+        return conv_apply(x, weight, kmap.nbr, kmap.n_out, False, None, bias.view(-1).contiguous() if bias is not None else None,
+                          packs=packs, planes=planes)
+    if route == "unfused":
         return SparseConv.apply(batchnorm_rows(bn, x, act, group), weight, bias, kmap, packs)
     with torch.no_grad():
         bn.num_batches_tracked += 1
@@ -752,9 +838,7 @@ def batchnorm_rows(bn, x: torch.Tensor, act: int = ACT_NONE, group=None) -> torc
             mom = 1.0 / float(bn.num_batches_tracked)
         rm, rv = (bn.running_mean, bn.running_var) if bn.training else (None, None)
         return BatchNormAct.apply(x, gamma, beta, bn.eps, act, group, rm, rv, mom)
-    w = bn.weight if bn.weight is not None else 1.0
-    scale = w * torch.rsqrt(bn.running_var + bn.eps)
-    shift = (bn.bias if bn.bias is not None else 0.0) - bn.running_mean * scale
+    scale, shift = bn_eval_coefs(bn)
     if torch.is_grad_enabled() and (x.requires_grad or scale.requires_grad or shift.requires_grad):
         return _act_torch(x * scale + shift, act)
     return affine_act(x.contiguous(), scale.contiguous(), shift.contiguous(), act)
