@@ -255,6 +255,71 @@ int pasco_xattn_backward(const float* q, const float* k, const float* v, const u
                          const float* out, const float* dout, int32_t Q, int64_t P, int32_t H, int32_t D, float scale,
                          float* dq, float* dk, float* dv, pasco_stream_t s);
 
+/* ---- test-time post-processing: the M-subnet ensemble (pasco/models/ensembler.py:20-187, reached from
+ *      net_panoptic_sparse.py:245-294) and panoptic inference (pasco/models/helper.py:91-303, reached from
+ *      Net.step_inference, net_panoptic_sparse.py:539-648), on sparse rows of the X x Y x Z reference grid -------------
+ * A cell is the linear index (x*Y + y)*Z + z; cell maps are int32 [X*Y*Z] holding a row index or −1.                */
+
+/* transform_utils.py:55-76,160-181 (transform + sample_scene): cell_row[cell] = row of the subnet's hash table (keys
+ * with batch index 0) at round((T·(cell*0.2 + 0.1 + lo) − lo − 0.1) / 0.2), lo = (0, −25.6, −2), in fp32 with
+ * round-half-to-even, or −1; T = rows 0-2 of the 4x4 pose (host float[12], row-major).  cell_mask (NULL allowed)
+ * receives cell_row >= 0 as a byte, ready for pasco_mask_block_counts / pasco_mask_compact.                        */
+int pasco_pose_lookup(const uint64_t* table_keys, const int32_t* table_vals, int64_t capacity, const float T[12],
+                      int32_t X, int32_t Y, int32_t Z, int32_t* cell_row, uint8_t* cell_mask, pasco_stream_t s);
+/* mask[i] = 1 where cell_row[i] >= 0, other bytes untouched: the union of row sets (ensembler.py:100-112, 182-186) */
+int pasco_cell_mask_or(const int32_t* cell_row, int64_t n, uint8_t* mask, pasco_stream_t s);
+/* out[r] = cell_row[lin[r]] */
+int pasco_lookup_rows(const int32_t* cell_row, const int32_t* lin, int64_t n, int32_t* out, pasco_stream_t s);
+
+/* ensembler.py:40-58 for the masks: out[r, q] = sigmoid(logits[rows[r], q]) fp32 [n, Q]; optionally (hi != NULL) the
+ * bf16 planes hi = bf16(out), lo = bf16(out − hi) [n, Qp], Qp % 16 == 0, columns past Q zero; colsum (NULL allowed)
+ * [Q] = column sums, reduced from per-CTA partials in CTA order; nonzero (NULL allowed) [n] = row has a non-zero. */
+int pasco_mask_rows_sigmoid(const float* logits, const int32_t* rows, int64_t n, int32_t Q, float* out, void* hi,
+                            void* lo, int32_t Qp, float* colsum, uint8_t* nonzero, pasco_stream_t s);
+/* ensembler.py:88-129: for output row r at cell lin[r] and column j,
+ *   a = A[cell_a[cell], a_col[j]] (0 when there is no anchor row), b likewise from B, cell_b, b_col
+ *   v = (b_col != NULL and b_col[j] >= 0) ? (a*weight + b) / (weight + 1) : a,  then v *= gate[cell] when gate != NULL
+ * (b may be NULL when the subnet has no row: every b then reads as zero)
+ * out fp32 [n, q_out]; planes, colsum and nonzero as in pasco_mask_rows_sigmoid.  The last step of the ensemble passes
+ * the kept queries as a_col (the mean-IoU keep) and the ensembled occupancy as gate.                                */
+int pasco_mask_merge(const float* a, const int32_t* cell_a, int32_t qa, const float* b, const int32_t* cell_b, int32_t qb,
+                     const int32_t* lin, int64_t n, const int32_t* a_col, const int32_t* b_col, int32_t q_out,
+                     int32_t weight, const uint8_t* gate, float* out, void* hi, void* lo, int32_t Qp, float* colsum,
+                     uint8_t* nonzero, pasco_stream_t s);
+/* ensembler.py:166-176: out[r, :] = softmax(logits[rows[r], :]) over K channels */
+int pasco_softmax_rows(const float* logits, const int32_t* rows, int64_t n, int32_t K, float* out, pasco_stream_t s);
+/* utils.py:153-198 + ensembler.py:78-86: from the intersections inter [Q, pitch] (pasco_conv_wgrad_planes with K = 1)
+ * and the column sums, iou = inter / (sum_a + sum_b − inter) (0 where the union is 0); gated [Q, Q] = iou > threshold
+ * ? iou : 0 — the matrix the host hands to linear_sum_assignment.                                                   */
+int pasco_soft_iou(const float* inter, int32_t Q, int64_t pitch, const float* sum_a, const float* sum_b, float threshold,
+                   float* gated, pasco_stream_t s);
+/* ensembler.py:160-187 + net_panoptic_sparse.py:278-294 (max_prob): per row r at cell lin[r], the mean over the M <= 8
+ * subnets of probs[m][cell_rows[m][cell]] (a subnet without a row there counts as one-hot class 0); pred[r] = its first
+ * argmax, conf[r] = its max; gate (NULL allowed) [cells] receives pred != 0 at the cell.  probs / cell_rows are host
+ * arrays of device pointers.                                                                                         */
+int pasco_sem_ensemble(int32_t M, const float* const probs[], const int32_t* const cell_rows[], const int32_t* lin,
+                       int64_t n, int32_t K, int32_t* pred, float* conf, uint8_t* gate, pasco_stream_t s);
+/* helper.py:135-186 pass 1 over the mask probabilities probs [n, Q] with class probabilities query_probs [Q, K1]:
+ * a query is kept when its first-argmax label is neither 0 nor K1 − 1 and its max > object_mask_threshold; per row,
+ * win = (q << 1) | (m_q >= vox_occ_threshold) for the kept q maximising prob_q * m_q (lowest q on ties), −1 without a
+ * kept query; m_win = m_q, m_sum = the sum of m over kept queries.  areas int32 [2Q], zeroed by the caller: [0, Q) the
+ * mask_area and [Q, 2Q) the original_area of every query (integer counts).                                          */
+int pasco_panoptic_pass1(const float* probs, int64_t n, int32_t Q, const float* query_probs, int32_t K1,
+                         float object_mask_threshold, float vox_occ_threshold, int32_t* win, float* m_win, float* m_sum,
+                         int32_t* areas, pasco_stream_t s);
+/* helper.py:187-250 on one thread: the walk over kept queries in ascending order (overlap filter mask_area /
+ * original_area in double, stuff classes merged into their first segment, sequential ids).  seg_of / cls_of int32 [Q]:
+ * the segment id a query paints (0 none) and its semantic class (−1 for merged stuff, which keeps semantic 0).
+ * records int32 [1 + 4Q]: the segment count, then per segment (query, class, float bits of the class probability,
+ * isthing).  thing_mask bit c = class c is a thing class; K1 <= 65.                                                 */
+int pasco_panoptic_segments(const float* query_probs, int32_t Q, int32_t K1, float object_mask_threshold,
+                            double overlap_threshold, uint64_t thing_mask, const int32_t* areas, int32_t* seg_of,
+                            int32_t* cls_of, int32_t* records, pasco_stream_t s);
+/* helper.py:236-247 pass 2 from the pass-1 records: panoptic / semantic int32 [n] and the confidence fp32 [n] =
+ * m_win / (m_sum + 1e-8) on rows painted by a non-merged segment, 0 elsewhere.                                     */
+int pasco_panoptic_pass2(const int32_t* win, const float* m_win, const float* m_sum, int64_t n, const int32_t* seg_of,
+                         const int32_t* cls_of, int32_t* panoptic, int32_t* semantic, float* confidence, pasco_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -61,6 +61,17 @@ PROTOTYPES = {
     "pasco_xattn_forward": (C.c_int, [_p, _p, _p, _p, _i32, _i64, _i32, _i32, C.c_float, _p, _p, _p]),
     "pasco_xattn_backward": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, C.c_float, _p, _p, _p, _p]),
     "pasco_bn_bwd_apply": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i32, _p, _p, _p, _p, _p]),
+    "pasco_pose_lookup": (C.c_int, [_p, _p, _i64, _p, _i32, _i32, _i32, _p, _p, _p]),
+    "pasco_cell_mask_or": (C.c_int, [_p, _i64, _p, _p]),
+    "pasco_lookup_rows": (C.c_int, [_p, _p, _i64, _p, _p]),
+    "pasco_mask_rows_sigmoid": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _p, _i32, _p, _p, _p]),
+    "pasco_mask_merge": (C.c_int, [_p, _p, _i32, _p, _p, _i32, _p, _i64, _p, _p, _i32, _i32, _p, _p, _p, _p, _i32, _p, _p, _p]),
+    "pasco_softmax_rows": (C.c_int, [_p, _p, _i64, _i32, _p, _p]),
+    "pasco_soft_iou": (C.c_int, [_p, _i32, _i64, _p, _p, C.c_float, _p, _p]),
+    "pasco_sem_ensemble": (C.c_int, [_i32, _p, _p, _p, _i64, _i32, _p, _p, _p, _p]),
+    "pasco_panoptic_pass1": (C.c_int, [_p, _i64, _i32, _p, _i32, C.c_float, C.c_float, _p, _p, _p, _p, _p]),
+    "pasco_panoptic_segments": (C.c_int, [_p, _i32, _i32, C.c_float, C.c_double, C.c_uint64, _p, _p, _p, _p, _p]),
+    "pasco_panoptic_pass2": (C.c_int, [_p, _p, _p, _i64, _p, _p, _p, _p, _p, _p]),
 }
 
 _lib: Optional[C.CDLL] = None

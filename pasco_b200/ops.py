@@ -981,3 +981,145 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
     if x.is_cuda and x.ndim == 2 and _linear_tc_ok(x.shape[0], weight.shape[1], weight.shape[0]):
         return LinearTC.apply(x, weight, bias)
     return torch.nn.functional.linear(x, weight, bias)
+
+
+# ----------------------------------------------------------------------------------------------
+# test-time post-processing (panoptic.cu): M-subnet ensemble and panoptic inference on sparse rows of the reference grid
+# ----------------------------------------------------------------------------------------------
+def plane_cols(q: int) -> int:
+    """Columns of the bf16 planes of a [N, q] mask matrix: q rounded up to the tensor-core channel rule (16)."""
+    return (q + 15) // 16 * 16
+
+
+def pose_lookup(table: HashTable, T: torch.Tensor, size: Sequence[int]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Every cell of the reference grid `size` → the row of `table` (keys with batch index 0) at the cell's nearest
+    voxel under the pose T (transform_utils.transform): (cell_row int32 [cells], −1 = none; cell_row >= 0 as uint8)."""
+    cells = int(size[0]) * int(size[1]) * int(size[2])
+    dev = table.keys.device
+    cell_row = torch.empty(cells, dtype=torch.int32, device=dev)
+    mask = torch.empty(cells, dtype=torch.uint8, device=dev)
+    t = T.detach().to("cpu", torch.float32).reshape(4, 4)[:3].contiguous().view(-1).tolist()
+    call("pasco_pose_lookup", ptr(table.keys), ptr(table.vals), table.capacity, (C.c_float * 12)(*t), int(size[0]),
+         int(size[1]), int(size[2]), ptr(cell_row), ptr(mask))
+    return cell_row, mask
+
+
+def cell_mask_or(cell_row: torch.Tensor, mask: torch.Tensor) -> None:
+    call("pasco_cell_mask_or", ptr(cell_row), cell_row.shape[0], ptr(mask))
+
+
+def lookup_rows(cell_row: torch.Tensor, lin: torch.Tensor) -> torch.Tensor:
+    out = torch.empty(lin.shape[0], dtype=torch.int32, device=lin.device)
+    call("pasco_lookup_rows", ptr(cell_row), ptr(lin), lin.shape[0], ptr(out))
+    return out
+
+
+def _mask_outputs(n: int, q: int, dev, planes: bool, colsum: bool):
+    qp = plane_cols(q)
+    out = torch.empty(n, q, dtype=torch.float32, device=dev)
+    hi = torch.empty(n, qp, dtype=torch.bfloat16, device=dev) if planes else None
+    lo = torch.empty(n, qp, dtype=torch.bfloat16, device=dev) if planes else None
+    cs = torch.empty(q, dtype=torch.float32, device=dev) if colsum else None
+    nz = torch.empty(n, dtype=torch.uint8, device=dev)
+    return out, hi, lo, qp, cs, nz
+
+
+def mask_rows_sigmoid(logits: torch.Tensor, rows: torch.Tensor, planes: bool = True):
+    """sigmoid(logits[rows]) → (probs fp32 [n, Q], (hi, lo) bf16 planes [n, plane_cols(Q)] or None, column sums [Q] or
+    None, non-zero row flags uint8 [n])."""
+    logits = logits.detach().float().contiguous()
+    out, hi, lo, qp, cs, nz = _mask_outputs(rows.shape[0], logits.shape[1], logits.device, planes, planes)
+    call("pasco_mask_rows_sigmoid", ptr(logits), ptr(rows), rows.shape[0], logits.shape[1], ptr(out), ptr(hi), ptr(lo),
+         qp, ptr(cs), ptr(nz))
+    return out, ((hi, lo) if planes else None), cs, nz
+
+
+def mask_merge(a: torch.Tensor, cell_a: torch.Tensor, b: Optional[torch.Tensor], cell_b: Optional[torch.Tensor],
+               lin: torch.Tensor, a_col: torch.Tensor, b_col: Optional[torch.Tensor], weight: int,
+               gate: Optional[torch.Tensor] = None, planes: bool = True):
+    """Rows at the cells lin: column j = (a[:, a_col[j]]·weight + b[:, b_col[j]]) / (weight + 1) (a missing row is a
+    zero row), times gate[cell] when given.  Returns what mask_rows_sigmoid returns."""
+    q = a_col.shape[0]
+    out, hi, lo, qp, cs, nz = _mask_outputs(lin.shape[0], q, a.device, planes, planes)
+    call("pasco_mask_merge", ptr(a), ptr(cell_a), a.shape[1], ptr(b), ptr(cell_b), b.shape[1] if b is not None else 0,
+         ptr(lin), lin.shape[0], ptr(a_col), ptr(b_col), q, int(weight), ptr(gate), ptr(out), ptr(hi), ptr(lo), qp, ptr(cs),
+         ptr(nz))
+    return out, ((hi, lo) if planes else None), cs, nz
+
+
+def softmax_rows(logits: torch.Tensor, rows: torch.Tensor) -> torch.Tensor:
+    logits = logits.detach().float().contiguous()
+    out = torch.empty(rows.shape[0], logits.shape[1], dtype=torch.float32, device=logits.device)
+    call("pasco_softmax_rows", ptr(logits), ptr(rows), rows.shape[0], logits.shape[1], ptr(out))
+    return out
+
+
+def soft_iou(a_prob, a_planes, a_sum, b_prob, b_planes, b_sum, nbr: torch.Tensor, threshold: float) -> torch.Tensor:
+    """Gated soft IoU [Q, Q] between the mask sets A (rows of the anchor) and B; nbr int32 [N_b] = the anchor row at the
+    cell of every row of B (−1 none).  The intersections are the weight gradient of a K = 1 convolution from A's planes
+    to B's (bf16x3, fixed-order reduction); a width outside the tensor-core channel rule takes the CUDA-core kernel."""
+    q = a_prob.shape[1]
+    dev = a_prob.device
+    nb = b_prob.shape[0]
+    nbr = nbr.view(1, -1)
+    qp = plane_cols(q)
+    # conv_path only decides tensor cores vs CUDA cores here: with K = 1 it names the register-gather kernel, but the
+    # masks already exist as planes, so every tensor-core case takes the plane-gather weight gradient
+    if conv_path("wgrad", qp, qp, 1, nbr, nb) == "simt":
+        inter = torch.zeros(1, q, q, dtype=torch.float32, device=dev)
+        pitch = q
+        if nb:
+            call("pasco_conv_wgrad_simt", ptr(a_prob), ptr(nbr), 1, nb, q, q, ptr(b_prob), ptr(inter))
+    else:
+        inter = torch.zeros(1, qp, qp, dtype=torch.float32, device=dev)
+        pitch = qp
+        if nb:
+            (ah, al), (bh, bl) = a_planes, b_planes
+            call("pasco_conv_wgrad_planes", ptr(ah), ptr(al), a_prob.shape[0], ptr(nbr), 1, nb, qp, qp, ptr(bh), ptr(bl),
+                 ptr(inter), 3, 0, 0)
+    gated = torch.empty(q, q, dtype=torch.float32, device=dev)
+    call("pasco_soft_iou", ptr(inter), q, pitch, ptr(a_sum), ptr(b_sum), float(threshold), ptr(gated))
+    return gated
+
+
+def sem_ensemble(probs: List[torch.Tensor], cell_rows: List[torch.Tensor], lin: torch.Tensor,
+                 gate: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Mean class distribution over the subnets at the cells lin (absent subnet = one-hot class 0) → (argmax int32,
+    max fp32); gate (uint8 [cells], zeroed) receives argmax != 0 at those cells."""
+    n, K, M = lin.shape[0], probs[0].shape[1], len(probs)
+    pred = torch.empty(n, dtype=torch.int32, device=lin.device)
+    conf = torch.empty(n, dtype=torch.float32, device=lin.device)
+    call("pasco_sem_ensemble", M, (C.c_void_p * M)(*[ptr(p) for p in probs]), (C.c_void_p * M)(*[ptr(c) for c in cell_rows]),
+         ptr(lin), n, K, ptr(pred), ptr(conf), ptr(gate))
+    return pred, conf
+
+
+def panoptic(probs: torch.Tensor, query_probs: torch.Tensor, overlap_threshold: float, object_mask_threshold: float,
+             thing_ids: Sequence[int], vox_occ_threshold: float = 0.3):
+    """helper.py:135-263 for one prediction: probs fp32 [N, Q] mask probabilities, query_probs fp32 [Q, K1].
+    Returns (panoptic int32 [N], semantic int32 [N], confidence fp32 [N], records int32 [1 + 4Q] on the host)."""
+    n, q = probs.shape
+    K1 = query_probs.shape[1]
+    dev = probs.device
+    qp = query_probs.detach().float().contiguous()
+    win = torch.empty(n, dtype=torch.int32, device=dev)
+    m_win = torch.empty(n, dtype=torch.float32, device=dev)
+    m_sum = torch.empty(n, dtype=torch.float32, device=dev)
+    areas = torch.zeros(2 * max(q, 1), dtype=torch.int32, device=dev)
+    seg_of = torch.empty(max(q, 1), dtype=torch.int32, device=dev)
+    cls_of = torch.empty(max(q, 1), dtype=torch.int32, device=dev)
+    records = torch.zeros(1 + 4 * q, dtype=torch.int32, device=dev)
+    pan = torch.empty(n, dtype=torch.int32, device=dev)
+    sem = torch.empty(n, dtype=torch.int32, device=dev)
+    conf = torch.empty(n, dtype=torch.float32, device=dev)
+    if q == 0:
+        return pan.zero_(), sem.zero_(), conf.zero_(), records.cpu()
+    mask = 0
+    for c in thing_ids:
+        mask |= 1 << int(c)
+    call("pasco_panoptic_pass1", ptr(probs.contiguous()), n, q, ptr(qp), K1, float(object_mask_threshold),
+         float(vox_occ_threshold), ptr(win), ptr(m_win), ptr(m_sum), ptr(areas))
+    call("pasco_panoptic_segments", ptr(qp), q, K1, float(object_mask_threshold), float(overlap_threshold), mask,
+         ptr(areas), ptr(seg_of), ptr(cls_of), ptr(records))
+    call("pasco_panoptic_pass2", ptr(win), ptr(m_win), ptr(m_sum), n, ptr(seg_of), ptr(cls_of), ptr(pan), ptr(sem), ptr(conf))
+    return pan, sem, conf, records.cpu()

@@ -1,0 +1,186 @@
+"""Panoptic scene completion with uncertainty: PascoNet.predict, the engine's form of what scripts/eval.py gets from the
+reference's Net.forward(..., Ts, return_ensemble=True) (net_panoptic_sparse.py:210-310) followed by Net.step_inference's
+panoptic_inference on every subnet and on the ensemble (net_panoptic_sparse.py:539-648, helper.py:91-303).
+
+Everything after the forward runs on the kernels of csrc/panoptic.cu, on sparse rows of the 256x256x32 reference grid:
+
+  warp            every reference cell looks up the nearest source voxel under the subnet's pose (pasco_pose_lookup), the
+                  row compaction turns the cell map into ascending cells `lin` (ME.to_sparse order) and source rows
+  activate        sigmoid (masks, with bf16 planes and column sums for the IoU) or softmax (semantic logits) of those rows
+  semantic        mean of the M class distributions per cell (an absent subnet counts as one-hot class 0)
+  masks           subnet 0 is the anchor; every later subnet is matched to it by soft IoU (a K = 1 weight gradient, then
+                  SciPy's linear_sum_assignment on the host, as in the reference) and averaged into it on the union rows
+  panoptic        pass 1 (winner record per voxel, integer areas per query), the sequential segment walk on one device
+                  thread, pass 2 (labels and confidences); the segment records are the one copy to the host per entry
+
+The torch restatement in ensemble.py is the reference these kernels are tested against.
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Optional, Sequence
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+from . import ops
+
+SCENE = (256, 256, 32)
+THING_IDS = (1, 2, 3, 4, 5, 6, 7, 8)          # pasco/data/semantic_kitti/params.py
+
+
+def _coords4(c: torch.Tensor) -> torch.Tensor:
+    """[N, 4] (batch, x, y, z) or [N, 3] rows → int32 [N, 4] with batch index 0."""
+    c = c[:, -3:].to(torch.int32)
+    return torch.cat([torch.zeros_like(c[:, :1]), c], 1).contiguous()
+
+
+def warp(coords: torch.Tensor, T: torch.Tensor, size=SCENE):
+    """Rows of a subnet (integer coords in its augmented frame) → (lin int32 [N'] ascending reference cells,
+    cell_row int32 [cells] = row index at each cell or −1, src int32 [N'] = the source row of every new row)."""
+    table, _ = ops.hash_insert(_coords4(coords))
+    cell_src, mask = ops.pose_lookup(table, T, size)
+    lin, cell_row, _ = ops.compact(mask)
+    return lin, cell_row, ops.lookup_rows(cell_src, lin)
+
+
+def _drop_zero_rows(prob: torch.Tensor, lin: torch.Tensor, nz: torch.Tensor):
+    """ME.to_sparse drops rows whose mask probabilities are all zero."""
+    kept, _, n = ops.compact(nz)
+    if n == prob.shape[0]:
+        return prob, lin
+    return ops._gather_rows(prob, kept), ops.lookup_rows(lin, kept)
+
+
+def _segments(records: torch.Tensor, query_probs: torch.Tensor) -> List[Dict]:
+    r = records.numpy()
+    out = []
+    for s in range(int(r[0])):
+        q, cls, conf, thing = r[1 + 4 * s: 5 + 4 * s]
+        out.append({"id": s + 1, "isthing": bool(thing), "category_id": int(cls), "query_id": int(q),
+                    "confidence": float(np.array(conf, dtype=np.int32).view(np.float32)),
+                    "all_class_probs": query_probs[int(q)]})
+    return out
+
+
+def postprocess(preds: Sequence[Dict], sems: Sequence, Ts: Sequence[torch.Tensor], *, thing_ids=THING_IDS,
+                overlap_threshold: float = 0.4, object_mask_threshold: float = 0.7, iou_threshold: float = 0.2,
+                size=SCENE, matches: Optional[list] = None) -> List[Dict]:
+    """preds[m] = {"voxel_logits": (logits [N_m, Q], coords [N_m, 3 or 4]), "query_logits": [1, Q, K1]} and sems[m] =
+    (semantic logits [S_m, K], coords) of subnet m, in the subnet's frame under pose Ts[m].  Returns M + 1 entries (the
+    subnets, then the ensemble); `matches` (a list) receives the (anchor, subnet) Hungarian assignment of every step."""
+    from scipy.optimize import linear_sum_assignment
+    M = len(preds)
+    if not 1 <= M <= 8:
+        raise ValueError(f"predict: 1 to 8 subnets (the semantic ensemble kernel's limit), got {M}")
+    dev = preds[0]["voxel_logits"][0].device
+    cells = int(size[0]) * int(size[1]) * int(size[2])
+    Q = preds[0]["voxel_logits"][0].shape[1]
+
+    masks, qprobs, sem_rows = [], [], []
+    for m in range(M):
+        logits, coords = preds[m]["voxel_logits"]
+        lin, cell_row, src = warp(coords, Ts[m], size)
+        prob, planes, colsum, nz = ops.mask_rows_sigmoid(logits, src, planes=M > 1)
+        masks.append(dict(prob=prob, lin=lin, cell=cell_row, planes=planes, colsum=colsum, nz=nz))
+        qprobs.append(F.softmax(preds[m]["query_logits"].detach().float(), -1))
+        s_logits, s_coords = sems[m]
+        s_lin, s_cell, s_src = warp(s_coords, Ts[m], size)
+        sem_rows.append((ops.softmax_rows(s_logits, s_src), s_lin, s_cell))
+
+    # semantic completion: every subnet on its own rows, the ensemble on the union of the rows (ensembler.py:160-187)
+    ssc = [(lin,) + ops.sem_ensemble([p], [cell], lin) for p, lin, cell in sem_rows]
+    union = torch.zeros(cells, dtype=torch.uint8, device=dev)
+    for _, _, cell in sem_rows:
+        ops.cell_mask_or(cell, union)
+    u_lin, _, _ = ops.compact(union)
+    gate = torch.zeros(cells, dtype=torch.uint8, device=dev)
+    ssc.append((u_lin,) + ops.sem_ensemble([p for p, _, _ in sem_rows], [c for _, _, c in sem_rows], u_lin, gate))
+
+    # masks: running average of the matched queries on the union rows (ensembler.py:20-129)
+    a = masks[0]
+    a_q = qprobs[0].clone()
+    ious = []
+    cols = torch.arange(Q, dtype=torch.int32, device=dev)
+    if M == 1:
+        ens = ops.mask_merge(a["prob"], a["cell"], None, None, a["lin"], cols, None, 0, gate, planes=False)
+        ens_prob, ens_lin = _drop_zero_rows(ens[0], a["lin"], ens[3])
+    for i in range(1, M):
+        b = masks[i]
+        gated = ops.soft_iou(a["prob"], a["planes"], a["colsum"], b["prob"], b["planes"], b["colsum"],
+                             ops.lookup_rows(a["cell"], b["lin"]), iou_threshold).cpu().numpy()
+        ai, bi = linear_sum_assignment(1.0 - gated)                                    # the reference's host crossing
+        if matches is not None:
+            matches.append((ai, bi))
+        ious.append(torch.from_numpy(gated[ai, bi]))
+        ai_t, bi_t = torch.as_tensor(ai, device=dev), torch.as_tensor(bi, device=dev)
+        a_q[:, ai_t] = (a_q[:, ai_t] * i + qprobs[i][:, bi_t]) / (i + 1)
+        b_of = np.full(Q, -1, dtype=np.int32)
+        b_of[ai] = bi
+        union = torch.zeros(cells, dtype=torch.uint8, device=dev)
+        ops.cell_mask_or(a["cell"], union)
+        ops.cell_mask_or(b["cell"], union)
+        lin, cell, _ = ops.compact(union)
+        if i < M - 1:
+            prob, planes, colsum, nz = ops.mask_merge(a["prob"], a["cell"], b["prob"], b["cell"], lin, cols,
+                                                      torch.as_tensor(b_of, device=dev), i)
+            a = dict(prob=prob, lin=lin, cell=cell, planes=planes, colsum=colsum)
+            continue
+        # last step: the mean-IoU keep, the ensembled occupancy gate and the all-zero-row drop in the same pass
+        keep = (torch.stack(ious, 0).mean(0) > iou_threshold).numpy()
+        kept = np.nonzero(keep)[0].astype(np.int32)
+        if len(kept) == 0:                       # no query kept: every row is all zeros and ME.to_sparse drops it
+            ens_prob, ens_lin = torch.zeros(0, 0, device=dev), lin[:0]
+        else:
+            prob, _, _, nz = ops.mask_merge(a["prob"], a["cell"], b["prob"], b["cell"], lin,
+                                            torch.as_tensor(kept, device=dev), torch.as_tensor(b_of[kept], device=dev), i,
+                                            gate, planes=False)
+            ens_prob, ens_lin = _drop_zero_rows(prob, lin, nz)
+        a_q = a_q[:, torch.as_tensor(keep, device=dev)]
+
+    entries = []
+    rows = [_drop_zero_rows(mk["prob"], mk["lin"], mk["nz"]) for mk in masks] + [(ens_prob, ens_lin)]
+    for (prob, lin), qp, (s_lin, s_pred, s_conf) in zip(rows, qprobs + [a_q], ssc):
+        pan, sem, conf, records = ops.panoptic(prob, qp[0], overlap_threshold, object_mask_threshold, thing_ids)
+        entries.append({"lin": lin.long(), "panoptic_seg": pan, "semantic_seg": sem, "vox_confidence": conf,
+                        "segments_info": _segments(records, qp[0]), "ssc_lin": s_lin.long(), "ssc_pred": s_pred,
+                        "ssc_confidence": s_conf, "query_probs": qp[0]})
+    return entries
+
+
+_DENSE = {"panoptic_seg": ("lin", 0.0), "semantic_seg": ("lin", 0.0), "vox_confidence": ("lin", 0.0),
+          "ssc_pred": ("ssc_lin", 0.0), "ssc_confidence": ("ssc_lin", 1.0)}
+
+
+def to_dense(entry: Dict, key: str, size=SCENE) -> torch.Tensor:
+    """The reference's dense [X, Y, Z] volume of one per-row output of an entry (metric code indexes these).  Cells
+    without a row hold the reference's fill: 1.0 for ssc_confidence (an empty cell is one-hot class 0), 0 elsewhere."""
+    rows_key, fill = _DENSE[key]
+    lin, v = entry[rows_key], entry[key]
+    X, Y, Z = (int(s) for s in size)
+    coords = torch.stack([torch.zeros_like(lin), lin // (Y * Z), (lin // Z) % Y, lin % Z], 1).to(torch.int32).contiguous()
+    dense = torch.full((1, 1, X, Y, Z), fill, dtype=torch.float32, device=v.device)
+    mc, st = ops._geom((0, 0, 0), (1, 1, 1))
+    ops.call("pasco_to_dense", ops.ptr(v.float().view(-1, 1).contiguous()), ops.ptr(coords), lin.shape[0], 1, mc, st,
+             ops.ptr(dense), 1, X, Y, Z, None)
+    dense = dense.view(X, Y, Z)
+    return dense.to(v.dtype) if v.dtype != torch.float32 else dense
+
+
+def predict(net, in_feats, in_coords, global_min, global_max, min_Cs, max_Cs, Ts=None, *, thing_ids=THING_IDS,
+            overlap_threshold=0.4, object_mask_threshold=0.7, iou_threshold=0.2, scene_size=SCENE) -> List[Dict]:
+    """PascoNet.predict: the eval forward (forward(test=True), no gradients), then postprocess."""
+    if net.training:
+        raise RuntimeError("PascoNet.predict runs the eval forward: call net.eval() first")
+    M = net.n_infers
+    if Ts is None:
+        Ts = [torch.eye(4) for _ in range(M)]
+    if len(Ts) != M:
+        raise ValueError(f"PascoNet.predict: {len(Ts)} poses for {M} subnets")
+    with torch.no_grad():
+        ret = net(in_feats, in_coords, global_min, global_max, min_Cs, max_Cs, predict_panop=True, test=True)
+        preds = [{"voxel_logits": (p["voxel_logits"].F, p["voxel_logits"].C), "query_logits": p["query_logits"]}
+                 for p in ret["panop_predictions"]]
+        sems = [(s.F, s.C) for s in ret["sem_logits_at_scales"][1]]
+        return postprocess(preds, sems, Ts, thing_ids=thing_ids, overlap_threshold=overlap_threshold,
+                           object_mask_threshold=object_mask_threshold, iou_threshold=iou_threshold, size=scene_size)
