@@ -41,14 +41,14 @@ def synthetic_batch(grid, occ, n_infers=1, in_ch=283, n_classes=20, seed=0):
     return batch
 
 
-def build_net(n_infers=1, f=64, heavy_decoder=False, n_classes=20, in_channels=283):
+def build_net(n_infers=1, f=64, heavy_decoder=False, n_classes=20, in_channels=283, num_queries=100):
     from pasco.models.net_panoptic_sparse import Net
     freqs = {f"1_{s}": np.ones(n_classes) for s in (1, 2, 4)}
     torch.manual_seed(0)
     return Net(n_classes=n_classes, class_names=[str(i) for i in range(n_classes)],
                class_weights=torch.ones(n_classes), encoder_dropouts=[0.0] * 3, decoder_dropouts=[0.0] * 3,
                dense3d_dropout=0.0, n_infers=n_infers, class_frequencies=freqs, in_channels=in_channels,
-               num_queries=100, f=f, heavy_decoder=heavy_decoder)
+               num_queries=num_queries, f=f, heavy_decoder=heavy_decoder)
 
 
 def forward(net, batch, test=False, is_predict_panop=True):

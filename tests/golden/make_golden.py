@@ -20,18 +20,12 @@ sys.path[:0] = [os.path.join(ROOT, "oracle", "shims"), os.path.join(ROOT, "compa
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+import parity  # noqa: E402
 from recipe import fill_state_dict  # noqa: E402
 from run_reference_on_oracle import build_net, forward  # noqa: E402
 from pasco_b200.synthetic import make_scene  # noqa: E402
-import me_oracle as OR  # noqa: E402
 
 GRID, OCC, SEED, STEP = (64, 64, 8), 0.05, 0, 8
-
-
-def canon(st):
-    C = st.C.cpu()
-    order = torch.argsort(OR.pack_keys(C))
-    return C[order].numpy().astype(np.int16), st.F.detach().cpu()[order].numpy()
 
 
 def make(n_infers, tag, step):
@@ -46,19 +40,7 @@ def make(n_infers, tag, step):
     manifest = {k: list(v.shape) for k, v in sd.items()
                 if not k.startswith(("unet3d.transformer_predictor.", "unet3d.decoder_generative.transformer_predictor.",
                                      "criterion."))}
-    for m in range(n_infers):
-        sfx = "" if n_infers == 1 else f"_m{m}"
-        for s, lg in out["sem_logits_at_scales"].items():
-            c, f = canon(lg[m])
-            arrays[f"sem{s}{sfx}_C"], arrays[f"sem{s}{sfx}_F"] = c, f[::step]
-            arrays[f"sem{s}{sfx}_sum"] = np.array([f.sum(dtype=np.float64), np.abs(f).sum(dtype=np.float64)])
-        p = out["panop_predictions"][m]
-        arrays[f"query_logits{sfx}"] = p["query_logits"][0].numpy()
-        c, f = canon(p["voxel_logits"])
-        arrays[f"vox{sfx}_C"], arrays[f"vox{sfx}_F"] = c, f[::step]
-        arrays[f"vox{sfx}_sum"] = np.array([f.sum(dtype=np.float64), np.abs(f).sum(dtype=np.float64)])
-        for i, aux in enumerate(p["aux_outputs"]):
-            arrays[f"aux{i}_query_logits{sfx}"] = aux["query_logits"][0].numpy()
+    parity.collect(out, n_infers, step, arrays, parity.rows)
     np.savez_compressed(os.path.join(HERE, f"net_{tag}.npz"), **arrays)
     json.dump({"grid": GRID, "occ": OCC, "seed": SEED, "row_step": step, "n_infers": n_infers, "params": manifest},
               open(os.path.join(HERE, f"net_{tag}_manifest.json"), "w"), indent=0)

@@ -12,7 +12,7 @@ an eval forward on them is degenerate, so each network is calibrated first:
   3. all running statistics (small; the weights are not stored) go into the case's npz as `stat::<reference name>`.
 
 Then net.eval() runs with test=True on the net_cfg1 scene at M = 1 and M = 2, and once at benchmark scale (256x256x32
-@10 %, M = 1).  Each case is stored as r2_big_eval-style summaries (make_golden_r2.collect: row count, wrap-around key sum
+@10 %, M = 1).  Each case is stored as r2_big_eval-style summaries (parity.summary: row count, wrap-around key sum
 and xor of the coordinate set, Σ / Σ|·| / max|·| of the features, a row subsample in sorted-key order, the query logits
 of all four levels), one file per case: net_cfg1_infer_<case>.npz, case m1 / m2 / big.  The benchmark-scale network is
 calibrated on a benchmark-scale scene: activations grow with the occupancy, and statistics from the small scene would
@@ -21,21 +21,17 @@ The generator asserts that no eval forward changed a running statistic or num_ba
 """
 import json
 import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-sys.path[:0] = [os.path.join(ROOT, "oracle", "shims"), os.path.join(ROOT, "compat"), "/root/reference", ROOT,
-                os.path.join(ROOT, "oracle"), os.path.join(ROOT, "oracle", "tools"), HERE]
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from recipe import fill_state_dict  # noqa: E402
-from run_reference_on_oracle import build_net, forward  # noqa: E402
-from pasco_b200.synthetic import make_scene  # noqa: E402
-from make_golden_r2 import collect  # noqa: E402
+import make_golden  # noqa: F401  (sets sys.path to the reference, the oracle and the shims)
+import parity
+from make_golden import HERE
+from recipe import fill_state_dict
+from run_reference_on_oracle import build_net, forward
+from pasco_b200.synthetic import make_scene
 
 GRID, OCC, SEED, CALIB_SEED = (64, 64, 8), 0.05, 0, 1
 BIG_GRID, BIG_OCC = (256, 256, 32), 0.10
@@ -84,7 +80,7 @@ def main():
         names = {k: list(v.shape) for k, v in st.items() if not k.endswith(".num_batches_tracked")}
         assert all(int(v) == 1 for k, v in st.items() if k.endswith(".num_batches_tracked"))
         arrays = {f"stat::{k}": st[k].numpy() for k in names}
-        collect(eval_forward(net, make_scene(grid, occ, M, seed=SEED)), M, step, arrays)
+        parity.collect(eval_forward(net, make_scene(grid, occ, M, seed=SEED)), M, step, arrays, parity.summary)
         np.savez_compressed(os.path.join(HERE, f"net_cfg1_infer_{tag}.npz"), **arrays)
         meta["cases"][tag] = {"grid": list(grid), "occ": occ, "seed": SEED, "row_step": step, "n_infers": M, "test": True,
                               "deterministic_sampling": False, "heavy_decoder": False, "n_classes": 20,

@@ -21,17 +21,15 @@ import os
 import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-sys.path[:0] = [os.path.join(ROOT, "oracle", "shims"), os.path.join(ROOT, "compat"), "/root/reference", ROOT,
-                os.path.join(ROOT, "oracle"), os.path.join(ROOT, "oracle", "tools"), HERE]
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from recipe import fill_state_dict  # noqa: E402
-from run_reference_on_oracle import build_net, forward  # noqa: E402
-from pasco_b200.synthetic import make_scene  # noqa: E402
+import make_golden  # noqa: F401  (sets sys.path to the reference, the oracle and the shims)
+import parity
+from make_golden import HERE
+from recipe import fill_state_dict
+from run_reference_on_oracle import build_net, forward
+from pasco_b200.synthetic import make_scene
 
 GRAD_PARAMS = [
     "feat.PPmodel.1.weight", "unet3d.encoder.enc_in_feats.kernel", "unet3d.encoder.s1.0.net.2.kernel",
@@ -49,25 +47,6 @@ GRAD_PARAMS = [
 ]
 
 
-def keys_of(C):
-    c = torch.as_tensor(C).long()
-    return ((c[:, 0] + 32768) << 48) | ((c[:, 1] + 32768) << 32) | ((c[:, 2] + 32768) << 16) | (c[:, 3] + 32768)
-
-
-def summarise(arrays, name, C, F, step):
-    """Canonical (sorted-key) summary of one sparse output: row count, wrap-around key sum and xor (bit-exact coordinate
-    set identity), sum / abs-sum of the features, every `step`-th row."""
-    k = keys_of(C.cpu())
-    order = torch.argsort(k)
-    k, F = k[order], F.detach().cpu()[order]
-    kn = k.numpy()
-    arrays[f"{name}_n"] = np.array([len(kn)], dtype=np.int64)
-    arrays[f"{name}_ksum"] = np.array([np.add.reduce(kn.astype(np.uint64)), np.bitwise_xor.reduce(kn.astype(np.uint64))], dtype=np.uint64)
-    arrays[f"{name}_Fsum"] = np.array([F.double().sum().item(), F.double().abs().sum().item(), F.abs().max().item()])
-    arrays[f"{name}_subK"] = kn[::step]
-    arrays[f"{name}_subF"] = F[::step].numpy()
-
-
 def _caller_coords(names):
     """Coordinates of the rows being ranked, read from the calling frame of the reference's
     predict_completion_sem_logit (decoder_v3.py:319-394: `sem_logit` / `x` are SparseTensors over those rows)."""
@@ -82,7 +61,7 @@ def _caller_coords(names):
 def largest_by_value_then_key(w, n, C):
     """The n largest entries of w, ties broken by the packed coordinate key of the row (NOT by the row index: row order
     is implementation-defined, and large regions of a generated scene carry bit-identical features)."""
-    order = torch.argsort(keys_of(C.cpu()), stable=True)
+    order = torch.argsort(parity.keys(C), stable=True)
     rank = torch.sort(w.detach().cpu()[order], descending=True, stable=True)[1][:n]
     return order[rank].to(w.device)
 
@@ -95,19 +74,6 @@ def det_multinomial(w, n, replacement=False, **_):
 def det_topk(x, k, dim=0, **_):
     i = largest_by_value_then_key(x, k, _caller_coords(("x", "sem_logit")))
     return x[i], i
-
-
-def collect(out, n_infers, step, arrays):
-    for m in range(n_infers):
-        sfx = "" if n_infers == 1 else f"_m{m}"
-        for s, lg in out["sem_logits_at_scales"].items():
-            summarise(arrays, f"sem{s}{sfx}", lg[m].C, lg[m].F, step)
-        if "panop_predictions" in out:
-            p = out["panop_predictions"][m]
-            arrays[f"query_logits{sfx}"] = p["query_logits"][0].detach().numpy()
-            summarise(arrays, f"vox{sfx}", p["voxel_logits"].C, p["voxel_logits"].F, step)
-            for i, aux in enumerate(p["aux_outputs"]):
-                arrays[f"aux{i}_query_logits{sfx}"] = aux["query_logits"][0].detach().numpy()
 
 
 def run_case(tag, grid, occ, n_infers=1, test=False, det=False, heavy=False, n_classes=20, in_ch=283, step=8,
@@ -129,7 +95,7 @@ def run_case(tag, grid, occ, n_infers=1, test=False, det=False, heavy=False, n_c
     finally:
         torch.multinomial, torch.topk = saved
     arrays = {}
-    collect(out, n_infers, step, arrays)
+    parity.collect(out, n_infers, step, arrays, parity.summary)
     meta = {"grid": list(grid), "occ": occ, "seed": seed, "row_step": step, "n_infers": n_infers, "test": test,
             "deterministic_sampling": det, "heavy_decoder": heavy, "n_classes": n_classes, "in_channels": in_ch,
             "thresholds": thresholds}

@@ -18,19 +18,14 @@ import numpy as np
 import torch
 
 import make_golden as G  # noqa: F401  (sets sys.path to the reference, the oracle and the shims)
-from make_golden import GRID, OCC, SEED, canon
+from make_golden import GRID, OCC, SEED
+import parity
 from recipe import fill_state_dict
 from run_reference_on_oracle import build_net, forward
 from pasco_b200.synthetic import make_scene
 
 WIDTHS = (32, 96)
 STEP = 32                  # row subsample of the feature arrays
-
-
-def _rows(arrays, name, st):
-    c, f = canon(st)
-    arrays[f"{name}_C"], arrays[f"{name}_F"] = c, f[::STEP]
-    arrays[f"{name}_sum"] = np.array([f.sum(dtype=np.float64), np.abs(f).sum(dtype=np.float64)])
 
 
 def main():
@@ -46,13 +41,7 @@ def main():
         with torch.no_grad():
             _, out = forward(net, batch)
         arrays = {}
-        for s, lg in out["sem_logits_at_scales"].items():
-            _rows(arrays, f"sem{s}", lg[0])
-        p = out["panop_predictions"][0]
-        arrays["query_logits"] = p["query_logits"][0].numpy()
-        _rows(arrays, "vox", p["voxel_logits"])
-        for i, aux in enumerate(p["aux_outputs"]):
-            arrays[f"aux{i}_query_logits"] = aux["query_logits"][0].numpy()
+        parity.collect(out, 1, STEP, arrays, parity.rows)
         np.savez_compressed(os.path.join(here, f"net_cfg1_f{f}.npz"), **arrays)
         manifests[str(f)] = {k: list(v.shape) for k, v in sd.items()
                              if not k.startswith(("unet3d.transformer_predictor.",

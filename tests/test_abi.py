@@ -35,6 +35,32 @@ def test_header_symbols_are_exported_and_typed(lib):
     assert sorted(_lib.PROTOTYPES) == names, "ctypes prototypes and header disagree"
 
 
+def test_header_declarations_match_ctypes_prototypes():
+    """Every pasco_* declaration's return and argument kinds equal _lib.PROTOTYPES: pointers, arrays and the stream →
+    c_void_p, `const char*` → c_char_p, the scalar types → their ctypes types."""
+    from pasco_b200 import _lib
+    C = _lib.C
+    scalar = {"int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64, "float": C.c_float,
+              "double": C.c_double, "pasco_stream_t": C.c_void_p}
+
+    def kind(text, ret=False):
+        """ctypes type of a return type, or of one parameter (type and name)."""
+        t = text.replace("const", " ")
+        if not ret:                                  # drop the name; an array parameter is a pointer
+            t = re.sub(r"\w+\s*(\[\d*\])?\s*$", lambda m: "" if m.group(1) is None else "*", t)
+        words = t.replace("*", " * ").split()
+        if "*" in words:
+            return C.c_char_p if ret and words[0] == "char" else C.c_void_p
+        return scalar[words[0]]
+
+    src = re.sub(r"/\*.*?\*/|//[^\n]*", "", open(os.path.join(ROOT, "include", "pasco_sm100.h")).read(), flags=re.S)
+    decls = re.findall(r"([\w\s\*]+?)\b(pasco_[a-z0-9_]+)\s*\(([^;{)]*)\)\s*;", src)
+    assert sorted(name for _, name, _ in decls) == _declared_symbols()
+    for ret, name, args in decls:
+        want = (kind(ret, ret=True), [kind(a) for a in args.split(",") if a.strip() not in ("", "void")])
+        assert want == _lib.PROTOTYPES[name], (name, want, _lib.PROTOTYPES[name])
+
+
 def test_abi_version_3_and_error_string(lib):
     assert lib.pasco_abi_version() == 3
     assert isinstance(lib.pasco_last_error(), bytes)

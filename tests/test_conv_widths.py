@@ -12,43 +12,23 @@ GPU part : forward, input gradient and weight gradient against the oracle at con
 The ring depths the planners pick for these shapes stay inside the ranges the lag replays of tests/test_pipeline_lag.py
 and tests/test_wgrad_pipeline.py cover (unit / A rings 3-8, B rings 2-3, gout rings 2-4, 1 or 2 units per row tile).
 """
-import contextlib
-import json
 import os
 import sys
 
-import numpy as np
 import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
-from recipe import fill_state_dict  # noqa: E402
-from test_golden_net import _compare  # noqa: E402
-from test_gpu_ops import ME, TOL_BF16, TOL_TIGHT, _run_conv_case, relerr  # noqa: E402,F401  (ME: module fixture)
+import parity  # noqa: E402
+from parity import TOL_BF16, TOL_TIGHT, relerr  # noqa: E402
 
-MANIFEST = json.load(open(os.path.join(HERE, "golden", "net_cfg1_widths_manifest.json")))
-
-
-def _pasconet(f):
-    from pasco_b200.net3d import PascoNet
-    torch.manual_seed(0)
-    return PascoNet(n_classes=20, n_infers=1, in_channels=283, f=f, num_queries=100, heavy_decoder=False)
+MANIFEST = parity.manifest("net_cfg1_widths_manifest.json")
 
 
-@contextlib.contextmanager
-def _launches():
-    """(kind, path, Cin, Cout) of every convolution launch inside the block."""
-    from pasco_b200 import ops
-    got = []
-    ops.PROFILE = []
-    try:
-        yield got
-    finally:
-        torch.cuda.synchronize()
-        got.extend((kind, m["path"], m["Cin"], m["Cout"]) for kind, _, _, m in ops.PROFILE)
-        ops.PROFILE = None
-        ops.PAIR_COUNTS.clear()
+@pytest.fixture(scope="module")
+def ME():
+    return parity.engine()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -96,7 +76,7 @@ def test_conv_path_follows_the_channel_contract(monkeypatch):
 
 @pytest.mark.parametrize("f", [32, 96])
 def test_width_manifest_matches_pasconet_state_dict(f):
-    mine = {k: list(v.shape) for k, v in _pasconet(f).reference_state_dict().items()}
+    mine = {k: list(v.shape) for k, v in parity.pasconet(f=f).reference_state_dict().items()}
     ref = MANIFEST["params"][str(f)]
     assert sorted(mine) == sorted(ref), (sorted(set(ref) - set(mine))[:5], sorted(set(mine) - set(ref))[:5])
     bad = [k for k in ref if mine[k] != ref[k]]
@@ -119,8 +99,8 @@ def _widths_case(ME, kind, cin, cout, prec, planes, tol):
     ops.set_precision(prec)
     ops.use_planes(planes)
     try:
-        with _launches() as launches:
-            e = _run_conv_case(ME, kind, cin, cout, tol)
+        with parity.launches() as launches:
+            e = parity.run_conv_case(ME, kind, cin, cout, tol)
     finally:
         ops.use_planes(True)
         ops.set_precision("fp32")
@@ -165,7 +145,7 @@ def test_conv_widths_split_k_match_fp64(cin, cout):
     b = torch.randn(cout, generator=g).cuda()
     G = torch.randn(N, cout, generator=g).cuda()
     koff = [K - 1 - k for k in range(K)]
-    with _launches() as launches:
+    with parity.launches() as launches:
         o_f = ops.conv_apply(F, W, nbr, N, False, None, b)
         o_g = ops.conv_apply(G, W, nbr, N, True, koff)
     assert [p for _, p, _, _ in launches] == ["splitk", "splitk"]
@@ -249,48 +229,16 @@ def test_conv_widths_plane_and_register_gather_are_bit_identical(prec, cin, cout
 # ------------------------------------------------------------------------------------------------
 # GPU: the network at other widths
 # ------------------------------------------------------------------------------------------------
-def _scene_on(dev):
-    from pasco_b200.synthetic import make_scene
-    b = make_scene(MANIFEST["grid"], MANIFEST["occ"], 1, seed=MANIFEST["seed"])
-    d = lambda t: t.to(dev)  # noqa: E731
-    return dict(b, in_feats=[d(t) for t in b["in_feats"]], in_coords=[d(t) for t in b["in_coords"]],
-                sem_labels={k: d(v) for k, v in b["sem_labels"].items()}, mask_classes=d(b["mask_classes"]))
-
-
-def _forward(net, sc):
-    return net(sc["in_feats"], sc["in_coords"], sc["global_min_Cs"], sc["global_max_Cs"], sc["min_Cs"], sc["max_Cs"])
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("f", [32, 96])
 def test_pasconet_width_matches_reference_golden(f):
     from pasco_b200 import ops
     ops.set_precision("fp32")
-    gold = np.load(os.path.join(HERE, "golden", f"net_cfg1_f{f}.npz"))
-    step = MANIFEST["row_step"]
-    net = _pasconet(f)
-    net.load_reference_state_dict(fill_state_dict(net.reference_state_dict()))
-    net.cuda().train()
-    with torch.no_grad(), _launches() as launches:
-        out = _forward(net, _scene_on(torch.device("cuda")))
+    net = parity.pasconet(f=f, recipe=True).cuda().train()
+    with torch.no_grad(), parity.launches() as launches:
+        out = parity.forward(net, parity.scene(MANIFEST))
     assert launches and not [x for x in launches if x[1] == "simt"], [x for x in launches if x[1] == "simt"][:5]
-    report = {}
-    for s in (4, 2, 1):
-        lg = out["sem_logits_at_scales"][s][0]
-        report[f"sem{s}"] = _compare(f"sem{s}", lg.C, lg.F, gold[f"sem{s}_C"], gold[f"sem{s}_F"], step)
-    p = out["panop_predictions"][0]
-    vox = p["voxel_logits"]
-    report["vox"] = _compare("voxel_logits", vox.C, vox.F, gold["vox_C"], gold["vox_F"], step)
-    if report["vox"][0] == 0:                  # same coordinates: the checksums over all rows agree too
-        v = vox.F.detach().double()
-        got = torch.stack([v.sum(), v.abs().sum()]).cpu().numpy()
-        report["vox_sum"] = float(np.abs(got - gold["vox_sum"]).max() / gold["vox_sum"][1])
-        assert report["vox_sum"] <= 1e-3, report
-    for name, q in [("query_logits", p["query_logits"])] + [(f"aux{i}_query_logits", a["query_logits"])
-                                                             for i, a in enumerate(p["aux_outputs"])]:
-        e = float((q[0].detach().cpu().double() - torch.as_tensor(gold[name]).double()).abs().max() / np.abs(gold[name]).max())
-        assert e <= 1e-3, f"{name} error {e:.3e}"
-        report[name] = e
+    report = parity.check_outputs(out, parity.fixture(f"net_cfg1_f{f}.npz"), MANIFEST, sums=True)
     print(f"PascoNet f={f} vs golden:", report)
 
 
@@ -302,11 +250,11 @@ def test_pasconet_width_training_step_runs_on_tensor_cores(f):
     from pasco_b200 import ops
     from pasco_b200.losses import total_loss
     ops.set_precision("fp32")
-    net = _pasconet(f).cuda().train()
-    sc = _scene_on(torch.device("cuda"))
+    net = parity.pasconet(f=f).cuda().train()
+    sc = parity.scene(MANIFEST)
     opt = torch.optim.AdamW(net.parameters(), lr=1e-4)
-    with _launches() as launches:
-        loss = total_loss(_forward(net, sc), sc, 20, net.class_frequencies)
+    with parity.launches() as launches:
+        loss = total_loss(parity.forward(net, sc), sc, 20, net.class_frequencies)
         loss.backward()
     assert torch.isfinite(loss), loss
     simt = [x for x in launches if x[1] == "simt"]

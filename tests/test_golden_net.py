@@ -6,7 +6,6 @@ GPU part : same recipe weights + same synthetic scene → sem logits at 3 scales
            logits agree with the golden subsample within the north_star tolerance (1e-3, max-abs
            normalised).  Coordinate sets must be identical up to argmax near-ties (≤ 0.1 % of rows).
 """
-import json
 import os
 import sys
 
@@ -16,19 +15,14 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
+import parity  # noqa: E402
 from recipe import fill_state_dict  # noqa: E402
 
-MANIFEST = json.load(open(os.path.join(HERE, "golden", "net_cfg1_manifest.json")))
-
-
-def _net():
-    from pasco_b200.net3d import PascoNet
-    torch.manual_seed(0)
-    return PascoNet(n_classes=20, n_infers=1, in_channels=283, f=64, num_queries=100, heavy_decoder=False)
+MANIFEST = parity.manifest("net_cfg1_manifest.json")
 
 
 def test_state_dict_names_and_shapes_match_the_reference():
-    sd = _net().reference_state_dict()
+    sd = parity.pasconet().reference_state_dict()
     mine = {k: list(v.shape) for k, v in sd.items()}
     ref = MANIFEST["params"]
     assert sorted(mine) == sorted(ref), (sorted(set(ref) - set(mine))[:5], sorted(set(mine) - set(ref))[:5])
@@ -41,16 +35,14 @@ def test_state_dict_names_and_shapes_match_the_reference():
 def test_state_dict_matches_reference_for_mimo_and_heavy_decoder(variant, M, heavy):
     """Checkpoint compatibility of the other shipped configurations: MIMO M=2/3 and heavy_decoder=True
     (manifests dumped from the reference's own Net.state_dict(), tests/golden/manifests_variants.json)."""
-    from pasco_b200.net3d import PascoNet
-    ref = json.load(open(os.path.join(HERE, "golden", "manifests_variants.json")))[variant]
-    net = PascoNet(n_classes=20, n_infers=M, in_channels=283, f=64, num_queries=100, heavy_decoder=heavy)
-    mine = {k: list(v.shape) for k, v in net.reference_state_dict().items()}
+    ref = parity.manifest("manifests_variants.json")[variant]
+    mine = {k: list(v.shape) for k, v in parity.pasconet(M, heavy=heavy).reference_state_dict().items()}
     assert sorted(mine) == sorted(ref), (sorted(set(ref) - set(mine))[:5], sorted(set(mine) - set(ref))[:5])
     assert all(mine[k] == ref[k] for k in ref)
 
 
 def test_reference_state_dict_round_trip():
-    net = _net()
+    net = parity.pasconet()
     sd = fill_state_dict(net.reference_state_dict())
     net.load_reference_state_dict(sd)
     back = net.reference_state_dict()
@@ -59,64 +51,14 @@ def test_reference_state_dict_round_trip():
         net.load_reference_state_dict({k: v for k, v in sd.items() if "enc_in_feats" not in k})
 
 
-def _keys(C):
-    c = torch.as_tensor(np.asarray(C, dtype=np.int64))
-    return ((c[:, 0] + 32768) << 48) | ((c[:, 1] + 32768) << 32) | ((c[:, 2] + 32768) << 16) | (c[:, 3] + 32768)
-
-
-def _compare(name, got_C, got_F, gold_C, gold_F_sub, step, tol=1e-3, check=True):
-    gk, rk = _keys(got_C.cpu().numpy()), _keys(gold_C)
-    order = torch.argsort(gk)
-    gk, gF = gk[order], got_F.detach().cpu()[order]
-    common = np.intersect1d(gk.numpy(), rk.numpy())
-    sym = (len(gk) - len(common)) + (len(rk) - len(common))
-    assert sym <= max(2, 0.001 * len(rk)), f"{name}: coordinate sets differ in {sym} of {len(rk)} rows"
-    sub_keys = rk[::step]
-    pos = torch.searchsorted(gk, sub_keys).clamp(max=len(gk) - 1)
-    hit = gk[pos] == sub_keys
-    ref = torch.as_tensor(gold_F_sub)[hit]
-    got = gF[pos[hit]]
-    rowerr = (got.double() - ref.double()).abs().max(1)[0] / ref.double().abs().max()
-    if sym == 0:
-        err = float(rowerr.max())
-    else:
-        # an argmax near-tie kept/dropped `sym` voxels differently from the CPU run: the 3x3x3 convs behind the output
-        # make their spatial neighbours differ too, everything else must still agree → judge the 99th percentile
-        err = float(torch.quantile(rowerr, 0.99))
-    assert (not check) or err <= tol, f"{name}: feature error {err:.3e} > {tol} (sym={sym})"
-    return sym, err
-
-
 @pytest.mark.gpu
 def test_full_forward_matches_reference_golden():
     from pasco_b200 import ops
-    from pasco_b200.synthetic import make_scene
     ops.set_precision("fp32")
-    gold = np.load(os.path.join(HERE, "golden", "net_cfg1.npz"))
-    net = _net()
-    net.load_reference_state_dict(fill_state_dict(net.reference_state_dict()))
-    net.cuda().train()
-    b = make_scene(MANIFEST["grid"], MANIFEST["occ"], 1, seed=MANIFEST["seed"])
-    dev = torch.device("cuda")
+    net = parity.pasconet(recipe=True).cuda().train()
     with torch.no_grad():
-        out = net([f.to(dev) for f in b["in_feats"]], [c.to(dev) for c in b["in_coords"]],
-                  b["global_min_Cs"], b["global_max_Cs"], b["min_Cs"], b["max_Cs"])
-    step = MANIFEST["row_step"]
-    report = {}
-    for s in (4, 2, 1):
-        lg = out["sem_logits_at_scales"][s][0]
-        report[f"sem{s}"] = _compare(f"sem{s}", lg.C, lg.F, gold[f"sem{s}_C"], gold[f"sem{s}_F"], step)
-    p = out["panop_predictions"][0]
-    report["vox"] = _compare("voxel_logits", p["voxel_logits"].C, p["voxel_logits"].F, gold["vox_C"], gold["vox_F"], step)
-    q = p["query_logits"][0].cpu()
-    eq = float((q.double() - torch.as_tensor(gold["query_logits"]).double()).abs().max()
-               / np.abs(gold["query_logits"]).max())
-    assert eq <= 1e-3, f"query logits error {eq:.3e}"
-    for i, aux in enumerate(p["aux_outputs"]):
-        ea = float((aux["query_logits"][0].cpu().double() - torch.as_tensor(gold[f"aux{i}_query_logits"]).double()).abs().max()
-                   / np.abs(gold[f"aux{i}_query_logits"]).max())
-        assert ea <= 1e-3, f"aux {i} query logits error {ea:.3e}"
-    print("golden parity:", report, "query", eq)
+        out = parity.forward(net, parity.scene(MANIFEST))
+    print("golden parity:", parity.check_outputs(out, parity.fixture("net_cfg1.npz"), MANIFEST))
 
 
 @pytest.mark.gpu
@@ -124,35 +66,9 @@ def test_mimo_m2_forward_matches_reference_golden():
     """MIMO wrapper, M=2 (two scenes channel-concatenated through one trunk, per-subnet heads and transformer
     passes incl. the reference's zero-padding of the shorter subnet): golden from the unmodified reference."""
     from pasco_b200 import ops
-    from pasco_b200.net3d import PascoNet
-    from pasco_b200.synthetic import make_scene
     ops.set_precision("fp32")
-    man = json.load(open(os.path.join(HERE, "golden", "net_cfg1_m2_manifest.json")))
-    gold = np.load(os.path.join(HERE, "golden", "net_cfg1_m2.npz"))
-    torch.manual_seed(0)
-    net = PascoNet(n_classes=20, n_infers=2, in_channels=283, f=64, num_queries=100)
-    net.load_reference_state_dict(fill_state_dict(net.reference_state_dict()))
-    net.cuda().train()
-    b = make_scene(man["grid"], man["occ"], 2, seed=man["seed"])
-    dev = torch.device("cuda")
+    man = parity.manifest("net_cfg1_m2_manifest.json")
+    net = parity.pasconet(2, recipe=True).cuda().train()
     with torch.no_grad():
-        out = net([f.to(dev) for f in b["in_feats"]], [c.to(dev) for c in b["in_coords"]],
-                  b["global_min_Cs"], b["global_max_Cs"], b["min_Cs"], b["max_Cs"])
-    step, report = man["row_step"], {}
-    for m in range(2):
-        for s in (4, 2, 1):
-            lg = out["sem_logits_at_scales"][s][m]
-            report[f"sem{s}_m{m}"] = _compare(f"sem{s}_m{m}", lg.C, lg.F, gold[f"sem{s}_m{m}_C"], gold[f"sem{s}_m{m}_F"], step, check=False)
-        p = out["panop_predictions"][m]
-        report[f"vox_m{m}"] = _compare(f"vox_m{m}", p["voxel_logits"].C, p["voxel_logits"].F, gold[f"vox_m{m}_C"],
-                                       gold[f"vox_m{m}_F"], step, check=False)
-        q = p["query_logits"][0].cpu()
-        eq = float((q.double() - torch.as_tensor(gold[f"query_logits_m{m}"]).double()).abs().max()
-                   / np.abs(gold[f"query_logits_m{m}"]).max())
-        report[f"query_m{m}"] = eq
-        for i, aux in enumerate(p["aux_outputs"]):
-            report[f"aux{i}_m{m}"] = float((aux["query_logits"][0].cpu().double() - torch.as_tensor(gold[f"aux{i}_query_logits_m{m}"]).double()).abs().max()
-                                           / np.abs(gold[f"aux{i}_query_logits_m{m}"]).max())
-    print("MIMO M=2 golden parity:", report)
-    worst = max(v[1] if isinstance(v, tuple) else v for v in report.values())
-    assert worst <= 1e-3, report
+        out = parity.forward(net, parity.scene(man, 2))
+    print("MIMO M=2 golden parity:", parity.check_outputs(out, parity.fixture("net_cfg1_m2.npz"), man, worst=True))

@@ -13,33 +13,23 @@ import json
 import os
 import sys
 
-import numpy as np
 import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-GOLD = os.path.join(HERE, "golden")
-sys.path.insert(0, GOLD)
-from recipe import fill_state_dict  # noqa: E402
+sys.path.insert(0, os.path.join(HERE, "golden"))
+import parity  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
 
-def _keys(C):
-    c = torch.as_tensor(C).long().cpu()
-    return ((c[:, 0] + 32768) << 48) | ((c[:, 1] + 32768) << 32) | ((c[:, 2] + 32768) << 16) | (c[:, 3] + 32768)
-
-
 def _load(tag):
-    return json.load(open(os.path.join(GOLD, f"r2_{tag}.json"))), np.load(os.path.join(GOLD, f"r2_{tag}.npz"))
+    return parity.manifest(f"r2_{tag}.json"), parity.fixture(f"r2_{tag}.npz")
 
 
 def _net(meta):
-    from pasco_b200.net3d import PascoNet
-    torch.manual_seed(0)
-    net = PascoNet(n_classes=meta["n_classes"], n_infers=meta["n_infers"], in_channels=meta["in_channels"], f=64,
-                   num_queries=100, heavy_decoder=meta["heavy_decoder"])
-    net.load_reference_state_dict(fill_state_dict(net.reference_state_dict()))
+    net = parity.pasconet(meta["n_infers"], heavy=meta["heavy_decoder"], n_classes=meta["n_classes"],
+                          in_channels=meta["in_channels"], recipe=True)
     if meta.get("thresholds"):
         dec = net.unet3d.decoder_generative
         dec.occ_thres = {int(k): v for k, v in meta["thresholds"]["occ"].items()}
@@ -49,66 +39,13 @@ def _net(meta):
 
 def _forward(net, meta, grad=False):
     from pasco_b200 import net3d
-    from pasco_b200.synthetic import make_scene
-    b = make_scene(meta["grid"], meta["occ"], meta["n_infers"], in_ch=meta["in_channels"], n_classes=meta["n_classes"],
-                   seed=meta["seed"])
-    dev = torch.device("cuda")
+    sc = parity.scene(meta, meta["n_infers"])
     net3d.set_deterministic_sampling(bool(meta["deterministic_sampling"]))
     try:
         with torch.set_grad_enabled(grad):
-            return net([f.to(dev) for f in b["in_feats"]], [c.to(dev) for c in b["in_coords"]], b["global_min_Cs"],
-                       b["global_max_Cs"], b["min_Cs"], b["max_Cs"], test=meta["test"])
+            return parity.forward(net, sc, test=meta["test"])
     finally:
         net3d.set_deterministic_sampling(False)
-
-
-def _check_sparse(name, C, F, gold, tol=1e-3, sym_frac=1e-3, q=0.99):
-    """→ (exact_set, err).  exact_set: count, key sum and key xor all equal (bit-exact coordinate parity)."""
-    k = _keys(C)
-    order = torch.argsort(k)
-    k, F = k[order], F.detach().float().cpu()[order]
-    kn = k.numpy().astype(np.uint64)
-    n_gold = int(gold[f"{name}_n"][0])
-    exact = (len(kn) == n_gold and np.add.reduce(kn) == gold[f"{name}_ksum"][0]
-             and np.bitwise_xor.reduce(kn) == gold[f"{name}_ksum"][1])
-    assert abs(len(kn) - n_gold) <= max(2, sym_frac * n_gold), f"{name}: {len(kn)} rows, reference {n_gold}"
-    sub_k = torch.as_tensor(gold[f"{name}_subK"].astype(np.int64))
-    pos = torch.searchsorted(k, sub_k).clamp(max=len(k) - 1)
-    hit = k[pos] == sub_k
-    assert float(hit.float().mean()) >= 1.0 - 2 * sym_frac - 2.0 / max(len(sub_k), 1), f"{name}: {int((~hit).sum())} subsample rows missing"
-    ref = torch.as_tensor(gold[f"{name}_subF"])[hit].double()
-    amax = float(gold[f"{name}_Fsum"][2])
-    rowerr = (F[pos[hit]].double() - ref).abs().max(1)[0] / amax
-    if exact:
-        err = float(rowerr.max())
-        s_err = abs(float(F.double().sum()) - float(gold[f"{name}_Fsum"][0])) / float(gold[f"{name}_Fsum"][1])
-        assert s_err <= tol, f"{name}: checksum Σ differs by {s_err:.2e} of Σ|.|"
-    else:       # an argmax / rank near-tie kept a few other voxels than the CPU run: neighbours differ, the rest must agree
-        err = float(torch.quantile(rowerr, q))
-        med = float(rowerr.median())
-        assert med <= tol / 2, f"{name}: median feature error {med:.3e} > {tol / 2} (exact_set={exact})"
-    assert err <= tol, f"{name}: feature error {err:.3e} > {tol} (exact_set={exact})"
-    return exact, err
-
-
-def _check_all(out, meta, gold, tol=1e-3, sym_frac=1e-3, need_exact=(), q=0.99, head_tol=None):
-    """head_tol: tolerance of the transformer outputs (mask / query logits); default = tol, and 5x tol for the query logits
-    when the voxel set they attend over is not bit-identical to the reference's (a flipped voxel changes every query)."""
-    rep = {}
-    for m in range(meta["n_infers"]):
-        sfx = "" if meta["n_infers"] == 1 else f"_m{m}"
-        for s in (4, 2, 1):
-            lg = out["sem_logits_at_scales"][s][m]
-            rep[f"sem{s}{sfx}"] = _check_sparse(f"sem{s}{sfx}", lg.C, lg.F, gold, tol, sym_frac, q)
-        p = out["panop_predictions"][m]
-        rep[f"vox{sfx}"] = _check_sparse(f"vox{sfx}", p["voxel_logits"].C, p["voxel_logits"].F, gold, head_tol or tol, sym_frac, q)
-        ql, gl = p["query_logits"][0].detach().double().cpu(), torch.as_tensor(gold[f"query_logits{sfx}"]).double()
-        rep[f"query{sfx}"] = float((ql - gl).abs().max() / gl.abs().max())
-        qtol = head_tol or (tol if rep[f"vox{sfx}"][0] else 5 * tol)
-        assert rep[f"query{sfx}"] <= qtol, rep
-    for n in need_exact:
-        assert rep[n][0], f"{n}: coordinate set is not bit-identical to the reference's ({rep})"
-    return rep
 
 
 def test_benchmark_scale_forward_no_caps_matches_reference():
@@ -118,7 +55,7 @@ def test_benchmark_scale_forward_no_caps_matches_reference():
     meta, gold = _load("big_eval")
     # 1.7 M decoder voxels: a handful of argmax near-ties (class 0 vs not) may fall the other way than in the CPU run, so
     # the coordinate sets are compared by count (0.1 %) and subsample hits, the features by the 99th percentile
-    rep = _check_all(_forward(_net(meta), meta), meta, gold)
+    rep = parity.check_outputs(_forward(_net(meta), meta), gold, meta, aux=False)
     print("big_eval:", rep)
 
 
@@ -130,7 +67,7 @@ def test_benchmark_scale_cap_branch_matches_reference():
     # rank near-ties at the caps (25 000th of 28 244 candidates at scale 4, fp noise 3e-5 vs value spacing 3e-5) move one or
     # two voxels in or out; each scale-4 voxel owns a (8 + halo)^3 region of the scale-1 output, ~1 % of its rows per flip:
     # the bound is on the 90th percentile (and on the median, 2x tighter), row counts must still equal the caps
-    rep = _check_all(_forward(_net(meta), meta), meta, gold, q=0.90)
+    rep = parity.check_outputs(_forward(_net(meta), meta), gold, meta, aux=False, q=0.90)
     for s, cap in ((4, 25000), (2, 120000), (1, 400000)):
         assert int(gold[f"sem{s}_n"][0]) == cap
     print("big_capped:", rep)
@@ -143,7 +80,7 @@ def test_variant_forward_matches_reference(tag):
     meta, gold = _load(tag)
     # M = 3: the query logits sit behind three attention layers over ~30 k voxels whose masks threshold at logit 0; measured
     # 9.1e-4 for one subnet of the KITTI-360 case — the sparse outputs keep the 1e-3 bound, the transformer heads get 2e-3
-    rep = _check_all(_forward(_net(meta), meta), meta, gold, head_tol=2e-3 if meta["n_infers"] >= 3 else None)
+    rep = parity.check_outputs(_forward(_net(meta), meta), gold, meta, aux=False, head_tol=2e-3 if meta["n_infers"] >= 3 else None)
     print(tag, rep)
 
 
@@ -154,7 +91,7 @@ def test_full_network_gradients_match_reference():
     meta, gold = _load("grads")
     net = _net(meta)
     out = _forward(net, meta, grad=True)
-    _check_all(out, meta, gold)
+    parity.check_outputs(out, gold, meta, aux=False)
     loss = 0.0
     for s in (4, 2, 1):
         loss = loss + out["sem_logits_at_scales"][s][0].F.square().mean()
@@ -199,7 +136,7 @@ def test_network_level_bf16_mode_within_2e2():
         # flipped voxel changes its 3x3x3 neighbourhood: for the semantic logits 4e-2 on the 90th percentile and 2e-2
         # on the median of the per-row error (SURVEY.md §8c item 4: 2e-2 per op — measured 2e-3 per convolution); the mask
         # and query logits sit behind three more attention layers: 1e-1 / 5e-2 (measured 5.9e-2 at the 90th percentile)
-        rep = _check_all(_forward(_net(meta), meta), meta, gold, tol=4e-2, sym_frac=2e-2, q=0.90, head_tol=1e-1)   # median <= tol/2
+        rep = parity.check_outputs(_forward(_net(meta), meta), gold, meta, aux=False, tol=4e-2, sym_frac=2e-2, q=0.90, head_tol=1e-1)   # median <= tol/2
     finally:
         ops.set_precision("fp32")
     print("bf16 network parity:", rep)

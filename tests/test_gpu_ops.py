@@ -5,58 +5,25 @@ Integer work (coordinate maps, kernel maps) must match bit-exactly after canonic
 SURVEY.md §8c item 3).  fp32 features: max-abs-normalised error ≤ 1e-3 (north_star), in practice
 ~1e-5 for the bf16x3 path and exactly-rounded fp32 for the CUDA-core path.
 """
+import os
+import sys
+
 import pytest
 import torch
 
 import me_oracle as OR
 
-pytestmark = pytest.mark.gpu
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+import parity  # noqa: E402
+from parity import (TOL_BF16, TOL_FP32, TOL_TIGHT, assert_same_sparse, canon, conv_pair, relerr,  # noqa: E402
+                    run_conv_case, sparse_scene)
 
-TOL_FP32 = 1e-3      # north_star tolerance for fp32 features
-TOL_TIGHT = 2e-5     # what bf16x3 / fp32 SIMT actually deliver
-TOL_BF16 = 2e-2      # bf16 operands (SURVEY.md §8c item 4)
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
 def ME():
-    from pasco_b200 import build
-    build.build()
-    from pasco_b200 import me
-    return me
-
-
-def scene(shape=(24, 20, 12), p=0.3, C=64, batch=1, lo=(0, 0, 0), seed=0, stride=1):
-    g = torch.Generator().manual_seed(seed)
-    cs = []
-    for b in range(batch):
-        occ = torch.rand(*shape, generator=g) < p
-        c = torch.nonzero(occ).int() * stride + torch.tensor(lo, dtype=torch.int32)
-        cs.append(c)
-    bc = OR.utils.batched_coordinates(cs)
-    f = torch.randn(bc.shape[0], C, generator=g)
-    return bc, f
-
-
-def relerr(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).abs().max() / b.abs().max().clamp(min=1e-30))
-
-
-def canon(C, F=None):
-    """Sort rows by packed coordinate key."""
-    C = C.detach().cpu()
-    order = torch.argsort(OR.pack_keys(C))
-    return (C[order], None if F is None else F.detach().cpu()[order])
-
-
-def assert_same_sparse(got, ref, tol):
-    gc, gf = canon(got.C, got.F)
-    rc, rf = canon(ref.C, ref.F)
-    assert gc.shape == rc.shape and torch.equal(gc, rc), "coordinate sets differ"
-    assert got.tensor_stride == ref.tensor_stride
-    e = relerr(gf, rf)
-    assert e <= tol, f"feature error {e:.3e} > {tol}"
-    return e
+    return parity.engine()
 
 
 def triples(nbr, in_c, out_c):
@@ -72,7 +39,7 @@ def triples(nbr, in_c, out_c):
 # integer parity
 # ------------------------------------------------------------------------------------------------
 def test_insert_dedups_first_wins_and_keeps_order(ME):
-    C, F = scene(p=0.2, C=8, lo=(-8, 4, -2))
+    C, F = sparse_scene(p=0.2, C=8, lo=(-8, 4, -2))
     C2 = torch.cat([C, C[:50]], 0)
     F2 = torch.cat([F, F[:50] + 100.0], 0)
     ref = OR.SparseTensor(F2, C2)
@@ -82,7 +49,7 @@ def test_insert_dedups_first_wins_and_keeps_order(ME):
 
 @pytest.mark.parametrize("lo", [(0, 0, 0), (-16, -8, -4)])
 def test_kernel_map_k3_bit_exact(ME, lo):
-    C, F = scene(C=8, batch=2, lo=lo)
+    C, F = sparse_scene(C=8, batch=2, lo=lo)
     ref = OR.SparseTensor(F, C)
     got = ME.SparseTensor(F.cuda(), C.cuda())
     rk = ref.coordinate_manager.kernel_map(ref.coordinate_map_key, ref.coordinate_map_key, 3)
@@ -95,7 +62,7 @@ def test_kernel_map_k3_bit_exact(ME, lo):
 
 @pytest.mark.parametrize("lo", [(0, 0, 0), (-16, -8, -4)])
 def test_stride_map_and_down_kernel_map_bit_exact(ME, lo):
-    C, F = scene(C=8, batch=2, lo=lo)
+    C, F = sparse_scene(C=8, batch=2, lo=lo)
     ref = OR.SparseTensor(F, C)
     got = ME.SparseTensor(F.cuda(), C.cuda())
     rcm, gcm = ref.coordinate_manager, got.coordinate_manager
@@ -109,7 +76,7 @@ def test_stride_map_and_down_kernel_map_bit_exact(ME, lo):
 
 
 def test_generative_map_union_and_prune_bit_exact(ME):
-    C, F = scene(shape=(6, 5, 4), p=0.5, C=8, stride=2, lo=(-4, 0, 2))
+    C, F = sparse_scene(shape=(6, 5, 4), p=0.5, C=8, stride=2, lo=(-4, 0, 2))
     ref = OR.SparseTensor(F, C, tensor_stride=2)
     got = ME.SparseTensor(F.cuda(), C.cuda(), tensor_stride=2)
     rkey = ref.coordinate_manager.generate(ref.coordinate_map_key, 2, 2)
@@ -117,7 +84,7 @@ def test_generative_map_union_and_prune_bit_exact(ME):
     rc, gc = ref.coordinate_manager.get_coordinates(rkey), got.coordinate_manager.get_coordinates(gkey)
     assert torch.equal(canon(gc)[0], canon(rc)[0]) and gkey.tensor_stride == (1, 1, 1)
     # union of two partially overlapping sets inside one manager
-    C2, F2 = scene(shape=(12, 10, 8), p=0.3, C=8, seed=5, lo=(-4, 0, 2))
+    C2, F2 = sparse_scene(shape=(12, 10, 8), p=0.3, C=8, seed=5, lo=(-4, 0, 2))
     ra = OR.SparseTensor(torch.ones(rc.shape[0], 8), coordinate_map_key=rkey, coordinate_manager=ref.coordinate_manager)
     rb = OR.SparseTensor(F2, C2, coordinate_manager=ref.coordinate_manager)
     ga = ME.SparseTensor(torch.ones(gc.shape[0], 8).cuda(), coordinate_map_key=gkey,
@@ -134,7 +101,7 @@ def test_generative_map_union_and_prune_bit_exact(ME):
 
 
 def test_dense_and_to_sparse_match(ME):
-    C, F = scene(shape=(9, 7, 5), p=0.4, C=6, batch=2, lo=(-4, 0, 2))
+    C, F = sparse_scene(shape=(9, 7, 5), p=0.4, C=6, batch=2, lo=(-4, 0, 2))
     F[5] = 0
     ref, got = OR.SparseTensor(F, C), ME.SparseTensor(F.cuda(), C.cuda())
     mn = torch.IntTensor([-4, 0, 2])
@@ -151,56 +118,13 @@ def test_dense_and_to_sparse_match(ME):
 # ------------------------------------------------------------------------------------------------
 # convolution parity (forward + both gradients), tensor-core and CUDA-core paths
 # ------------------------------------------------------------------------------------------------
-def _conv_pair(ME, kind, cin, cout, seed=0, bias=False):
-    torch.manual_seed(seed)
-    if kind == "k3":
-        r = OR.MinkowskiConvolution(cin, cout, kernel_size=3, bias=bias, dimension=3)
-        g = ME.MinkowskiConvolution(cin, cout, kernel_size=3, bias=bias, dimension=3)
-    elif kind == "down":
-        r = OR.MinkowskiConvolution(cin, cout, kernel_size=2, stride=2, dimension=3)
-        g = ME.MinkowskiConvolution(cin, cout, kernel_size=2, stride=2, dimension=3)
-    else:
-        r = OR.MinkowskiConvolutionTranspose(cin, cout, kernel_size=2, stride=2, dimension=3, expand_coordinates=True)
-        g = ME.MinkowskiConvolutionTranspose(cin, cout, kernel_size=2, stride=2, dimension=3, expand_coordinates=True)
-    g.load_state_dict(r.state_dict())
-    return r, g.cuda()
-
-
-def _run_conv_case(ME, kind, cin, cout, tol, shape=(20, 18, 10), p=0.3, bias=False):
-    ts = 2 if kind == "up" else 1
-    C, F = scene(shape=shape, p=p, C=cin, batch=2, lo=(-8, 0, 4), stride=ts)
-    rconv, gconv = _conv_pair(ME, kind, cin, cout, bias=bias)
-    Fr = F.clone().requires_grad_(True)
-    Fg = F.clone().cuda().requires_grad_(True)
-    ref = rconv(OR.SparseTensor(Fr, C, tensor_stride=ts))
-    got = gconv(ME.SparseTensor(Fg, C.cuda(), tensor_stride=ts))
-    e_f = assert_same_sparse(got, ref, tol)
-    # same upstream gradient on matching rows
-    order_r = torch.argsort(OR.pack_keys(ref.C))
-    order_g = torch.argsort(OR.pack_keys(got.C.cpu()))
-    gup = torch.randn(ref.F.shape, generator=torch.Generator().manual_seed(7))
-    gr = torch.empty_like(gup)
-    gr[order_r] = gup
-    gg = torch.empty_like(gup)
-    gg[order_g] = gup
-    ref.F.backward(gr)
-    got.F.backward(gg.cuda())
-    e_i = relerr(Fg.grad, Fr.grad)
-    e_w = relerr(gconv.kernel.grad, rconv.kernel.grad)
-    assert e_i <= tol, f"dgrad error {e_i:.3e}"
-    assert e_w <= tol, f"wgrad error {e_w:.3e}"
-    if bias:
-        assert relerr(gconv.bias.grad, rconv.bias.grad) <= tol
-    return e_f, e_i, e_w
-
-
 @pytest.mark.parametrize("kind,cin,cout", [("k3", 64, 64), ("k3", 128, 128), ("k3", 256, 256), ("down", 64, 128),
                                            ("down", 128, 256), ("up", 256, 128), ("up", 128, 64), ("k3", 64, 128)])
 def test_conv_tensor_core_fp32_mode(ME, kind, cin, cout):
     from pasco_b200 import ops
     ops.set_precision("fp32")
     ops.force_simt(False)
-    e = _run_conv_case(ME, kind, cin, cout, TOL_TIGHT, bias=(kind == "k3" and cin == 64 and cout == 64))
+    e = run_conv_case(ME, kind, cin, cout, TOL_TIGHT, bias=(kind == "k3" and cin == 64 and cout == 64))
     print(f"bf16x3 {kind} {cin}->{cout}: fwd {e[0]:.2e} dgrad {e[1]:.2e} wgrad {e[2]:.2e}")
 
 
@@ -209,7 +133,7 @@ def test_conv_tensor_core_bf16_mode(ME, kind, cin, cout):
     from pasco_b200 import ops
     ops.set_precision("bf16")
     try:
-        e = _run_conv_case(ME, kind, cin, cout, TOL_BF16)
+        e = run_conv_case(ME, kind, cin, cout, TOL_BF16)
         print(f"bf16 {kind} {cin}->{cout}: fwd {e[0]:.2e} dgrad {e[1]:.2e} wgrad {e[2]:.2e}")
     finally:
         ops.set_precision("fp32")
@@ -220,7 +144,7 @@ def test_conv_cuda_core_path(ME, kind, cin, cout):
     from pasco_b200 import ops
     ops.force_simt(True)
     try:
-        e = _run_conv_case(ME, kind, cin, cout, TOL_TIGHT, shape=(12, 10, 8))
+        e = run_conv_case(ME, kind, cin, cout, TOL_TIGHT, shape=(12, 10, 8))
     finally:
         ops.force_simt(False)
 
@@ -234,7 +158,7 @@ def test_conv_register_gather_path(ME, kind, cin, cout):
     ops.set_precision("fp32")
     ops.use_planes(False)
     try:
-        _run_conv_case(ME, kind, cin, cout, TOL_TIGHT, bias=(cin == 64 and cout == 64))
+        run_conv_case(ME, kind, cin, cout, TOL_TIGHT, bias=(cin == 64 and cout == 64))
     finally:
         ops.use_planes(True)
 
@@ -362,7 +286,7 @@ def test_conv_many_tiles_per_cta(ME):
     accumulating in registers), unlike the small cases above."""
     from pasco_b200 import ops
     ops.set_precision("fp32")
-    e = _run_conv_case(ME, "k3", 64, 64, TOL_TIGHT, shape=(64, 64, 32), p=0.225)
+    e = run_conv_case(ME, "k3", 64, 64, TOL_TIGHT, shape=(64, 64, 32), p=0.225)
     print(f"bf16x3 k3 64->64 @59k rows: fwd {e[0]:.2e} dgrad {e[1]:.2e} wgrad {e[2]:.2e}")
 
 
@@ -409,8 +333,8 @@ def test_conv_tile_tail_and_single_voxel(ME):
     from pasco_b200 import ops
     ops.set_precision("fp32")
     for shape, p in (((7, 6, 5), 0.63), ((1, 1, 1), 1.1)):
-        C, F = scene(shape=shape, p=p, C=64)
-        rconv, gconv = _conv_pair(ME, "k3", 64, 64)
+        C, F = sparse_scene(shape=shape, p=p, C=64)
+        rconv, gconv = conv_pair(ME, "k3", 64, 64)
         assert_same_sparse(gconv(ME.SparseTensor(F.cuda(), C.cuda())), rconv(OR.SparseTensor(F, C)), TOL_TIGHT)
 
 
@@ -436,7 +360,7 @@ def test_conv_full_grid_matches_dense_conv3d(ME):
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("s", [2, 4])
 def test_maxpool_matches(ME, s):
-    C, F = scene(shape=(16, 12, 8), p=0.4, C=10, batch=2, lo=(-8, 0, 4))
+    C, F = sparse_scene(shape=(16, 12, 8), p=0.4, C=10, batch=2, lo=(-8, 0, 4))
     ref = OR.MinkowskiMaxPooling(kernel_size=s, stride=s, dimension=3)(OR.SparseTensor(F, C))
     got = ME.MinkowskiMaxPooling(kernel_size=s, stride=s, dimension=3)(ME.SparseTensor(F.cuda(), C.cuda()))
     assert_same_sparse(got, ref, 0.0)
@@ -601,7 +525,7 @@ def test_unet_slice_forward_backward_matches_oracle(ME, simt):
     gnet = _mini_net(ME)
     gnet.load_state_dict(rnet.state_dict())
     gnet.cuda()
-    C, F = scene(shape=(20, 16, 8), p=0.25, C=16, batch=1)
+    C, F = sparse_scene(shape=(20, 16, 8), p=0.25, C=16, batch=1)
     ry = rnet(OR.SparseTensor(F, C))
     gy = gnet(ME.SparseTensor(F.cuda(), C.cuda()))
     e = assert_same_sparse(gy, ry, TOL_FP32)

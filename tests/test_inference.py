@@ -7,11 +7,9 @@ its running statistics, and the engine folds them into the convolutions —
     in eval mode on the CPU oracle (tests/golden/make_golden_infer.py, running statistics calibrated there and stored);
   * PascoNet's fused eval forward bit for bit against the same forward with the fusions off (ops.inference_fusion);
   * the unmodified Net.step_inference (eval.py's path: ensembling + panoptic post-processing) on the drop-in;
-  * CPU: which calls take the fused forms, the fixture manifest, the new entry point's header and ctypes signature.
+  * CPU: which calls take the fused forms, the fixture manifest.
 """
-import json
 import os
-import re
 import sys
 import types
 
@@ -20,19 +18,9 @@ import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-GOLD = os.path.join(HERE, "golden")
-sys.path.insert(0, GOLD)
-from recipe import fill_state_dict  # noqa: E402
-
-MANIFEST = json.load(open(os.path.join(GOLD, "net_cfg1_infer_manifest.json")))
-STAT_SUFFIXES = (".running_mean", ".running_var")
-
-
-def _pasconet(M=1):
-    from pasco_b200.net3d import PascoNet
-    torch.manual_seed(0)
-    return PascoNet(n_classes=20, n_infers=M, in_channels=283, f=64, num_queries=100, heavy_decoder=False)
+sys.path.insert(0, os.path.join(HERE, "golden"))
+import parity  # noqa: E402
+from parity import STAT_SUFFIXES, INFER_MANIFEST as MANIFEST  # noqa: E402
 
 
 # ------------------------------------------------------------------------------------------------
@@ -53,7 +41,7 @@ def test_routing_predicates(monkeypatch):
     x = types.SimpleNamespace(is_cuda=True)
     w = torch.empty(27, 64, 64)
     kmap = types.SimpleNamespace(K=27, nbr=object(), n_out=100_000, n_in=100_000)
-    net = _pasconet()
+    net = parity.pasconet()
 
     def route():
         return ops.bn_act_conv_route(bn, x, w, kmap)
@@ -105,8 +93,8 @@ def test_infer_fixture_manifest_matches_pasconet():
     case holds the summaries of every output."""
     for tag, case in MANIFEST["cases"].items():
         M = case["n_infers"]
-        z = np.load(os.path.join(GOLD, f"net_cfg1_infer_{tag}.npz"))
-        mine = {k: list(v.shape) for k, v in _pasconet(M).reference_state_dict().items() if k.endswith(STAT_SUFFIXES)}
+        z = parity.fixture(f"net_cfg1_infer_{tag}.npz")
+        mine = {k: list(v.shape) for k, v in parity.pasconet(M).reference_state_dict().items() if k.endswith(STAT_SUFFIXES)}
         ref = case["running_stats"]
         assert sorted(mine) == sorted(ref), (tag, sorted(set(ref) ^ set(mine))[:5])
         assert all(mine[k] == ref[k] for k in ref), tag
@@ -123,41 +111,12 @@ def test_infer_fixture_manifest_matches_pasconet():
             for lvl in ["query_logits"] + [f"aux{i}_query_logits" for i in range(3)]:
                 assert z[f"{lvl}{sfx}"].shape == (100, 21)
     assert sorted(MANIFEST["cases"]) == ["big", "m1", "m2"]
-    assert int(np.load(os.path.join(GOLD, "net_cfg1_infer_big.npz"))["sem1_n"][0]) > 1_000_000
-
-
-_CT = {"void*": "p", "int32_t*": "p", "float*": "p", "int64_t": "i64", "int32_t": "i32", "pasco_stream_t": "p"}
-
-
-def test_infer_entry_point_header_matches_ctypes():
-    from pasco_b200 import _lib
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "pasco_sm100.h")).read(), flags=re.S)
-    m = re.search(r"int\s+pasco_conv_forward_planes_infer\s*\(([^)]*)\)", src)
-    assert m, "pasco_conv_forward_planes_infer is not declared"
-    kinds = []
-    for arg in m.group(1).split(","):
-        t = " ".join(arg.replace("const", "").split()[:-1]).replace(" *", "*")
-        if arg.strip().split()[-1].startswith("*"):
-            t += "*"
-        kinds.append(_CT[t])
-    ctm = {_lib.C.c_void_p: "p", _lib.C.c_int64: "i64", _lib.C.c_int32: "i32"}
-    res, args = _lib.PROTOTYPES["pasco_conv_forward_planes_infer"]
-    assert res is _lib.C.c_int
-    assert [ctm[a] for a in args] == kinds
+    assert int(parity.fixture("net_cfg1_infer_big.npz")["sem1_n"][0]) > 1_000_000
 
 
 # ------------------------------------------------------------------------------------------------
 # GPU: the inference epilogue against the composition of existing ops
 # ------------------------------------------------------------------------------------------------
-def _launches():
-    from pasco_b200 import ops
-    torch.cuda.synchronize()
-    out = [(kind, m["path"]) for kind, _, _, m in ops.PROFILE]
-    ops.PROFILE = None
-    ops.PAIR_COUNTS.clear()
-    return out
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 @pytest.mark.parametrize("C", [16, 32, 64, 80, 128, 192, 256])
@@ -190,11 +149,11 @@ def test_inference_epilogue_is_the_unfused_sequence_bit_for_bit(C, precision):
                     (True, True, True, False, ops.ACT_LEAKY, ops.ACT_LEAKY, True),
                     (False, True, True, True, 0, ops.ACT_LEAKY, False)):      # planes without an affine
                 bias_t = bias if use_bias else None
-                ops.PROFILE = []
-                out, nxt = ops.conv_infer(planes, W, bias_t, kmap, packs, residual=res if use_res else None, act_out=act_out,
-                                          want_out=want_out, next_coefs=(sc1, sh1) if coefs else None, next_act=act_next,
-                                          want_next=use_next)
-                assert _launches() == [("fwd", "planes_infer")]
+                with parity.launches() as launches:
+                    out, nxt = ops.conv_infer(planes, W, bias_t, kmap, packs, residual=res if use_res else None,
+                                              act_out=act_out, want_out=want_out, next_coefs=(sc1, sh1) if coefs else None,
+                                              next_act=act_next, want_next=use_next)
+                assert [x[:2] for x in launches] == [("fwd", "planes_infer")]
                 y = ops.conv_apply(x, W, kmap.nbr, n, False, None, bias_t.view(-1) if use_bias else None, packs=packs,
                                    planes=planes)
                 if use_res:
@@ -210,64 +169,26 @@ def test_inference_epilogue_is_the_unfused_sequence_bit_for_bit(C, precision):
         with pytest.raises(RuntimeError):
             ops.conv_infer(planes, W, None, kmap, packs)             # gradients enabled: refused
     finally:
-        ops.PROFILE = None
         ops.set_precision("fp32")
 
 
 # ------------------------------------------------------------------------------------------------
 # GPU: networks in eval mode against the eval-mode golden vectors
 # ------------------------------------------------------------------------------------------------
-def _gold(tag):
-    z = np.load(os.path.join(GOLD, f"net_cfg1_infer_{tag}.npz"))
-    return {k: z[k] for k in z.files}
-
-
-def _load_eval(net, tag, ref_names=True):
-    """Recipe weights + the calibrated running statistics of fixture `tag`; eval mode."""
-    gold = _gold(tag)
-    sd = fill_state_dict(net.reference_state_dict() if ref_names else net.state_dict())
-    n = 0
-    for k in sd:
-        if k.endswith(STAT_SUFFIXES) and f"stat::{k}" in gold:
-            sd[k] = torch.from_numpy(gold[f"stat::{k}"]).to(sd[k].dtype)
-            n += 1
-    assert n == len(MANIFEST["cases"][tag]["running_stats"]), (n, tag)
-    (net.load_reference_state_dict if ref_names else net.load_state_dict)(sd)
-    return net.cuda().eval(), gold
-
-
-def _check_golden(out, meta, gold, q=0.99):
-    """test_golden_r2's checks (coordinate-set checksums, Σ, row subsample, query logits) plus the aux query logits."""
-    from test_golden_r2 import _check_all
-    rep = _check_all(out, meta, gold, q=q)
-    for m in range(meta["n_infers"]):
-        sfx = "" if meta["n_infers"] == 1 else f"_m{m}"
-        for i, aux in enumerate(out["panop_predictions"][m]["aux_outputs"]):
-            ref = torch.as_tensor(gold[f"aux{i}_query_logits{sfx}"]).double()
-            e = float((aux["query_logits"][0].detach().cpu().double() - ref).abs().max() / ref.abs().max())
-            rep[f"aux{i}{sfx}"] = e
-            assert e <= 1e-3, (i, sfx, e)
-    return rep
-
-
 def _stats(net):
     return {k: v.clone() for k, v in net.state_dict().items() if k.endswith(STAT_SUFFIXES + (".num_batches_tracked",))}
 
 
-def _run(net, b, fused=True):
+def _run(net, sc, fused=True):
     from pasco_b200 import ops
-    dev = torch.device("cuda")
     ops.inference_fusion(fused)
-    ops.PROFILE = []
     c0 = ops.CALLS
     try:
-        with torch.no_grad():
-            out = net([f.to(dev) for f in b["in_feats"]], [c.to(dev) for c in b["in_coords"]], b["global_min_Cs"],
-                      b["global_max_Cs"], b["min_Cs"], b["max_Cs"], test=True)
-        return out, ops.CALLS - c0, _launches()
+        with torch.no_grad(), parity.launches() as launches:
+            out = parity.forward(net, sc, test=True)
+        return out, ops.CALLS - c0, launches
     finally:
         ops.inference_fusion(True)
-        ops.PROFILE = None
 
 
 def _outputs(out, M):
@@ -306,63 +227,49 @@ def _check_fused_vs_unfused(net, b, M):
 @pytest.mark.parametrize("M", [1, 2])
 def test_pasconet_eval_matches_reference_eval_golden(M):
     from pasco_b200 import ops
-    from pasco_b200.synthetic import make_scene
     ops.set_precision("fp32")
     meta = MANIFEST["cases"][f"m{M}"]
-    net, gold = _load_eval(_pasconet(M), f"m{M}")
-    b = make_scene(meta["grid"], meta["occ"], M, seed=meta["seed"])
-    out, calls, calls_ref = _check_fused_vs_unfused(net, b, M)
-    rep = _check_golden(out, meta, gold)
+    net, gold = parity.load_eval(parity.pasconet(M), f"m{M}")
+    out, calls, calls_ref = _check_fused_vs_unfused(net, parity.scene(meta, M), M)
+    rep = parity.check_outputs(out, gold, meta)
     print(f"eval M={M}: C-ABI calls fused {calls} / unfused {calls_ref};", rep)
 
 
 @pytest.mark.gpu
 def test_pasconet_eval_benchmark_scale_matches_reference_eval_golden():
     from pasco_b200 import ops
-    from pasco_b200.synthetic import make_scene
     ops.set_precision("fp32")
     meta = MANIFEST["cases"]["big"]
-    net, gold = _load_eval(_pasconet(1), "big")
-    b = make_scene(meta["grid"], meta["occ"], 1, seed=meta["seed"])
-    out, calls, calls_ref = _check_fused_vs_unfused(net, b, 1)
+    net, gold = parity.load_eval(parity.pasconet(1), "big")
+    out, calls, calls_ref = _check_fused_vs_unfused(net, parity.scene(meta), 1)
     # 1.74 M decoder voxels: argmax near-ties keep ~20 scale-1 and ~3 scale-2 voxels other than the CPU run (the parent
     # engine does the same; this forward is bit-identical to it), and a flipped voxel changes the features of its
     # neighbourhood through the residual blocks, the voxel head and the attention masks.  Measured on an H100: voxel-logit
     # row error 1.4e-4 at the 95th percentile, 8e-3 at the 99th; every other output 1.2e-4 at the 99th.  Bound: the 95th
     # percentile at 1e-3 and the median at 5e-4 (test_golden_r2's near-tie rule with the cap-branch quantile's margin).
-    rep = _check_golden(out, meta, gold, q=0.95)
+    rep = parity.check_outputs(out, gold, meta, q=0.95)
     print(f"eval benchmark scale: C-ABI calls fused {calls} / unfused {calls_ref};", rep)
 
 
 def _reference_net():
-    from test_dropin_reference import REF, _reference_net as make
-    if not os.path.isdir(os.path.join(REF, "pasco")):
+    if not os.path.isdir(os.path.join(parity.REF, "pasco")):
         pytest.skip("oracle/_ref not staged")
-    return make()
+    return parity.reference_net()
 
 
 @pytest.mark.gpu
 def test_unmodified_reference_eval_on_the_engine_matches_golden():
     from pasco_b200 import ops
-    from pasco_b200.synthetic import make_scene
-    from test_dropin_reference import _forward_reference
     ops.set_precision("fp32")
     ME, net = _reference_net()
-    net, gold = _load_eval(net, "m1", ref_names=False)
-    dev = torch.device("cuda")
+    net, gold = parity.load_eval(net, "m1", ref_names=False)
     meta = MANIFEST["cases"]["m1"]
-    b = make_scene(meta["grid"], meta["occ"], 1, seed=meta["seed"])
     before = _stats(net)
-    ops.PROFILE = []
-    try:
-        with torch.no_grad():
-            out = _forward_reference(ME, net, b, dev, test=True)
-        launches = _launches()
-    finally:
-        ops.PROFILE = None
+    with torch.no_grad(), parity.launches() as launches:
+        out = parity.forward_reference(ME, net, parity.scene(meta), torch.device("cuda"), test=True)
     assert all(torch.equal(v, _stats(net)[k]) for k, v in before.items())
     assert launches and not [x for x in launches if x[1] == "simt"]
-    rep = _check_golden(out, MANIFEST["cases"]["m1"], gold)
+    rep = parity.check_outputs(out, gold, meta)
     print("drop-in eval vs golden:", rep)
 
 
@@ -381,19 +288,15 @@ def test_unmodified_step_inference_runs_on_the_engine():
     """eval.py's path: Net.step_inference(batch, "test") in eval mode — the forward, the reference Ensembler and
     panoptic_inference (eval=False: no metrics)."""
     from pasco_b200 import ops
-    from pasco_b200.synthetic import make_scene
     ops.set_precision("fp32")
     ME, net = _reference_net()
-    net, _ = _load_eval(net, "m1", ref_names=False)
+    net, _ = parity.load_eval(net, "m1", ref_names=False)
     dev = torch.device("cuda")
-    meta = MANIFEST["cases"]["m1"]
-    b = make_scene(meta["grid"], meta["occ"], 1, seed=meta["seed"])
-    batch = _RecordingBatch(in_feats=[t.to(dev) for t in b["in_feats"]], in_coords=[t.to(dev) for t in b["in_coords"]],
-                            min_Cs=[t.to(dev) for t in b["min_Cs"]], max_Cs=[t.to(dev) for t in b["max_Cs"]],
-                            Ts=[t.to(dev) for t in b["Ts"]], global_min_Cs=b["global_min_Cs"].to(dev),
-                            global_max_Cs=b["global_max_Cs"].to(dev),
-                            geo_labels={k: v.to(dev) for k, v in b["sem_labels"].items()},
-                            mask_classes=b["mask_classes"].to(dev))
+    sc = parity.scene(MANIFEST["cases"]["m1"])
+    batch = _RecordingBatch(in_feats=sc["in_feats"], in_coords=sc["in_coords"], min_Cs=[t.to(dev) for t in sc["min_Cs"]],
+                            max_Cs=[t.to(dev) for t in sc["max_Cs"]], Ts=[t.to(dev) for t in sc["Ts"]],
+                            global_min_Cs=sc["global_min_Cs"].to(dev), global_max_Cs=sc["global_max_Cs"].to(dev),
+                            geo_labels=sc["sem_labels"], mask_classes=sc["mask_classes"])
     c0 = ops.CALLS
     with torch.no_grad():
         res = net.step_inference(batch, "test")

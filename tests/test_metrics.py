@@ -17,7 +17,6 @@ against a fixture the reference's own code produced (tests/golden/make_golden_ev
 import json
 import math
 import os
-import re
 import sys
 import warnings
 
@@ -32,6 +31,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, GOLD)
 import make_golden_eval as GE  # noqa: E402  (gt_scene rebuilds the fixture's ground truth; the reference is not imported)
 import make_golden_predict as GP  # noqa: E402
+import parity  # noqa: E402
 
 from pasco_b200 import metrics as MT  # noqa: E402
 
@@ -54,15 +54,6 @@ ECE_ATOL = 1e-7
 # ------------------------------------------------------------------------------------------------
 # CPU
 # ------------------------------------------------------------------------------------------------
-def test_header_and_prototypes():
-    from pasco_b200._lib import PROTOTYPES
-    hdr = open(os.path.join(ROOT, "include", "pasco_sm100.h")).read()
-    for name in ("pasco_eval_gt", "pasco_eval_pairs", "pasco_eval_ssc", "pasco_eval_vox"):
-        m = re.search(r"int " + name + r"\(([^;]*)\);", hdr)
-        assert m, name
-        assert len(m.group(1).split(",")) == len(PROTOTYPES[name][1]), name
-
-
 def test_calibration_error_bins():
     conf = torch.tensor([1.0, 0.5, 0.05, 1.0])
     correct = torch.tensor([True, False, True, False])
@@ -361,19 +352,14 @@ def test_calibration_slots_at_fp32_boundaries():
 def test_pasconet_predict_end_to_end():
     """PascoNet.predict(keep_sem_rows=True) on fixture (b)'s scene, evaluated by the device passes, gives the integer
     tables of the restatement fed by ensemble.py's post-processing of the same network outputs."""
-    from test_inference import _load_eval, _pasconet
-    from test_inference import MANIFEST as IM
     from pasco_b200 import ops
-    from pasco_b200.synthetic import make_scene
     import make_golden_predict as P_GP
     thr = json.load(open(os.path.join(GOLD, "predict_manifest.json")))["b"]["thresholds"]
     ops.set_precision("fp32")
-    meta = IM["cases"]["m2"]
-    net, _ = _load_eval(_pasconet(2), "m2")
-    b = make_scene(meta["grid"], meta["occ"], 2, seed=meta["seed"])
+    net, _ = parity.load_eval(parity.pasconet(2), "m2")
+    b = parity.scene(parity.INFER_MANIFEST["cases"]["m2"], 2)
     dev = torch.device("cuda")
-    args = ([f.to(dev) for f in b["in_feats"]], [c.to(dev) for c in b["in_coords"]], b["global_min_Cs"],
-            b["global_max_Cs"], b["min_Cs"], b["max_Cs"])
+    args = (b["in_feats"], b["in_coords"], b["global_min_Cs"], b["global_max_Cs"], b["min_Cs"], b["max_Cs"])
     Ts = P_GP.poses()[:2]
     entries = net.predict(*args, Ts, keep_sem_rows=True, **thr)
     with torch.no_grad():

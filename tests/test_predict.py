@@ -17,7 +17,6 @@ import collections
 import json
 import math
 import os
-import re
 import sys
 import warnings
 
@@ -31,6 +30,7 @@ GOLD = os.path.join(HERE, "golden")
 sys.path.insert(0, ROOT)
 sys.path.insert(0, GOLD)
 import make_golden_predict as GP  # noqa: E402  (scene_a rebuilds fixture (a)'s inputs; the reference is not imported)
+import parity  # noqa: E402
 
 FIX_A = np.load(os.path.join(GOLD, "predict_post.npz"))
 FIX_B = np.load(os.path.join(GOLD, "predict_e2e.npz"))
@@ -166,31 +166,6 @@ def test_confidence_outputs_match_the_literal_reference_loop():
     assert torch.equal(pan, rp) and torch.equal(sem, rs) and torch.equal(conf, rc)
     _same_infos(infos, ri)
     assert pan[20:40].eq(1).all() and sem[20:40].eq(0).all() and conf[20:40].eq(0).all() and conf[:20].gt(0.99).all()
-
-
-_CT = {"void*": "p", "int32_t*": "p", "float*": "p", "uint8_t*": "p", "uint64_t*": "p", "float": "f", "double": "d",
-       "int64_t": "i64", "int32_t": "i32", "uint64_t": "u64", "pasco_stream_t": "p"}
-NEW = ["pasco_pose_lookup", "pasco_cell_mask_or", "pasco_lookup_rows", "pasco_mask_rows_sigmoid", "pasco_mask_merge",
-       "pasco_softmax_rows", "pasco_soft_iou", "pasco_sem_ensemble", "pasco_panoptic_pass1", "pasco_panoptic_segments",
-       "pasco_panoptic_pass2"]
-
-
-@pytest.mark.parametrize("name", NEW)
-def test_entry_point_header_matches_ctypes(name):
-    from pasco_b200 import _lib
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "pasco_sm100.h")).read(), flags=re.S)
-    m = re.search(rf"int\s+{name}\s*\(([^;]*)\);", src)
-    assert m, f"{name} is not declared"
-    kinds = []
-    for arg in m.group(1).split(","):
-        arg = re.sub(r"\[\d*\]", "*", arg.replace("const", ""))          # float T[12], const float* const probs[]
-        words = arg.replace("*", " * ").split()
-        kinds.append("p" if "*" in words else _CT[words[0]])
-    ctm = {_lib.C.c_void_p: "p", _lib.C.c_int64: "i64", _lib.C.c_int32: "i32", _lib.C.c_float: "f",
-           _lib.C.c_double: "d", _lib.C.c_uint64: "u64"}
-    res, args = _lib.PROTOTYPES[name]
-    assert res is _lib.C.c_int
-    assert [ctm[a] for a in args] == kinds
 
 
 def test_predict_refuses_training_mode():
@@ -472,16 +447,13 @@ def test_pasconet_predict_matches_reference_fixture_b():
     """PascoNet.predict on the net_cfg1 scene at M = 2 (calibrated running statistics of net_cfg1_infer_m2.npz) against the
     reference's Net.forward(return_ensemble=True) + panoptic_inference, with the eval tests' near-tie tolerance: the
     forward agrees to rounding, so a few argmax near-ties may move rows; everything else must agree."""
-    from test_inference import MANIFEST as IM, _load_eval, _pasconet
     from pasco_b200 import ops, predict as P
-    from pasco_b200.synthetic import make_scene
     ops.set_precision("fp32")
-    meta = IM["cases"]["m2"]
-    net, _ = _load_eval(_pasconet(2), "m2")
-    b = make_scene(meta["grid"], meta["occ"], 2, seed=meta["seed"])
-    dev = torch.device("cuda")
-    got = net.predict([f.to(dev) for f in b["in_feats"]], [c.to(dev) for c in b["in_coords"]], b["global_min_Cs"],
-                      b["global_max_Cs"], b["min_Cs"], b["max_Cs"], GP.poses()[:2], **MANIFEST["b"]["thresholds"])
+    meta = parity.INFER_MANIFEST["cases"]["m2"]
+    net, _ = parity.load_eval(parity.pasconet(2), "m2")
+    b = parity.scene(meta, 2)
+    got = net.predict(b["in_feats"], b["in_coords"], b["global_min_Cs"], b["global_max_Cs"], b["min_Cs"], b["max_Cs"],
+                      GP.poses()[:2], **MANIFEST["b"]["thresholds"])
     z = FIX_B
     assert len(got) == 3
     rep = {}

@@ -7,33 +7,23 @@ GPU part : the kernels against an fp64 reference for Q = 129 … 385, the rows o
            come from net_cfg1.npz).
 CPU part : the golden manifest's parameter names / shapes equal PascoNet(num_queries=200).reference_state_dict().
 """
-import json
 import os
 import sys
 
-import numpy as np
 import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-REF = os.path.join(ROOT, "oracle", "_ref")
 sys.path.insert(0, os.path.join(HERE, "golden"))
+import parity  # noqa: E402
 from recipe import fill_state_dict  # noqa: E402
-from test_golden_net import _compare  # noqa: E402
 
 NQ = 200
-MANIFEST = json.load(open(os.path.join(HERE, "golden", f"net_cfg1_q{NQ}_manifest.json")))
-
-
-def _pasconet():
-    from pasco_b200.net3d import PascoNet
-    torch.manual_seed(0)
-    return PascoNet(n_classes=20, n_infers=1, in_channels=283, f=64, num_queries=NQ, heavy_decoder=False)
+MANIFEST = parity.manifest(f"net_cfg1_q{NQ}_manifest.json")
 
 
 def test_q200_manifest_matches_pasconet_state_dict():
-    mine = {k: list(v.shape) for k, v in _pasconet().reference_state_dict().items()}
+    mine = {k: list(v.shape) for k, v in parity.pasconet(num_queries=NQ).reference_state_dict().items()}
     ref = MANIFEST["params"]
     assert MANIFEST["num_queries"] == NQ
     assert sorted(mine) == sorted(ref), (sorted(set(ref) - set(mine))[:5], sorted(set(mine) - set(ref))[:5])
@@ -45,11 +35,6 @@ def test_q200_manifest_matches_pasconet_state_dict():
 # ------------------------------------------------------------------------------------------------
 # kernel
 # ------------------------------------------------------------------------------------------------
-def _relerr(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).abs().max() / b.abs().max().clamp(min=1e-30))
-
-
 def _inputs(Q, P, H, D, masked, seed):
     g = torch.Generator().manual_seed(seed)
     q, k, v = (torch.randn(n, H * D, generator=g) for n in (Q, P, P))
@@ -107,8 +92,8 @@ def test_xattn_many_queries_matches_fp64_reference(Q, P, H, D, masked):
     qg, kg, vg = (t.clone().cuda().requires_grad_(True) for t in (q, k, v))
     yg = ops.MaskedCrossAttention.apply(qg, kg, vg, mask.cuda() if mask is not None else None, H)
     (yg * up.cuda()).sum().backward()
-    e = _relerr(yg, yr)
-    eg = max(_relerr(qg.grad, qr.grad), _relerr(kg.grad, kr.grad), _relerr(vg.grad, vr.grad))
+    e = parity.relerr(yg, yr)
+    eg = max(parity.relerr(qg.grad, qr.grad), parity.relerr(kg.grad, kr.grad), parity.relerr(vg.grad, vr.grad))
     print(f"xattn Q={Q} P={P} H={H} D={D} masked={masked}: fwd {e:.2e} grads {eg:.2e}")
     assert e <= 1e-4 and eg <= 5e-4
 
@@ -152,61 +137,29 @@ def test_xattn_many_queries_is_deterministic():
 # ------------------------------------------------------------------------------------------------
 # network: PascoNet and the hooked unmodified reference with num_queries=200
 # ------------------------------------------------------------------------------------------------
-def _gold():
-    return np.load(os.path.join(HERE, "golden", f"net_cfg1_q{NQ}.npz"))
-
-
-def _check_against_gold(out, gold, sem=True):
-    cfg1 = np.load(os.path.join(HERE, "golden", MANIFEST["coords_and_sem_from"]))
-    cfg1_step = json.load(open(os.path.join(HERE, "golden", "net_cfg1_manifest.json")))["row_step"]
-    report = {}
-    if sem:
-        for s in (4, 2, 1):
-            lg = out["sem_logits_at_scales"][s][0]
-            report[f"sem{s}"] = _compare(f"sem{s}", lg.C, lg.F, cfg1[f"sem{s}_C"], cfg1[f"sem{s}_F"], cfg1_step)
+def _check_against_gold(out, sem=True):
+    """Coordinates and semantic logits from net_cfg1 at its row step, the voxel rows at the q200 step."""
     p = out["panop_predictions"][0]
-    vox = p["voxel_logits"]
-    assert p["query_logits"].shape[-2] == NQ and vox.F.shape[1] == NQ
-    report["vox"] = _compare("voxel_logits", vox.C, vox.F, cfg1["vox_C"], gold["vox_F"], MANIFEST["row_step"])
-    if report["vox"][0] == 0:                  # same coordinates: the checksums over all rows agree too
-        f = vox.F.detach().double()
-        got = torch.stack([f.sum(), f.abs().sum()]).cpu().numpy()
-        report["vox_sum"] = float(np.abs(got - gold["vox_sum"]).max() / gold["vox_sum"][1])
-        assert report["vox_sum"] <= 1e-3, report
-    q = p["query_logits"][0].detach().cpu().double()
-    report["query"] = float((q - torch.as_tensor(gold["query_logits"]).double()).abs().max()
-                            / np.abs(gold["query_logits"]).max())
-    assert report["query"] <= 1e-3, report
-    for i, aux in enumerate(p["aux_outputs"]):
-        ea = float((aux["query_logits"][0].detach().cpu().double() - torch.as_tensor(gold[f"aux{i}_query_logits"]).double()).abs().max()
-                   / np.abs(gold[f"aux{i}_query_logits"]).max())
-        assert ea <= 1e-3, f"aux {i} query logits error {ea:.3e}"
-    return report
+    assert p["query_logits"].shape[-2] == NQ and p["voxel_logits"].F.shape[1] == NQ
+    gold = dict(parity.fixture(MANIFEST["coords_and_sem_from"]), **parity.fixture(f"net_cfg1_q{NQ}.npz"))
+    return parity.check_outputs(out, gold, parity.manifest("net_cfg1_manifest.json"), sem=sem, sums=True,
+                                vox_step=MANIFEST["row_step"])
 
 
 @pytest.mark.gpu
 def test_pasconet_200_queries_matches_reference_golden_and_trains():
     from pasco_b200 import ops
     from pasco_b200.losses import total_loss
-    from pasco_b200.synthetic import make_scene
     ops.set_precision("fp32")
-    net = _pasconet()
-    net.load_reference_state_dict(fill_state_dict(net.reference_state_dict()))
-    net.cuda().train()
-    dev = torch.device("cuda")
-    b = make_scene(MANIFEST["grid"], MANIFEST["occ"], 1, seed=MANIFEST["seed"])
+    net = parity.pasconet(num_queries=NQ, recipe=True).cuda().train()
+    sc = parity.scene(MANIFEST)
     with torch.no_grad():
-        out = net([f.to(dev) for f in b["in_feats"]], [c.to(dev) for c in b["in_coords"]],
-                  b["global_min_Cs"], b["global_max_Cs"], b["min_Cs"], b["max_Cs"])
-    print("PascoNet num_queries=200 vs golden:", _check_against_gold(out, _gold()))
+        out = parity.forward(net, sc)
+    print("PascoNet num_queries=200 vs golden:", _check_against_gold(out))
 
     # one training step: forward + loss + backward, every transformer parameter gets a finite gradient
-    d = lambda t: t.to(dev)  # noqa: E731
-    scd = dict(b, in_feats=[d(t) for t in b["in_feats"]], in_coords=[d(t) for t in b["in_coords"]],
-               sem_labels={k: d(v) for k, v in b["sem_labels"].items()}, mask_classes=d(b["mask_classes"]))
     opt = torch.optim.SGD(net.parameters(), lr=1e-4)
-    out = net(scd["in_feats"], scd["in_coords"], b["global_min_Cs"], b["global_max_Cs"], b["min_Cs"], b["max_Cs"])
-    loss = total_loss(out, scd, 20, net.class_frequencies)
+    loss = total_loss(parity.forward(net, sc), sc, 20, net.class_frequencies)
     loss.backward()
     torch.cuda.synchronize()
     assert torch.isfinite(loss), loss
@@ -220,33 +173,21 @@ def test_pasconet_200_queries_matches_reference_golden_and_trains():
 
 
 @pytest.mark.gpu
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "pasco")),
+@pytest.mark.skipif(not os.path.isdir(os.path.join(parity.REF, "pasco")),
                     reason="no upstream PaSCo checkout was readable when build() ran: oracle/_ref not staged")
 def test_reference_200_queries_with_attention_hooks_matches_golden():
     from pasco_b200 import ops, hooks
-    from pasco_b200.synthetic import make_scene
-    from test_dropin_reference import _forward_reference
     ops.set_precision("fp32")
-    for p in (REF, os.path.join(ROOT, "compat")):
-        if p not in sys.path:
-            sys.path.insert(0, p)
-    import MinkowskiEngine as ME
-    from pasco.models.net_panoptic_sparse import Net
-    n_classes = 20
-    torch.manual_seed(0)
-    net = Net(n_classes=n_classes, class_names=[str(i) for i in range(n_classes)], class_weights=torch.ones(n_classes),
-              encoder_dropouts=[0.0] * 3, decoder_dropouts=[0.0] * 3, dense3d_dropout=0.0, n_infers=1,
-              class_frequencies={f"1_{s}": np.ones(n_classes) for s in (1, 2, 4)}, in_channels=283, num_queries=NQ,
-              f=64, heavy_decoder=False)
+    dev = torch.device("cuda")
+    ME, net = parity.reference_net(num_queries=NQ)
     net.load_state_dict(fill_state_dict(net.state_dict()))
-    net.to(torch.device("cuda")).train()
+    net.to(dev).train()
     assert hooks.install()
     try:
-        b = make_scene(MANIFEST["grid"], MANIFEST["occ"], 1, seed=MANIFEST["seed"])
         calls0 = ops.CALLS
-        out = _forward_reference(ME, net, b, torch.device("cuda"))
+        out = parity.forward_reference(ME, net, parity.scene(MANIFEST), dev)
         assert ops.CALLS - calls0 > 100
-        report = _check_against_gold(out, _gold(), sem=False)
+        report = _check_against_gold(out, sem=False)
         p = out["panop_predictions"][0]
         (p["voxel_logits"].F.square().mean() + p["query_logits"].square().mean()).backward()
         g = net.transformer_predictor.transformer_cross_attention_layers[1].multihead_attn.in_proj_weight.grad
