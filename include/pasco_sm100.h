@@ -302,23 +302,45 @@ int pasco_sem_ensemble(int32_t M, const float* const probs[], const int32_t* con
 /* helper.py:135-186 pass 1 over the mask probabilities probs [n, Q] with class probabilities query_probs [Q, K1]:
  * a query is kept when its first-argmax label is neither 0 nor K1 − 1 and its max > object_mask_threshold; per row,
  * win = (q << 1) | (m_q >= vox_occ_threshold) for the kept q maximising prob_q * m_q (lowest q on ties), −1 without a
- * kept query; m_win = m_q, m_sum = the sum of m over kept queries.  areas int32 [2Q], zeroed by the caller: [0, Q) the
- * mask_area and [Q, 2Q) the original_area of every query (integer counts).                                          */
+ * kept query; m_win = m_q, m_sum = the sum of m over kept queries; c_sum (NULL allowed) = the sum of prob_q * m_q over
+ * kept queries.  areas int32 [2Q], zeroed by the caller: [0, Q) the mask_area and [Q, 2Q) the original_area of every
+ * query (integer counts).                                                                                           */
 int pasco_panoptic_pass1(const float* probs, int64_t n, int32_t Q, const float* query_probs, int32_t K1,
                          float object_mask_threshold, float vox_occ_threshold, int32_t* win, float* m_win, float* m_sum,
-                         int32_t* areas, pasco_stream_t s);
+                         float* c_sum, int32_t* areas, pasco_stream_t s);
 /* helper.py:187-250 on one thread: the walk over kept queries in ascending order (overlap filter mask_area /
  * original_area in double, stuff classes merged into their first segment, sequential ids).  seg_of / cls_of int32 [Q]:
  * the segment id a query paints (0 none) and its semantic class (−1 for merged stuff, which keeps semantic 0).
  * records int32 [1 + 4Q]: the segment count, then per segment (query, class, float bits of the class probability,
- * isthing).  thing_mask bit c = class c is a thing class; K1 <= 65.                                                 */
+ * isthing).  kept (NULL allowed) int32 [1 + Q]: the kept-query count kq, then the kept queries in ascending order.
+ * thing_mask bit c = class c is a thing class; K1 <= 65.                                                           */
 int pasco_panoptic_segments(const float* query_probs, int32_t Q, int32_t K1, float object_mask_threshold,
                             double overlap_threshold, uint64_t thing_mask, const int32_t* areas, int32_t* seg_of,
-                            int32_t* cls_of, int32_t* records, pasco_stream_t s);
+                            int32_t* cls_of, int32_t* records, int32_t* kept, pasco_stream_t s);
 /* helper.py:236-247 pass 2 from the pass-1 records: panoptic / semantic int32 [n] and the confidence fp32 [n] =
  * m_win / (m_sum + 1e-8) on rows painted by a non-merged segment, 0 elsewhere.                                     */
 int pasco_panoptic_pass2(const int32_t* win, const float* m_win, const float* m_sum, int64_t n, const int32_t* seg_of,
                          const int32_t* cls_of, int32_t* panoptic, int32_t* semantic, float* confidence, pasco_stream_t s);
+/* helper.py:246-281: the dense volumes of panoptic_inference from the rows of passes 1 and 2.  Row r (coords int32
+ * [n, 4], batch 0) lands at cell coord − min_c of the X x Y x Z box; every output is zeroed by the caller.  panoptic /
+ * semantic int32 and confidence fp32 [X, Y, Z] take the pass-2 rows; on rows with semantic != 0 (painted by a segment
+ * of its own), ins_uncertainty = the winner's class probability, vox_uncertainty = prob_q * m_q / c_sum and
+ * all_mask_probs fp32 [kq, X, Y, Z] = probs[r, kept[k]] (kept int32 [kq]: the kept queries, as pass 1 orders them).
+ * A row outside the box or of another batch sets *err_flag = 1 and is skipped.                                     */
+int pasco_panoptic_dense(const int32_t* coords, int64_t n, const int32_t min_c[3], int32_t X, int32_t Y, int32_t Z,
+                         const int32_t* panoptic_rows, const int32_t* semantic_rows, const float* confidence_rows,
+                         const int32_t* win, const float* m_win, const float* c_sum, const float* query_probs, int32_t K1,
+                         const float* probs, int32_t Q, const int32_t* kept, int32_t kq, int32_t* panoptic,
+                         int32_t* semantic, float* confidence, float* ins_uncertainty, float* vox_uncertainty,
+                         float* all_mask_probs, int32_t* err_flag, pasco_stream_t s);
+/* ensembler.py:159-187: the dense class distributions [K, cells] of ensemble_sem_compl.  subnet_out (NULL allowed, or a
+ * host array of M device pointers, each NULL allowed) [m] = subnet m's softmax row at every cell where it has one and
+ * one-hot class 0 elsewhere; ensemble_out (NULL allowed) = their mean, computed as pasco_sem_ensemble computes it; gate
+ * (NULL allowed) [cells] = first argmax of that mean != 0.  probs / cell_rows as in pasco_sem_ensemble.             */
+int pasco_sem_dense(int32_t M, const float* const probs[], const int32_t* const cell_rows[], int64_t cells, int32_t K,
+                    float* const subnet_out[], float* ensemble_out, uint8_t* gate, pasco_stream_t s);
+/* ensembler.py:102-105: gate [cells] = first argmax over the K channels of dense [K, cells] != 0.                   */
+int pasco_class_gate(const float* dense, int64_t cells, int32_t K, uint8_t* gate, pasco_stream_t s);
 
 /* ---- evaluation of the predictions against a scene's ground truth: the counting passes of Net.evaluate_all
  *      (net_panoptic_sparse.py:650-765), finished on the host by pasco_b200/metrics.py --------------------------------

@@ -69,9 +69,13 @@ PROTOTYPES = {
     "pasco_softmax_rows": (C.c_int, [_p, _p, _i64, _i32, _p, _p]),
     "pasco_soft_iou": (C.c_int, [_p, _i32, _i64, _p, _p, C.c_float, _p, _p]),
     "pasco_sem_ensemble": (C.c_int, [_i32, _p, _p, _p, _i64, _i32, _p, _p, _p, _p]),
-    "pasco_panoptic_pass1": (C.c_int, [_p, _i64, _i32, _p, _i32, C.c_float, C.c_float, _p, _p, _p, _p, _p]),
-    "pasco_panoptic_segments": (C.c_int, [_p, _i32, _i32, C.c_float, C.c_double, C.c_uint64, _p, _p, _p, _p, _p]),
+    "pasco_panoptic_pass1": (C.c_int, [_p, _i64, _i32, _p, _i32, C.c_float, C.c_float, _p, _p, _p, _p, _p, _p]),
+    "pasco_panoptic_segments": (C.c_int, [_p, _i32, _i32, C.c_float, C.c_double, C.c_uint64, _p, _p, _p, _p, _p, _p]),
     "pasco_panoptic_pass2": (C.c_int, [_p, _p, _p, _i64, _p, _p, _p, _p, _p, _p]),
+    "pasco_panoptic_dense": (C.c_int, [_p, _i64, _p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _i32, _p,
+                                       _i32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "pasco_sem_dense": (C.c_int, [_i32, _p, _p, _i64, _i32, _p, _p, _p, _p]),
+    "pasco_class_gate": (C.c_int, [_p, _i64, _i32, _p, _p]),
     "pasco_eval_gt": (C.c_int, [_p, _i32, _p, _p, _i64, _i32, _i32, _p, _p, _p, _p, _p]),
     "pasco_eval_pairs": (C.c_int, [_p, _p, _i64, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
     "pasco_eval_ssc": (C.c_int, [_p, _p, _p, _i64, _p, _i64, _i32, _p, _i32, _p, _p, _p, _p, _p, _p, _p]),

@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(256) k_panoptic_pass1(const float* __restrict_
                                                         const float* __restrict__ qp, int K1, float mask_thr,
                                                         float vox_thr, int32_t* __restrict__ win,
                                                         float* __restrict__ m_win, float* __restrict__ m_sum,
-                                                        int32_t* __restrict__ areas) {
+                                                        float* __restrict__ c_sum, int32_t* __restrict__ areas) {
   extern __shared__ int s_mem[];
   int* s_q = s_mem;                                            // [Q] kept query ids
   float* s_p = reinterpret_cast<float*>(s_mem + Q);            // [Q] their class probabilities
@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(256) k_panoptic_pass1(const float* __restrict_
   const int64_t w0 = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t r = w0; r < n; r += nw) {
     const float* row = probs + r * Q;
-    float best = -INFINITY, bm = 0.f, sum = 0.f;
+    float best = -INFINITY, bm = 0.f, sum = 0.f, csum = 0.f;
     int bk = 0x7fffffff;
     for (int k = lane; k < kq; k += 32) {
       const int q = s_q[k];
@@ -285,6 +285,7 @@ __global__ void __launch_bounds__(256) k_panoptic_pass1(const float* __restrict_
         bm = m;
       }
       sum = __fadd_rn(sum, m);
+      csum = __fadd_rn(csum, cmb);
       if (m >= vox_thr) atomicAdd(s_orig + q, 1);
     }
 #pragma unroll
@@ -297,6 +298,7 @@ __global__ void __launch_bounds__(256) k_panoptic_pass1(const float* __restrict_
         bm = om;
       }
       sum = __fadd_rn(sum, __shfl_xor_sync(0xffffffffu, sum, d));
+      csum = __fadd_rn(csum, __shfl_xor_sync(0xffffffffu, csum, d));
     }
     if (lane == 0) {
       if (kq == 0) {
@@ -310,6 +312,7 @@ __global__ void __launch_bounds__(256) k_panoptic_pass1(const float* __restrict_
         m_win[r] = bm;
       }
       m_sum[r] = sum;
+      if (c_sum) c_sum[r] = csum;
     }
   }
   __syncthreads();
@@ -323,17 +326,19 @@ __global__ void __launch_bounds__(256) k_panoptic_pass1(const float* __restrict_
 __global__ void k_panoptic_segments(const float* __restrict__ qp, int Q, int K1, float mask_thr, double overlap_thr,
                                     unsigned long long thing_mask, const int32_t* __restrict__ areas,
                                     int32_t* __restrict__ seg_of, int32_t* __restrict__ cls_of,
-                                    int32_t* __restrict__ records) {
+                                    int32_t* __restrict__ records, int32_t* __restrict__ kept) {
   __shared__ int stuff_id[64];                                 // segment id of every stuff class seen so far
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   for (int c = 0; c < 64; ++c) stuff_id[c] = 0;
-  int cur = 0;
+  int cur = 0, kq = 0;
   for (int q = 0; q < Q; ++q) {
     seg_of[q] = 0;
     cls_of[q] = 0;
     float pr;
     int lb;
     if (!query_kept(qp, q, K1, mask_thr, pr, lb)) continue;
+    if (kept) kept[1 + kq] = q;
+    ++kq;
     const int ma = areas[q], oa = areas[Q + q];
     if (!(ma > 0 && oa > 0) || (double)ma / (double)oa < overlap_thr) continue;
     const bool isthing = (thing_mask >> lb) & 1ull;             // lb < K1 - 1 <= 64
@@ -353,6 +358,7 @@ __global__ void k_panoptic_segments(const float* __restrict__ qp, int Q, int K1,
     rec[3] = isthing;
   }
   records[0] = cur;
+  if (kept) kept[0] = kq;
 }
 
 __global__ void k_panoptic_pass2(const int32_t* __restrict__ win, const float* __restrict__ m_win,
@@ -376,6 +382,116 @@ __global__ void k_panoptic_pass2(const int32_t* __restrict__ win, const float* _
     pan[i] = p;
     sem[i] = s;
     conf[i] = cf;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// dense volumes of panoptic_inference (helper.py:206-281): rows → channel-first [C, X, Y, Z] at coord − min_c
+// ------------------------------------------------------------------------------------------------
+struct PanopticDenseParams {
+  const int32_t* coords;                 // [n, 4] (batch, x, y, z)
+  int64_t n;
+  int min_c[3];
+  int X, Y, Z;
+  const int32_t* pan_row;                // pass 2
+  const int32_t* sem_row;
+  const float* conf_row;
+  const int32_t* win;                    // pass 1
+  const float* m_win;
+  const float* c_sum;
+  const float* qp;                       // [Q, K1]
+  int K1;
+  const float* probs;                    // [n, Q]
+  int Q;
+  const int32_t* kept;                   // [kq]: the query of every kept column, ascending
+  int kq;
+  int32_t* pan;                          // [X, Y, Z]
+  int32_t* sem;
+  float* conf;
+  float* ins;
+  float* vox;
+  float* all;                            // [kq, X, Y, Z]
+  int32_t* err;
+};
+
+// one thread per row, so rows in ascending cell order write every plane coalesced; the volumes are zeroed by the caller
+__global__ void k_panoptic_dense(const __grid_constant__ PanopticDenseParams p) {
+  const int64_t cells = (int64_t)p.X * p.Y * p.Z;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < p.n; r += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t* c = p.coords + 4 * r;
+    const int x = __ldg(c + 1) - p.min_c[0], y = __ldg(c + 2) - p.min_c[1], z = __ldg(c + 3) - p.min_c[2];
+    if (__ldg(c) != 0 || x < 0 || x >= p.X || y < 0 || y >= p.Y || z < 0 || z >= p.Z) {
+      *p.err = 1;
+      continue;
+    }
+    const int64_t cell = ((int64_t)x * p.Y + y) * p.Z + z;
+    const int s = __ldg(p.sem_row + r);
+    p.pan[cell] = __ldg(p.pan_row + r);
+    p.sem[cell] = s;
+    p.conf[cell] = __ldg(p.conf_row + r);
+    if (s == 0) continue;     // not painted by a segment of its own: class 0, merged stuff or no segment (all stay 0)
+    const int q = __ldg(p.win + r) >> 1;
+    float pr;
+    int lb;
+    query_kept(p.qp, q, p.K1, 0.f, pr, lb);
+    p.ins[cell] = pr;
+    // max_k(c_k / Σc) = max_k(c_k) / Σc: one rounding, monotone; the winner's c_k is pass 1's product
+    p.vox[cell] = __fdiv_rn(__fmul_rn(pr, __ldg(p.m_win + r)), __ldg(p.c_sum + r));
+    const float* row = p.probs + r * p.Q;
+    for (int k = 0; k < p.kq; ++k) p.all[k * cells + cell] = __ldg(row + __ldg(p.kept + k));
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// dense class distributions of ensemble_sem_compl (ensembler.py:159-187): one thread per cell, a loop over channels
+// ------------------------------------------------------------------------------------------------
+struct SemDenseOut {
+  float* sub[kMaxSubnets];   // [K, cells] of subnet m: its softmax row, one-hot class 0 where it has none (NULL = skip)
+  float* ens;                // [K, cells] the mean over the subnets (NULL = skip)
+  uint8_t* gate;             // [cells] argmax of ens != 0 (NULL = skip)
+};
+
+__global__ void k_sem_dense(const __grid_constant__ SemParams p, const __grid_constant__ SemDenseOut o, int64_t cells,
+                            int K) {
+  for (int64_t cell = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; cell < cells;
+       cell += (int64_t)gridDim.x * blockDim.x) {
+    int64_t r[kMaxSubnets];
+    sem_rows_at(p, cell, r);
+#pragma unroll
+    for (int m = 0; m < kMaxSubnets; ++m) {      // unrolled: r[] stays in registers
+      if (m >= p.M || !o.sub[m]) continue;
+      for (int c = 0; c < K; ++c)
+        o.sub[m][c * cells + cell] = r[m] >= 0 ? __ldg(p.prob[m] + r[m] * K + c) : (c == 0 ? 1.f : 0.f);
+    }
+    if (!o.ens && !o.gate) continue;
+    float best = -INFINITY;
+    int arg = 0;
+    for (int c = 0; c < K; ++c) {
+      const float v = sem_mean_prob(p, r, K, c);       // the value k_sem_ensemble ranks, so the gates agree
+      if (o.ens) o.ens[c * cells + cell] = v;
+      if (v > best) {                                  // first maximum, as torch.argmax
+        best = v;
+        arg = c;
+      }
+    }
+    if (o.gate) o.gate[cell] = arg != 0;
+  }
+}
+
+// the occupancy gate of ensembler.py:102-105 from a given dense distribution [K, cells]: first argmax != 0
+__global__ void k_class_gate(const float* __restrict__ dense, int64_t cells, int K, uint8_t* __restrict__ gate) {
+  for (int64_t cell = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; cell < cells;
+       cell += (int64_t)gridDim.x * blockDim.x) {
+    float best = -INFINITY;
+    int arg = 0;
+    for (int c = 0; c < K; ++c) {
+      const float v = __ldg(dense + c * cells + cell);
+      if (v > best) {
+        best = v;
+        arg = c;
+      }
+    }
+    gate[cell] = arg != 0;
   }
 }
 
@@ -531,24 +647,25 @@ extern "C" int pasco_sem_ensemble(int32_t M, const float* const probs[], const i
 
 extern "C" int pasco_panoptic_pass1(const float* probs, int64_t n, int32_t Q, const float* query_probs, int32_t K1,
                                     float object_mask_threshold, float vox_occ_threshold, int32_t* win, float* m_win,
-                                    float* m_sum, int32_t* areas, pasco_stream_t s) {
+                                    float* m_sum, float* c_sum, int32_t* areas, pasco_stream_t s) {
   PASCO_CHECK_ARG(Q >= 1 && Q <= 8192 && K1 >= 2, "pasco_panoptic_pass1: 1 <= Q <= 8192 queries, K1 >= 2 classes");
   if (n == 0) return 0;
   const size_t smem = sizeof(int) * 4 * Q;
   cudaFuncSetAttribute(k_panoptic_pass1, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   k_panoptic_pass1<<<grid_for(n * 32, 256, 2), 256, smem, (cudaStream_t)s>>>(probs, n, Q, query_probs, K1,
                                                                             object_mask_threshold, vox_occ_threshold, win,
-                                                                            m_win, m_sum, areas);
+                                                                            m_win, m_sum, c_sum, areas);
   PASCO_CHECK_LAUNCH("pasco_panoptic_pass1");
   return 0;
 }
 
 extern "C" int pasco_panoptic_segments(const float* query_probs, int32_t Q, int32_t K1, float object_mask_threshold,
                                        double overlap_threshold, uint64_t thing_mask, const int32_t* areas,
-                                       int32_t* seg_of, int32_t* cls_of, int32_t* records, pasco_stream_t s) {
+                                       int32_t* seg_of, int32_t* cls_of, int32_t* records, int32_t* kept,
+                                       pasco_stream_t s) {
   PASCO_CHECK_ARG(K1 >= 2 && K1 <= 65, "pasco_panoptic_segments: 2 <= K1 <= 65 classes (got %d)", K1);
   k_panoptic_segments<<<1, 32, 0, (cudaStream_t)s>>>(query_probs, Q, K1, object_mask_threshold, overlap_threshold,
-                                                     (unsigned long long)thing_mask, areas, seg_of, cls_of, records);
+                                                     (unsigned long long)thing_mask, areas, seg_of, cls_of, records, kept);
   PASCO_CHECK_LAUNCH("pasco_panoptic_segments");
   return 0;
 }
@@ -560,5 +677,77 @@ extern "C" int pasco_panoptic_pass2(const int32_t* win, const float* m_win, cons
   k_panoptic_pass2<<<grid_for(n, 256), 256, 0, (cudaStream_t)s>>>(win, m_win, m_sum, n, seg_of, cls_of, panoptic, semantic,
                                                                   confidence);
   PASCO_CHECK_LAUNCH("pasco_panoptic_pass2");
+  return 0;
+}
+
+extern "C" int pasco_panoptic_dense(const int32_t* coords, int64_t n, const int32_t min_c[3], int32_t X, int32_t Y,
+                                    int32_t Z, const int32_t* panoptic_rows, const int32_t* semantic_rows,
+                                    const float* confidence_rows, const int32_t* win, const float* m_win,
+                                    const float* c_sum, const float* query_probs, int32_t K1, const float* probs,
+                                    int32_t Q, const int32_t* kept, int32_t kq, int32_t* panoptic, int32_t* semantic,
+                                    float* confidence, float* ins_uncertainty, float* vox_uncertainty,
+                                    float* all_mask_probs, int32_t* err_flag, pasco_stream_t s) {
+  PASCO_CHECK_ARG(X > 0 && Y > 0 && Z > 0, "pasco_panoptic_dense: empty grid");
+  PASCO_CHECK_ARG(kq >= 0 && kq <= Q && (kq == 0 || (kept && all_mask_probs)),
+                  "pasco_panoptic_dense: 0 <= kq <= Q kept queries with their list and volume");
+  PASCO_CHECK_ARG(err_flag != nullptr, "pasco_panoptic_dense: the error flag is required");
+  if (n == 0) return 0;
+  PanopticDenseParams p = {};
+  p.coords = coords;
+  p.n = n;
+  for (int d = 0; d < 3; ++d) p.min_c[d] = min_c[d];
+  p.X = X;
+  p.Y = Y;
+  p.Z = Z;
+  p.pan_row = panoptic_rows;
+  p.sem_row = semantic_rows;
+  p.conf_row = confidence_rows;
+  p.win = win;
+  p.m_win = m_win;
+  p.c_sum = c_sum;
+  p.qp = query_probs;
+  p.K1 = K1;
+  p.probs = probs;
+  p.Q = Q;
+  p.kept = kept;
+  p.kq = kq;
+  p.pan = panoptic;
+  p.sem = semantic;
+  p.conf = confidence;
+  p.ins = ins_uncertainty;
+  p.vox = vox_uncertainty;
+  p.all = all_mask_probs;
+  p.err = err_flag;
+  k_panoptic_dense<<<grid_for(n, 256), 256, 0, (cudaStream_t)s>>>(p);
+  PASCO_CHECK_LAUNCH("pasco_panoptic_dense");
+  return 0;
+}
+
+extern "C" int pasco_sem_dense(int32_t M, const float* const probs[], const int32_t* const cell_rows[], int64_t cells,
+                               int32_t K, float* const subnet_out[], float* ensemble_out, uint8_t* gate,
+                               pasco_stream_t s) {
+  PASCO_CHECK_ARG(M >= 1 && M <= kMaxSubnets, "pasco_sem_dense: 1 <= M <= %d subnets (got %d)", kMaxSubnets, M);
+  PASCO_CHECK_ARG(K >= 1, "pasco_sem_dense: K >= 1 classes");
+  if (cells == 0) return 0;
+  SemParams p = {};
+  SemDenseOut o = {};
+  p.M = M;
+  for (int m = 0; m < M; ++m) {
+    p.prob[m] = probs[m];
+    p.cell_row[m] = cell_rows[m];
+    o.sub[m] = subnet_out ? subnet_out[m] : nullptr;
+  }
+  o.ens = ensemble_out;
+  o.gate = gate;
+  k_sem_dense<<<grid_for(cells, 256), 256, 0, (cudaStream_t)s>>>(p, o, cells, K);
+  PASCO_CHECK_LAUNCH("pasco_sem_dense");
+  return 0;
+}
+
+extern "C" int pasco_class_gate(const float* dense, int64_t cells, int32_t K, uint8_t* gate, pasco_stream_t s) {
+  PASCO_CHECK_ARG(K >= 1, "pasco_class_gate: K >= 1 classes");
+  if (cells == 0) return 0;
+  k_class_gate<<<grid_for(cells, 256), 256, 0, (cudaStream_t)s>>>(dense, cells, K, gate);
+  PASCO_CHECK_LAUNCH("pasco_class_gate");
   return 0;
 }

@@ -1,4 +1,5 @@
-"""Opt-in hooks that route the UNMODIFIED reference's mask-transformer hot spots onto the sm_90a attention kernels.
+"""Opt-in hooks that route the UNMODIFIED reference's mask-transformer hot spots onto the sm_90a attention kernels, and
+(install(postprocess=True)) its test-time post-processing onto the panoptic kernels.
 
 The MinkowskiEngine surface (`pasco_b200.me`) already carries every sparse-tensor op of the reference.  Two pieces of
 PaSCo's transformer are plain torch in the reference and therefore outside that surface:
@@ -15,17 +16,28 @@ bit-packed mask rows, no [Q, P] score volume in HBM) and the mask as a sparse ma
 parameters, same state_dict, same results within the fp32 tolerance (tests/test_dropin_reference.py runs the reference
 with and without the hooks).
 
+The post-processing hooks replace `Ensembler.ensemble_sem_compl` / `ensemble_panop` (ensembler.py:20-187: dense
+[Q, 256, 256, 32] mask volumes, a dense soft IoU, ME.to_sparse of every volume) and `panoptic_inference` (helper.py:91-303:
+a Python loop over the kept queries with .item() syncs) — the latter where it is used, in both Net modules, which import
+it by name.  They return the reference's structures, computed on the sparse rows of predict.py's stages and the dense
+emits of csrc/panoptic.cu; inputs outside what the kernels cover (CPU tensors, batch size != 1, more than 8 subnets or 64
+classes, rows outside the requested box) go to the saved originals (`_pasco_b200_orig_*`).
+
     import pasco_b200.hooks; pasco_b200.hooks.install()        # after `pasco` is importable, before building Net
+    pasco_b200.hooks.install(postprocess=True)                 # the attention and the post-processing
     PASCO_B200_HOOKS=1 python scripts/train.py ...              # compat/MinkowskiEngine calls install() lazily
+    PASCO_B200_HOOKS=attention,postprocess python scripts/eval.py ...
 """
 from __future__ import annotations
 
+import importlib
+import time
+
 import torch
+import torch.nn.functional as F
 
 from . import me as ME
-from . import ops
-
-_installed = False
+from . import ops, predict
 
 
 def _cross_attention_forward(self, q_embed, bb_feat, attn_mask=None, padding_mask=None, pos=None, query_pos=None):
@@ -70,11 +82,120 @@ def _compute_attn_mask(self, outputs_mask, voxel_coord, src, src_C, src_scale, m
     return m.unsqueeze(1).repeat(1, self.nheads, 1, 1).flatten(0, 1)
 
 
-def install() -> bool:
-    """Patch the reference classes (idempotent).  Returns False when `pasco` is not importable."""
-    global _installed
-    if _installed:
-        return True
+# ------------------------------------------------------------------------------------------------
+# post-processing: Ensembler.ensemble_sem_compl / ensemble_panop (ensembler.py:20-187) and panoptic_inference
+# (helper.py:91-303) on the row-form kernels of csrc/panoptic.cu (predict.py's stages)
+# ------------------------------------------------------------------------------------------------
+_PANOPTIC_USERS = ("pasco.models.helper", "pasco.models.net_panoptic_sparse", "pasco.models.net_panoptic_sparse_kitti360")
+_orig_panoptic_inference = None
+
+
+def _rows_at(lin: torch.Tensor, size=predict.SCENE) -> torch.Tensor:
+    """Ascending cells → int32 [n, 4] (0, x, y, z) rows, ME.to_sparse's coordinates."""
+    lin = lin.long()
+    Y, Z = int(size[1]), int(size[2])
+    return torch.stack([torch.zeros_like(lin), lin // (Y * Z), (lin // Z) % Y, lin % Z], 1).to(torch.int32).contiguous()
+
+
+def _ensemble_sem_compl(self, sem_logits_at_scales, Ts):
+    """ensembler.py:159-187: the M + 1 dense class distributions [K, 256, 256, 32] from the softmax rows of every subnet.
+    The ensemble's occupancy gate is kept on the instance for the ensemble_panop call that follows."""
+    sems = sem_logits_at_scales[1]
+    self._pasco_b200_sem_state = None
+    if len(sems) > 8 or sems[0].F.shape[1] > 64 or not all(s.F.is_cuda for s in sems):
+        return self._pasco_b200_orig_ensemble_sem_compl(sem_logits_at_scales, Ts)
+    rows = predict.semantic_rows([(s.F, s.C) for s in sems], Ts)
+    cells = predict.SCENE[0] * predict.SCENE[1] * predict.SCENE[2]
+    gate = torch.empty(cells, dtype=torch.uint8, device=rows[0][0].device)
+    subs, ens = ops.sem_dense([p for p, _, _ in rows], [c for _, _, c in rows], cells, gate=gate)
+    out = [v.view(-1, *predict.SCENE) for v in subs + [ens]]
+    self._pasco_b200_sem_state = (out[-1], gate)
+    return out
+
+
+def _ensemble_panop(self, panop_predictions, ensemble_sem_prob_denses, scene_size, Ts, iou_threshold=0.2,
+                    measure_time=False):
+    """ensembler.py:20-131 on rows: {"sem_probs", "voxel_probs", "query_probs"} per subnet and for the ensemble, the
+    voxel probabilities on a fresh coordinate manager in ME.to_sparse order (ascending cell of the 256 x 256 x 32 grid,
+    all-zero rows dropped).  measure_time: "ensemble_time" covers the matching and the merge, as the reference times it
+    (ensembler.py:69-113), not the per-subnet warps before it."""
+    ql = panop_predictions[0]["query_logits"]
+    ens_vol = ensemble_sem_prob_denses[-1]
+    if (len(panop_predictions) > 8 or ql.shape[0] != 1 or not ql.is_cuda or not ens_vol.is_cuda
+            or ens_vol.shape[0] > 64 or tuple(ens_vol.shape[1:]) != predict.SCENE
+            or not all(p["voxel_logits"].F.is_cuda for p in panop_predictions)):
+        return self._pasco_b200_orig_ensemble_panop(panop_predictions, ensemble_sem_prob_denses, scene_size, Ts,
+                                                    iou_threshold=iou_threshold, measure_time=measure_time)
+    state = getattr(self, "_pasco_b200_sem_state", None)
+    self._pasco_b200_sem_state = None                 # used once: do not keep the volume alive past this scene
+    gate = state[1] if state is not None and state[0] is ens_vol else ops.class_gate(ens_vol)
+    preds = [{"voxel_logits": (p["voxel_logits"].F, p["voxel_logits"].C), "query_logits": p["query_logits"]}
+             for p in panop_predictions]
+    masks, qprobs = predict.mask_warps(preds, Ts)
+    if measure_time:
+        torch.cuda.synchronize()
+        t0 = time.time()
+    rows, qprobs = predict.mask_rows(masks, qprobs, gate, iou_threshold=iou_threshold)
+    if measure_time:
+        torch.cuda.synchronize()
+        ensemble_time = time.time() - t0
+    out = []
+    for (prob, lin), qp, sem_dense in zip(rows, qprobs, ensemble_sem_prob_denses):
+        coords = _rows_at(lin)
+        sem = ops.from_dense_raw(sem_dense.detach().float().unsqueeze(0).contiguous(), coords, (0, 0, 0), (1, 1, 1))
+        entry = {"sem_probs": ME.SparseTensor(sem, coords), "voxel_probs": ME.SparseTensor(prob, coords),
+                 "query_probs": qp}
+        if measure_time:
+            entry["ensemble_time"] = ensemble_time
+        out.append(entry)
+    return out
+
+
+def _squeezed(t: torch.Tensor) -> torch.Tensor:
+    """helper.py:264-281: to_dense_tensor's [C, X, Y, Z] volume with C = 1 for the per-voxel outputs, then .squeeze()."""
+    return t.unsqueeze(0).squeeze()
+
+
+def _panoptic_inference(voxel_output, query_output, overlap_threshold, object_mask_threshold, thing_ids, min_C,
+                        scene_size, input_query_logit=True, input_voxel_logit=False, vox_occ_threshold=0.3):
+    """helper.py:91-303 for batch size 1 on pasco_panoptic_pass1 / segments / pass2 / dense: the reference's dict with its
+    shapes and dtypes.  Two host synchronisations (the segment records, the box check), plus one for each of min_C and
+    scene_size given as device tensors (Net.step's call) — whatever the query count."""
+    args = (voxel_output, query_output, overlap_threshold, object_mask_threshold, thing_ids, min_C, scene_size,
+            input_query_logit, input_voxel_logit, vox_occ_threshold)
+    F_ = voxel_output.F
+    Q, K1 = query_output.shape[1], query_output.shape[-1]
+    if (query_output.shape[0] != 1 or not (F_.is_cuda and query_output.is_cuda) or not 2 <= K1 <= 65
+            or not 1 <= Q <= 8192 or F_.shape[1] != Q):
+        return _orig_panoptic_inference(*args)
+    voxel_probs = ME.MinkowskiSigmoid()(voxel_output) if input_voxel_logit else voxel_output
+    qp = F.softmax(query_output[0], dim=-1) if input_query_logit else query_output[0]
+    coords = voxel_probs.C.to(torch.int32).contiguous()
+    min_c = [int(v) for v in torch.as_tensor(min_C).reshape(-1).tolist()]
+    size = [int(v) for v in (scene_size.tolist() if torch.is_tensor(scene_size) else scene_size)]
+    pan_rows, records, vol = ops.panoptic_dense(voxel_probs.F.detach().float(), coords, qp, overlap_threshold,
+                                                object_mask_threshold, thing_ids, min_c, size, vox_occ_threshold)
+    if vol is None:                                    # a row outside the box: the reference's own indexing decides
+        return _orig_panoptic_inference(*args)
+    return {
+        "vox_all_mask_probs_denses": [vol["all_mask_probs"].squeeze()],
+        "panoptic_seg_denses": _squeezed(vol["panoptic"]).unsqueeze(0),
+        "semantic_seg_denses": _squeezed(vol["semantic"]).unsqueeze(0),
+        "ins_uncertainty_denses": _squeezed(vol["ins_uncertainty"]).unsqueeze(0),
+        "vox_confidence_denses": _squeezed(vol["confidence"]).unsqueeze(0),
+        "vox_uncertainty_denses": _squeezed(vol["vox_uncertainty"]).unsqueeze(0),
+        "panoptic_seg_sparses": [pan_rows],
+        "segments_infos": [predict._segments(records, qp)],
+    }
+
+
+# ------------------------------------------------------------------------------------------------
+# install / uninstall
+# ------------------------------------------------------------------------------------------------
+_installed = set()     # "attention", "postprocess"
+
+
+def _install_attention() -> bool:
     try:
         from pasco.models.transformer import blocks
         from pasco.models.transformer.transformer_predictor_v2 import TransformerPredictorV2
@@ -84,16 +205,62 @@ def install() -> bool:
     blocks.CrossAttentionLayer.forward = _cross_attention_forward
     TransformerPredictorV2._pasco_b200_orig_compute_attn_mask = TransformerPredictorV2.compute_attn_mask
     TransformerPredictorV2.compute_attn_mask = _compute_attn_mask
-    _installed = True
+    return True
+
+
+def _users():
+    """The modules that hold the name panoptic_inference (the Net modules import it by name); kitti360 when importable."""
+    mods = []
+    for name in _PANOPTIC_USERS:
+        try:
+            mods.append(importlib.import_module(name))
+        except Exception:
+            if name != _PANOPTIC_USERS[-1]:
+                raise
+    return mods
+
+
+def _install_postprocess() -> bool:
+    global _orig_panoptic_inference
+    try:
+        from pasco.models.ensembler import Ensembler
+        users = _users()
+    except Exception:
+        return False
+    Ensembler._pasco_b200_orig_ensemble_sem_compl = Ensembler.ensemble_sem_compl
+    Ensembler.ensemble_sem_compl = _ensemble_sem_compl
+    Ensembler._pasco_b200_orig_ensemble_panop = Ensembler.ensemble_panop
+    Ensembler.ensemble_panop = _ensemble_panop
+    _orig_panoptic_inference = users[0].panoptic_inference
+    for mod in users:
+        mod._pasco_b200_orig_panoptic_inference = _orig_panoptic_inference
+        mod.panoptic_inference = _panoptic_inference
+    return True
+
+
+def install(attention: bool = True, postprocess: bool = False) -> bool:
+    """Patch the reference (idempotent per group).  attention: the cross-attention and its mask; postprocess: the
+    Ensembler and panoptic_inference.  Returns False when a requested group's `pasco` modules are not importable."""
+    for name, wanted, fn in (("attention", attention, _install_attention),
+                             ("postprocess", postprocess, _install_postprocess)):
+        if wanted and name not in _installed:
+            if not fn():
+                return False
+            _installed.add(name)
     return True
 
 
 def uninstall() -> None:
-    global _installed
-    if not _installed:
-        return
-    from pasco.models.transformer import blocks
-    from pasco.models.transformer.transformer_predictor_v2 import TransformerPredictorV2
-    blocks.CrossAttentionLayer.forward = blocks.CrossAttentionLayer._pasco_b200_orig_forward
-    TransformerPredictorV2.compute_attn_mask = TransformerPredictorV2._pasco_b200_orig_compute_attn_mask
-    _installed = False
+    """Restore every attribute install() patched."""
+    if "attention" in _installed:
+        from pasco.models.transformer import blocks
+        from pasco.models.transformer.transformer_predictor_v2 import TransformerPredictorV2
+        blocks.CrossAttentionLayer.forward = blocks.CrossAttentionLayer._pasco_b200_orig_forward
+        TransformerPredictorV2.compute_attn_mask = TransformerPredictorV2._pasco_b200_orig_compute_attn_mask
+    if "postprocess" in _installed:
+        from pasco.models.ensembler import Ensembler
+        Ensembler.ensemble_sem_compl = Ensembler._pasco_b200_orig_ensemble_sem_compl
+        Ensembler.ensemble_panop = Ensembler._pasco_b200_orig_ensemble_panop
+        for mod in _users():
+            mod.panoptic_inference = mod._pasco_b200_orig_panoptic_inference
+    _installed.clear()

@@ -235,17 +235,33 @@ class TensorField:
     """Referenced only in isinstance checks (pasco/models/dropout.py:23,47)."""
 
 
-_HOOKS_PENDING = os.environ.get("PASCO_B200_HOOKS", "0") == "1"
+def _hook_groups(value: str) -> frozenset:
+    """PASCO_B200_HOOKS: "0" / unset = none, "1" = the attention hooks, else a comma list of "attention", "postprocess"."""
+    if value in ("", "0"):
+        return frozenset()
+    if value == "1":
+        return frozenset({"attention"})
+    groups = frozenset(v.strip() for v in value.split(",") if v.strip())
+    if not groups <= {"attention", "postprocess"}:
+        raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of attention, postprocess")
+    return groups
+
+
+_HOOK_GROUPS = _hook_groups(os.environ.get("PASCO_B200_HOOKS", "0"))
+_HOOKS_PENDING = bool(_HOOK_GROUPS)
+_HOOK_MODULES = {"attention": ("pasco.models.transformer.transformer_predictor_v2",),
+                 "postprocess": ("pasco.models.ensembler", "pasco.models.helper")}     # either Net module imports both
 
 
 def _maybe_install_hooks() -> None:
-    """PASCO_B200_HOOKS=1: once the reference's transformer module has been imported, route its cross-attention and
-    attention-mask construction onto the engine (pasco_b200/hooks.py).  Checked when a SparseTensor is built."""
+    """PASCO_B200_HOOKS: once the reference modules of the requested hook groups have been imported, route the
+    cross-attention and attention-mask construction ("attention") and the Ensembler and panoptic_inference
+    ("postprocess") onto the engine (pasco_b200/hooks.py).  Checked when a SparseTensor is built."""
     global _HOOKS_PENDING
-    if _HOOKS_PENDING and "pasco.models.transformer.transformer_predictor_v2" in sys.modules:
+    if _HOOKS_PENDING and all(m in sys.modules for g in _HOOK_GROUPS for m in _HOOK_MODULES[g]):
         _HOOKS_PENDING = False
         from .. import hooks
-        hooks.install()
+        hooks.install(attention="attention" in _HOOK_GROUPS, postprocess="postprocess" in _HOOK_GROUPS)
 
 
 class _LazyRows:

@@ -1094,35 +1094,98 @@ def sem_ensemble(probs: List[torch.Tensor], cell_rows: List[torch.Tensor], lin: 
     return pred, conf
 
 
-def panoptic(probs: torch.Tensor, query_probs: torch.Tensor, overlap_threshold: float, object_mask_threshold: float,
-             thing_ids: Sequence[int], vox_occ_threshold: float = 0.3):
-    """helper.py:135-263 for one prediction: probs fp32 [N, Q] mask probabilities, query_probs fp32 [Q, K1].
-    Returns (panoptic int32 [N], semantic int32 [N], confidence fp32 [N], records int32 [1 + 4Q] on the host)."""
+def _panoptic_passes(probs, qp, overlap_threshold, object_mask_threshold, thing_ids, vox_occ_threshold, dense: bool):
+    """Passes 1, segments and 2 → (panoptic, semantic, confidence rows, device int32 [1 + 4Q (+ 1 + Q)] = the records
+    (then the kept-query count and list when dense), win, m_win, c_sum or None)."""
     n, q = probs.shape
-    K1 = query_probs.shape[1]
+    K1 = qp.shape[1]
     dev = probs.device
-    qp = query_probs.detach().float().contiguous()
     win = torch.empty(n, dtype=torch.int32, device=dev)
     m_win = torch.empty(n, dtype=torch.float32, device=dev)
     m_sum = torch.empty(n, dtype=torch.float32, device=dev)
+    c_sum = torch.empty(n, dtype=torch.float32, device=dev) if dense else None
     areas = torch.zeros(2 * max(q, 1), dtype=torch.int32, device=dev)
     seg_of = torch.empty(max(q, 1), dtype=torch.int32, device=dev)
     cls_of = torch.empty(max(q, 1), dtype=torch.int32, device=dev)
-    records = torch.zeros(1 + 4 * q, dtype=torch.int32, device=dev)
+    out = torch.zeros(1 + 4 * q + (1 + q if dense else 0), dtype=torch.int32, device=dev)
     pan = torch.empty(n, dtype=torch.int32, device=dev)
     sem = torch.empty(n, dtype=torch.int32, device=dev)
     conf = torch.empty(n, dtype=torch.float32, device=dev)
     if q == 0:
-        return pan.zero_(), sem.zero_(), conf.zero_(), records.cpu()
+        return pan.zero_(), sem.zero_(), conf.zero_(), out, win, m_win, c_sum
     mask = 0
     for c in thing_ids:
         mask |= 1 << int(c)
     call("pasco_panoptic_pass1", ptr(probs.contiguous()), n, q, ptr(qp), K1, float(object_mask_threshold),
-         float(vox_occ_threshold), ptr(win), ptr(m_win), ptr(m_sum), ptr(areas))
+         float(vox_occ_threshold), ptr(win), ptr(m_win), ptr(m_sum), ptr(c_sum), ptr(areas))
     call("pasco_panoptic_segments", ptr(qp), q, K1, float(object_mask_threshold), float(overlap_threshold), mask,
-         ptr(areas), ptr(seg_of), ptr(cls_of), ptr(records))
+         ptr(areas), ptr(seg_of), ptr(cls_of), ptr(out[:1 + 4 * q]), ptr(out[1 + 4 * q:]) if dense else None)
     call("pasco_panoptic_pass2", ptr(win), ptr(m_win), ptr(m_sum), n, ptr(seg_of), ptr(cls_of), ptr(pan), ptr(sem), ptr(conf))
+    return pan, sem, conf, out, win, m_win, c_sum
+
+
+def panoptic(probs: torch.Tensor, query_probs: torch.Tensor, overlap_threshold: float, object_mask_threshold: float,
+             thing_ids: Sequence[int], vox_occ_threshold: float = 0.3):
+    """helper.py:135-263 for one prediction: probs fp32 [N, Q] mask probabilities, query_probs fp32 [Q, K1].
+    Returns (panoptic int32 [N], semantic int32 [N], confidence fp32 [N], records int32 [1 + 4Q] on the host)."""
+    qp = query_probs.detach().float().contiguous()
+    pan, sem, conf, records = _panoptic_passes(probs, qp, overlap_threshold, object_mask_threshold, thing_ids,
+                                               vox_occ_threshold, False)[:4]
     return pan, sem, conf, records.cpu()
+
+
+def panoptic_dense(probs: torch.Tensor, coords: torch.Tensor, query_probs: torch.Tensor, overlap_threshold: float,
+                   object_mask_threshold: float, thing_ids: Sequence[int], min_c: Sequence[int], size: Sequence[int],
+                   vox_occ_threshold: float = 0.3):
+    """helper.py:135-281 for one prediction whose rows sit at coords int32 [N, 4] (batch 0): the passes of `panoptic`,
+    then every dense volume panoptic_inference returns, channel-first over the box of `size` cells from min_c.
+    Returns (panoptic rows int32 [N], records int32 [1 + 4Q] on the host, {"panoptic", "semantic" int32 [X, Y, Z],
+    "confidence", "ins_uncertainty", "vox_uncertainty" fp32 [X, Y, Z], "all_mask_probs" fp32 [kq, X, Y, Z]}), or None
+    when a row lies outside the box or in another batch (checked on a flag of its own, so a pending error of another
+    pass is left to raise_pending_errors).  Two host synchronisations: the records, then the box check."""
+    n, q = probs.shape
+    dev = probs.device
+    qp = query_probs.detach().float().contiguous()
+    probs = probs.contiguous()
+    pan, sem, conf, out, win, m_win, c_sum = _panoptic_passes(probs, qp, overlap_threshold, object_mask_threshold,
+                                                              thing_ids, vox_occ_threshold, True)
+    host = out.cpu()
+    kq = int(host[1 + 4 * q])
+    X, Y, Z = (int(s) for s in size)
+    vol = {k: torch.zeros(X, Y, Z, dtype=dt, device=dev) for k, dt in
+           (("panoptic", torch.int32), ("semantic", torch.int32), ("confidence", torch.float32),
+            ("ins_uncertainty", torch.float32), ("vox_uncertainty", torch.float32))}
+    vol["all_mask_probs"] = torch.zeros(kq, X, Y, Z, dtype=torch.float32, device=dev)
+    flag = torch.zeros(1, dtype=torch.int32, device=dev)
+    call("pasco_panoptic_dense", ptr(coords), n, int_array(min_c), X, Y, Z, ptr(pan), ptr(sem), ptr(conf), ptr(win),
+         ptr(m_win), ptr(c_sum), ptr(qp), qp.shape[1], ptr(probs), q, ptr(out[2 + 4 * q:2 + 4 * q + kq]), kq,
+         ptr(vol["panoptic"]), ptr(vol["semantic"]), ptr(vol["confidence"]), ptr(vol["ins_uncertainty"]),
+         ptr(vol["vox_uncertainty"]), ptr(vol["all_mask_probs"]) if kq else None, ptr(flag))
+    if n and int(flag.item()):
+        return pan, host[:1 + 4 * q], None
+    return pan, host[:1 + 4 * q], vol
+
+
+def sem_dense(probs: List[torch.Tensor], cell_rows: List[torch.Tensor], cells: int, subnets: bool = True,
+              gate: Optional[torch.Tensor] = None) -> Tuple[Optional[List[torch.Tensor]], torch.Tensor]:
+    """The dense class distributions fp32 [K, cells] of every subnet (when `subnets`; one-hot class 0 where a subnet has no
+    row) and of their mean, as sem_ensemble computes it; gate (uint8 [cells]) receives the mean's argmax != 0."""
+    M, K = len(probs), probs[0].shape[1]
+    dev = probs[0].device
+    subs = [torch.empty(K, cells, dtype=torch.float32, device=dev) for _ in range(M)] if subnets else None
+    ens = torch.empty(K, cells, dtype=torch.float32, device=dev)
+    call("pasco_sem_dense", M, (C.c_void_p * M)(*[ptr(p) for p in probs]), (C.c_void_p * M)(*[ptr(c) for c in cell_rows]),
+         cells, K, (C.c_void_p * M)(*[ptr(s) for s in subs]) if subnets else None, ptr(ens), ptr(gate))
+    return subs, ens
+
+
+def class_gate(dense: torch.Tensor) -> torch.Tensor:
+    """dense fp32 [K, X, Y, Z] → uint8 [X·Y·Z]: first argmax over the channels != 0."""
+    d = dense.detach().float().contiguous()
+    cells = d[0].numel()
+    gate = torch.empty(cells, dtype=torch.uint8, device=d.device)
+    call("pasco_class_gate", ptr(d), cells, d.shape[0], ptr(gate))
+    return gate
 
 
 # ----------------------------------------------------------------------------------------------

@@ -72,26 +72,39 @@ def postprocess(preds: Sequence[Dict], sems: Sequence, Ts: Sequence[torch.Tensor
     keep_sem_rows: every entry also holds "sem_rows", the (softmax rows [n, K], cell map int32 [cells]) pairs its
     semantic output averaged — the subnet's own pair, all M for the ensemble — so that p[c] of the class distribution
     can be evaluated at any cell (metrics.Evaluator's NLL)."""
-    from scipy.optimize import linear_sum_assignment
     M = len(preds)
     if not 1 <= M <= 8:
         raise ValueError(f"predict: 1 to 8 subnets (the semantic ensemble kernel's limit), got {M}")
-    dev = preds[0]["voxel_logits"][0].device
+    sem_rows = semantic_rows(sems, Ts, size)
+    ssc, gate = semantic(sem_rows, size)
+    rows, qprobs = mask_rows(*mask_warps(preds, Ts, size), gate, iou_threshold=iou_threshold, size=size, matches=matches)
+    entries = []
+    for (prob, lin), qp, (s_lin, s_pred, s_conf) in zip(rows, qprobs, ssc):
+        pan, sem, conf, records = ops.panoptic(prob, qp[0], overlap_threshold, object_mask_threshold, thing_ids)
+        entries.append({"lin": lin.long(), "panoptic_seg": pan, "semantic_seg": sem, "vox_confidence": conf,
+                        "segments_info": _segments(records, qp[0]), "ssc_lin": s_lin.long(), "ssc_pred": s_pred,
+                        "ssc_confidence": s_conf, "query_probs": qp[0]})
+    if keep_sem_rows:
+        for m, e in enumerate(entries):
+            e["sem_rows"] = [(p, cell) for p, _, cell in (sem_rows[m:m + 1] if m < M else sem_rows)]
+    return entries
+
+
+def semantic_rows(sems: Sequence, Ts: Sequence[torch.Tensor], size=SCENE) -> List[tuple]:
+    """The semantic logits of every subnet warped to the reference grid: [(softmax rows fp32 [n, K], lin int32 [n]
+    ascending cells, cell map int32 [cells])]."""
+    out = []
+    for (s_logits, s_coords), T in zip(sems, Ts):
+        s_lin, s_cell, s_src = warp(s_coords, T, size)
+        out.append((ops.softmax_rows(s_logits, s_src), s_lin, s_cell))
+    return out
+
+
+def semantic(sem_rows: Sequence[tuple], size=SCENE):
+    """Semantic completion (ensembler.py:160-187): every subnet on its own rows, the ensemble on the union of the rows →
+    ([(lin, argmax int32, max fp32)] for the M subnets and the ensemble, the ensemble's occupancy gate uint8 [cells])."""
     cells = int(size[0]) * int(size[1]) * int(size[2])
-    Q = preds[0]["voxel_logits"][0].shape[1]
-
-    masks, qprobs, sem_rows = [], [], []
-    for m in range(M):
-        logits, coords = preds[m]["voxel_logits"]
-        lin, cell_row, src = warp(coords, Ts[m], size)
-        prob, planes, colsum, nz = ops.mask_rows_sigmoid(logits, src, planes=M > 1)
-        masks.append(dict(prob=prob, lin=lin, cell=cell_row, planes=planes, colsum=colsum, nz=nz))
-        qprobs.append(F.softmax(preds[m]["query_logits"].detach().float(), -1))
-        s_logits, s_coords = sems[m]
-        s_lin, s_cell, s_src = warp(s_coords, Ts[m], size)
-        sem_rows.append((ops.softmax_rows(s_logits, s_src), s_lin, s_cell))
-
-    # semantic completion: every subnet on its own rows, the ensemble on the union of the rows (ensembler.py:160-187)
+    dev = sem_rows[0][0].device
     ssc = [(lin,) + ops.sem_ensemble([p], [cell], lin) for p, lin, cell in sem_rows]
     union = torch.zeros(cells, dtype=torch.uint8, device=dev)
     for _, _, cell in sem_rows:
@@ -99,8 +112,37 @@ def postprocess(preds: Sequence[Dict], sems: Sequence, Ts: Sequence[torch.Tensor
     u_lin, _, _ = ops.compact(union)
     gate = torch.zeros(cells, dtype=torch.uint8, device=dev)
     ssc.append((u_lin,) + ops.sem_ensemble([p for p, _, _ in sem_rows], [c for _, _, c in sem_rows], u_lin, gate))
+    return ssc, gate
 
-    # masks: running average of the matched queries on the union rows (ensembler.py:20-129)
+
+def mask_warps(preds: Sequence[Dict], Ts: Sequence[torch.Tensor], size=SCENE):
+    """The sigmoid rows of every subnet on the reference grid (ensembler.py:36-64) → (per subnet: dict of the
+    probabilities, cells, cell map, bf16 planes and column sums when M > 1, non-zero row flags; the M query class
+    probabilities [1, Q, K1])."""
+    M = len(preds)
+    masks, qprobs = [], []
+    for m in range(M):
+        logits, coords = preds[m]["voxel_logits"]
+        lin, cell_row, src = warp(coords, Ts[m], size)
+        prob, planes, colsum, nz = ops.mask_rows_sigmoid(logits, src, planes=M > 1)
+        masks.append(dict(prob=prob, lin=lin, cell=cell_row, planes=planes, colsum=colsum, nz=nz))
+        qprobs.append(F.softmax(preds[m]["query_logits"].detach().float(), -1))
+    return masks, qprobs
+
+
+def mask_rows(masks: Sequence[Dict], qprobs: Sequence[torch.Tensor], gate: torch.Tensor, *, iou_threshold: float = 0.2,
+              size=SCENE, matches: Optional[list] = None):
+    """The mask ensemble (ensembler.py:66-113) on mask_warps' rows: the running average of the matched queries on the
+    union rows, with the mean-IoU keep and the occupancy gate.  Returns M + 1 (probabilities fp32 [n, q], lin int32 [n]
+    ascending cells) with all-zero rows dropped (ME.to_sparse), and the M + 1 query class probabilities [1, q, K1]."""
+    from scipy.optimize import linear_sum_assignment
+    M = len(masks)
+    dev = masks[0]["prob"].device
+    cells = int(size[0]) * int(size[1]) * int(size[2])
+    Q = masks[0]["prob"].shape[1]
+    qprobs = list(qprobs)
+
+    # running average of the matched queries on the union rows
     a = masks[0]
     a_q = qprobs[0].clone()
     ious = []
@@ -140,18 +182,8 @@ def postprocess(preds: Sequence[Dict], sems: Sequence, Ts: Sequence[torch.Tensor
                                             gate, planes=False)
             ens_prob, ens_lin = _drop_zero_rows(prob, lin, nz)
         a_q = a_q[:, torch.as_tensor(keep, device=dev)]
-
-    entries = []
     rows = [_drop_zero_rows(mk["prob"], mk["lin"], mk["nz"]) for mk in masks] + [(ens_prob, ens_lin)]
-    for (prob, lin), qp, (s_lin, s_pred, s_conf) in zip(rows, qprobs + [a_q], ssc):
-        pan, sem, conf, records = ops.panoptic(prob, qp[0], overlap_threshold, object_mask_threshold, thing_ids)
-        entries.append({"lin": lin.long(), "panoptic_seg": pan, "semantic_seg": sem, "vox_confidence": conf,
-                        "segments_info": _segments(records, qp[0]), "ssc_lin": s_lin.long(), "ssc_pred": s_pred,
-                        "ssc_confidence": s_conf, "query_probs": qp[0]})
-    if keep_sem_rows:
-        for m, e in enumerate(entries):
-            e["sem_rows"] = [(p, cell) for p, _, cell in (sem_rows[m:m + 1] if m < M else sem_rows)]
-    return entries
+    return rows, qprobs + [a_q]
 
 
 _DENSE = {"panoptic_seg": ("lin", 0.0), "semantic_seg": ("lin", 0.0), "vox_confidence": ("lin", 0.0),
