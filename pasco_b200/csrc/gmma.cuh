@@ -164,6 +164,29 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint6
         "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB));
 }
+// D[64 x 256] += A[64 x 16] · B[16 x 256]: one A read for four 64-column blocks; d[32 q .. 32 q + 31] = columns 64 q ..
+// 64 q + 63
+#define GMMA_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define GMMA_F32(i) GMMA_F8(i), GMMA_F8(i + 8), GMMA_F8(i + 16), GMMA_F8(i + 24)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, %130, %131;\n\t}"
+      : GMMA_F32(0), GMMA_F32(32), GMMA_F32(64), GMMA_F32(96)
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB));
+}
+#undef GMMA_F32
+#undef GMMA_F8
 // D[64 x 16] += A[64 x 16] · B[16 x 16], both operands K-major
 __device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
