@@ -254,6 +254,17 @@ int pasco_xattn_forward(const float* q, const float* k, const float* v, const ui
 int pasco_xattn_backward(const float* q, const float* k, const float* v, const uint32_t* mask, const float* lse,
                          const float* out, const float* dout, int32_t Q, int64_t P, int32_t H, int32_t D, float scale,
                          float* dq, float* dk, float* dv, pasco_stream_t s);
+/* the attention mask of transformer_predictor_v2.py:220-289 and line 164, built directly as the bit rows above:
+ * key v of the P keys is masked for query q unless some scale-1 voxel u in v's stride-s block has logit[u, q] > 0.
+ * logits [*, Q] float32 with row pitch ld; voxel u reads logit row rows[u] (NULL: row u) for u < n_child;
+ * parent_of [n_child] = u's row among the n_parent stride-s voxels (NULL: identity, n_parent = n_child; −1 skipped);
+ * key_parent [P] = key v's row among those n_parent voxels (−1: no voxel, masked).
+ * Out: mask uint32 [Q, 2*ceil(P/64)]; keys beyond P masked; a query whose P keys are all masked gets those P bits
+ * cleared (it attends everywhere) and keeps its padding bits.  Scratch from the caller, zero-filled: pooled uint32
+ * [n_parent, ceil(Q/32)] and seen int32 [Q].  Integer atomicOr only: two calls give identical bits.               */
+int pasco_attn_mask_bits(const float* logits, int64_t ld, int32_t Q, const int32_t* rows, int64_t n_child,
+                         const int32_t* parent_of, int64_t n_parent, const int32_t* key_parent, int64_t P,
+                         uint32_t* pooled, int32_t* seen, uint32_t* mask, pasco_stream_t s);
 
 /* ---- test-time post-processing: the M-subnet ensemble (pasco/models/ensembler.py:20-187, reached from
  *      net_panoptic_sparse.py:245-294) and panoptic inference (pasco/models/helper.py:91-303, reached from

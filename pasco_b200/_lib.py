@@ -60,6 +60,7 @@ PROTOTYPES = {
     "pasco_bn_bwd_reduce": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i32, _p, _p]),
     "pasco_xattn_forward": (C.c_int, [_p, _p, _p, _p, _i32, _i64, _i32, _i32, C.c_float, _p, _p, _p]),
     "pasco_xattn_backward": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _i32, _i64, _i32, _i32, C.c_float, _p, _p, _p, _p]),
+    "pasco_attn_mask_bits": (C.c_int, [_p, _i64, _i32, _p, _i64, _p, _i64, _p, _i64, _p, _p, _p, _p]),
     "pasco_bn_bwd_apply": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i32, _p, _p, _p, _p, _p]),
     "pasco_pose_lookup": (C.c_int, [_p, _p, _i64, _p, _i32, _i32, _i32, _p, _p, _p]),
     "pasco_cell_mask_or": (C.c_int, [_p, _i64, _p, _p]),

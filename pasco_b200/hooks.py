@@ -9,12 +9,16 @@ PaSCo's transformer are plain torch in the reference and therefore outside that 
   * `TransformerPredictorV2.compute_attn_mask` (transformer/transformer_predictor_v2.py:220-289): a dense
     [1, 100, X/s, Y/s, Z/s] volume (839 MB at scale 1) built only to be sampled at the key voxels.
 
-`install()` replaces those two methods — at run time, on the imported classes, without touching the reference's files —
-with calls into the engine: the attention through ops.cross_attention, which net3d's own decoder uses too (K/V
-projections on the wgmma GEMM, the masked softmax·V as `pasco_xattn_forward/backward`: streaming two-pass softmax,
-bit-packed mask rows, no [Q, P] score volume in HBM) and the mask as a sparse max-pool + hash look-up.  Same
-parameters, same state_dict, same results within the fp32 tolerance (tests/test_dropin_reference.py runs the reference
-with and without the hooks).
+The reference's `TransformerPredictorV2.forward` (transformer_predictor_v2.py:111-218) then repeats that bool mask over
+the heads and sums it in int64 (line 164): 37.5 GiB at M = 3 and full scene size.  `install()` replaces that forward
+— at run time, on the imported class, without touching the reference's files — with one that calls the reference's own
+submodules but builds each level's mask on the device directly as the bit rows the attention kernels read
+(ops.attention_mask_bits: an OR-pool of the thresholded logits to the key scale, a hash look-up of the keys, Q·P/8
+bytes per item), and `CrossAttentionLayer.forward` with one that takes those bits into ops.cross_attention, which
+net3d's own decoder uses too (K/V projections on the wgmma GEMM, the masked softmax·V as
+`pasco_xattn_forward/backward`: streaming two-pass softmax, no [Q, P] score volume in HBM).  Same parameters, same
+state_dict, same results within the fp32 tolerance (tests/test_dropin_reference.py and tests/test_attn_mask_bits.py
+run the reference with and without the hooks).
 
 The post-processing hooks replace `Ensembler.ensemble_sem_compl` / `ensemble_panop` (ensembler.py:20-187: dense
 [Q, 256, 256, 32] mask volumes, a dense soft IoU, ME.to_sparse of every volume) and `panoptic_inference` (helper.py:91-303:
@@ -40,46 +44,82 @@ from . import me as ME
 from . import ops, predict
 
 
+def _transformer_forward(self, xs, sem_logits, min_Cs, max_Cs, keep_pad):
+    """transformer_predictor_v2.py:111-218 with the attention masks built on the device as bit rows
+    (ops.attention_mask_bits): the reference's own submodules, outputs and padding semantics — padded rows of a MIMO
+    batch take part in attention — without its [B·heads, Q, P] bool mask and the int64 row sum of line 164.
+    xs[scale] = (F [B, P_s, C], C [B, P_s, 4]) with B = n_infers."""
+    F1, C1 = xs[1]
+    if not F1.is_cuda:
+        return self._pasco_b200_orig_forward(xs, sem_logits, min_Cs, max_Cs, keep_pad)
+    bs = sem_logits[0].shape[0]
+    assert self.n_infers == bs, "batch size should be equal to number of inference"
+    output = self.query_feat.weight.reshape(bs, -1, self.hidden_dim)
+    query_embed = self.query_embed.weight.reshape(bs, -1, self.hidden_dim)
+    pos = [self.pe_layer(xs[s][1].reshape(-1, 4)[:, 1:]).reshape(bs, -1, self.hidden_dim) for s in self.src_scales]
+    voxel_feat = self.mask_feat_proj(F1) + pos[-1]
+    cls, msk = self.pred_heads(output, voxel_feat)
+    classes, masks = [cls], [msk]
+    voxels = [_voxel_map(c) for c in C1]
+    for i, s in enumerate(self.src_scales):
+        src_F, src_C = xs[s]
+        src_F = self.input_projs[i](src_F)
+        bits = torch.stack([_mask_bits(voxels[b], masks[-1][b], src_C[b], s) for b in range(bs)])
+        output = self.transformer_cross_attention_layers[i](output, src_F, attn_mask=bits, pos=pos[i],
+                                                            query_pos=query_embed)
+        output = self.transformer_self_attention_layers[i](output, attn_mask=None, padding_mask=None,
+                                                           query_pos=query_embed)
+        output = self.transformer_ffn_layers[i](output)
+        cls, msk = self.pred_heads(output, voxel_feat)
+        classes.append(cls)
+        masks.append(msk)
+    preds = []
+    for b in range(bs):
+        keep = keep_pad[b]
+        item_classes = [c[b].unsqueeze(0) for c in classes]
+        item_masks = [ME.SparseTensor(m[b][keep], C1[b][keep]) for m in masks]
+        preds.append({"query_logits": item_classes[-1], "voxel_logits": item_masks[-1],
+                      "aux_outputs": self.set_aux(item_classes, item_masks)})
+    return preds
+
+
+def _voxel_map(coords: torch.Tensor):
+    """One batch item's scale-1 voxels on a coordinate manager of their own: (manager, key, logit row of each unique
+    voxel or None).  Padded rows of a MIMO batch share voxel (0,0,0); the first row of a voxel stands for it."""
+    C1 = coords.to(torch.int32).clone()
+    C1[:, 0] = 0
+    mgr = ME.CoordinateManager()
+    key1, uidx = mgr.insert_and_map(C1.contiguous())
+    return mgr, key1, uidx
+
+
+def _mask_bits(voxels, logits: torch.Tensor, src_C: torch.Tensor, scale: int) -> torch.Tensor:
+    """transformer_predictor_v2.py:220-289 and 164 for one batch item: logits [P1, Q], src_C [P_s, 4] →
+    ops.attention_mask_bits' int32 bit rows [Q, 2*ceil(P_s/64)]."""
+    mgr, key1, uidx = voxels
+    parent_of, key_s = None, key1
+    if scale != 1:
+        key_s = mgr.stride(key1, scale)
+        parent_of = mgr.pool_map(key1, key_s, scale)
+    Cs = src_C.to(torch.int32).clone()
+    Cs[:, 0] = 0
+    return ops.attention_mask_bits(logits.detach(), ops.hash_lookup(mgr._table(key_s), Cs.contiguous()), uidx,
+                                   parent_of, mgr.size(key_s))
+
+
 def _cross_attention_forward(self, q_embed, bb_feat, attn_mask=None, padding_mask=None, pos=None, query_pos=None):
-    """blocks.py:73-92 with the attention itself on xattn.cu.  q_embed [B, Q, d]; bb_feat / pos [B, P, d]; attn_mask
-    bool [B*heads, Q, P] (True = masked; the reference repeats one [Q, P] mask over the heads)."""
-    if padding_mask is not None or not bb_feat.is_cuda:
+    """blocks.py:73-92 with the attention on xattn.cu, for the bit-row masks [B, Q, words] the hooked
+    TransformerPredictorV2.forward passes; any other mask (the reference's bool [B·heads, Q, P]) goes to the original.
+    q_embed [B, Q, d]; bb_feat / pos [B, P, d]."""
+    if attn_mask is None or attn_mask.dtype != torch.int32 or padding_mask is not None or not bb_feat.is_cuda:
         return self._pasco_b200_orig_forward(q_embed, bb_feat, attn_mask, padding_mask, pos, query_pos)
-    h = self.multihead_attn.num_heads
     q_embed = self.norm(q_embed)
     outs = []
     for b in range(q_embed.shape[0]):
         qb = q_embed[b] if query_pos is None else q_embed[b] + query_pos[b]
         kv = bb_feat[b] if pos is None else bb_feat[b] + pos[b]
-        m = attn_mask[b * h] if attn_mask is not None else None    # all heads of an item share one mask
-        outs.append(ops.cross_attention(self.multihead_attn, qb, kv, m))
+        outs.append(ops.cross_attention(self.multihead_attn, qb, kv, attn_mask[b]))
     return q_embed + self.dropout(torch.stack(outs, 0))
-
-
-def _compute_attn_mask(self, outputs_mask, voxel_coord, src, src_C, src_scale, min_Cs, max_Cs):
-    """transformer_predictor_v2.py:220-289 without the dense volume: mask[q, v] = not OR_{u in block_s(v)} (logit[u, q] > 0).
-    outputs_mask [B, P1, Q]; voxel_coord [B, P1, 4]; src_C [B, Ps, 4] → bool [B*heads, Q, Ps]."""
-    masks = []
-    for b in range(outputs_mask.shape[0]):
-        keep = (outputs_mask[b].detach() > 0).float().contiguous()               # sigmoid(x) > 0.5
-        C1 = voxel_coord[b].to(torch.int32).clone()
-        C1[:, 0] = 0
-        mgr = ME.CoordinateManager()
-        key1, uidx = mgr.insert_and_map(C1.contiguous())                          # padded rows share voxel (0,0,0)
-        if uidx is not None:
-            keep = ops._gather_rows(keep, uidx)
-        if src_scale == 1:
-            pooled, pooled_key = keep, key1
-        else:
-            pooled_key = mgr.stride(key1, src_scale)
-            pooled = ops.MaxPoolRows.apply(keep, mgr.pool_map(key1, pooled_key, src_scale), mgr.size(pooled_key))
-        Cs = src_C[b].to(torch.int32).clone()
-        Cs[:, 0] = 0
-        rows = ops.hash_lookup(mgr._table(pooled_key), Cs.contiguous())
-        at_keys = ops._gather_rows(pooled.contiguous(), rows)                     # [Ps, Q], zero where no child
-        masks.append((at_keys == 0).t())
-    m = torch.stack(masks, 0)                                                     # [B, Q, Ps]
-    return m.unsqueeze(1).repeat(1, self.nheads, 1, 1).flatten(0, 1)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -201,10 +241,10 @@ def _install_attention() -> bool:
         from pasco.models.transformer.transformer_predictor_v2 import TransformerPredictorV2
     except Exception:
         return False
+    TransformerPredictorV2._pasco_b200_orig_forward = TransformerPredictorV2.forward
+    TransformerPredictorV2.forward = _transformer_forward
     blocks.CrossAttentionLayer._pasco_b200_orig_forward = blocks.CrossAttentionLayer.forward
     blocks.CrossAttentionLayer.forward = _cross_attention_forward
-    TransformerPredictorV2._pasco_b200_orig_compute_attn_mask = TransformerPredictorV2.compute_attn_mask
-    TransformerPredictorV2.compute_attn_mask = _compute_attn_mask
     return True
 
 
@@ -239,7 +279,8 @@ def _install_postprocess() -> bool:
 
 
 def install(attention: bool = True, postprocess: bool = False) -> bool:
-    """Patch the reference (idempotent per group).  attention: the cross-attention and its mask; postprocess: the
+    """Patch the reference (idempotent per group).  attention: TransformerPredictorV2.forward with its masks as
+    bit rows, and the cross-attention layer that takes them; postprocess: the
     Ensembler and panoptic_inference.  Returns False when a requested group's `pasco` modules are not importable."""
     for name, wanted, fn in (("attention", attention, _install_attention),
                              ("postprocess", postprocess, _install_postprocess)):
@@ -255,8 +296,8 @@ def uninstall() -> None:
     if "attention" in _installed:
         from pasco.models.transformer import blocks
         from pasco.models.transformer.transformer_predictor_v2 import TransformerPredictorV2
+        TransformerPredictorV2.forward = TransformerPredictorV2._pasco_b200_orig_forward
         blocks.CrossAttentionLayer.forward = blocks.CrossAttentionLayer._pasco_b200_orig_forward
-        TransformerPredictorV2.compute_attn_mask = TransformerPredictorV2._pasco_b200_orig_compute_attn_mask
     if "postprocess" in _installed:
         from pasco.models.ensembler import Ensembler
         Ensembler.ensemble_sem_compl = Ensembler._pasco_b200_orig_ensemble_sem_compl

@@ -858,11 +858,34 @@ def pack_mask_bits(mask: torch.Tensor) -> torch.Tensor:
     return words.to(torch.int32).contiguous()
 
 
+def attention_mask_bits(logits: torch.Tensor, key_parent: torch.Tensor, rows: Optional[torch.Tensor] = None,
+                        parent_of: Optional[torch.Tensor] = None, n_parent: Optional[int] = None) -> torch.Tensor:
+    """The attention mask of transformer_predictor_v2.py:220-289 and 164 as pack_mask_bits' int32 [Q, 2*ceil(P/64)]
+    bit rows, without a [Q, P] intermediate: key v is masked for query q unless a scale-1 voxel u of v's stride-s block
+    has logits[rows[u], q] > 0; a query with every key masked attends to all P keys.
+    logits [*, Q] float32 with unit column stride (a column slice is fine); rows [n] int32 = the logit row of each
+    scale-1 voxel (None: voxel u is row u); parent_of [n] int32 = each voxel's row among the n_parent stride-s voxels
+    (None: s = 1); key_parent [P] int32 = each key's row among those (−1: no voxel, masked)."""
+    assert logits.dtype == torch.float32 and logits.is_cuda and logits.dim() == 2 and logits.stride(1) == 1
+    Q = logits.shape[1]
+    n_child = rows.shape[0] if rows is not None else logits.shape[0]
+    if parent_of is None:
+        n_parent = n_child
+    P = key_parent.shape[0]
+    dev = logits.device
+    pooled = torch.zeros(n_parent, (Q + 31) // 32, dtype=torch.int32, device=dev)
+    seen = torch.zeros(Q, dtype=torch.int32, device=dev)
+    bits = torch.empty(Q, 2 * ((P + 63) // 64), dtype=torch.int32, device=dev)
+    call("pasco_attn_mask_bits", logits.data_ptr(), logits.stride(0), Q, ptr(rows), n_child, ptr(parent_of), n_parent,
+         ptr(key_parent), P, ptr(pooled), ptr(seen), ptr(bits))
+    return bits
+
+
 class MaskedCrossAttention(torch.autograd.Function):
     """out[q] = concat_h softmax_v(scale·q_h·k_h[v] | mask[q,v]) · v_h[v]  — blocks.py:73-92 with the mask of
     transformer_predictor_v2.py:220-289.  q [Q, H*D] with any Q >= 1, k / v [P, H*D], D <= 64 and a multiple of 4,
-    mask bool [Q, P] (True = masked) or None.  Forward: two streaming wgmma passes (row statistics, then output);
-    backward: one streaming pass with five wgmma GEMMs per 64-key tile that recomputes the probabilities from the
+    mask = int32 bit rows [Q, 2*ceil(P/64)] (attention_mask_bits, pack_mask_bits), bool [Q, P] (True = masked) or
+    None.  Forward: two streaming wgmma passes (row statistics, then output); backward: one streaming pass with five wgmma GEMMs per 64-key tile that recomputes the probabilities from the
     saved log-sum-exp (xattn.cu).  Each pass splits the keys into chunks whose shares of out / dq are added in a fixed
     order; the per-chunk scratch comes from the library's own stream-ordered pool.  The kernels hold 128 queries at a
     time: above 128 every block of 128 queries streams K and V again, and the backward adds the blocks' dk / dv
@@ -876,7 +899,7 @@ class MaskedCrossAttention(torch.autograd.Function):
         P = k.shape[0]
         D = HD // heads
         scale = float(D) ** -0.5
-        bits = pack_mask_bits(mask) if mask is not None else None
+        bits = pack_mask_bits(mask) if mask is not None and mask.dtype == torch.bool else mask
         out = torch.zeros(Q, HD, dtype=torch.float32, device=q.device)
         lse = torch.empty(heads, Q, dtype=torch.float32, device=q.device)
         call("pasco_xattn_forward", ptr(q), ptr(k), ptr(v), ptr(bits), Q, P, heads, D, C.c_float(scale), ptr(out),
@@ -902,7 +925,8 @@ class MaskedCrossAttention(torch.autograd.Function):
 def cross_attention(mha: torch.nn.MultiheadAttention, q: torch.Tensor, kv: torch.Tensor,
                     mask: Optional[torch.Tensor]) -> torch.Tensor:
     """`mha(q, kv, kv, attn_mask=mask)` of blocks.py:73-92 for one scene: q [Q, d] (query position already added),
-    kv [P, d] (key position already added), mask bool [Q, P] (True = masked) or None → [Q, d].  The K / V projections
+    kv [P, d] (key position already added), mask = attention_mask_bits' bit rows, bool [Q, P] (True = masked) or None
+    → [Q, d].  The K / V projections
     over all voxels run on the wgmma GEMM, the masked softmax·V on MaskedCrossAttention."""
     d = q.shape[-1]
     wq, wk, wv = mha.in_proj_weight.split(d, 0)
