@@ -388,6 +388,28 @@ int pasco_eval_ssc(const int64_t* lin, const int32_t* pred, const float* conf, i
 int pasco_eval_vox(const int64_t* lin, const int32_t* panoptic, const float* confidence, int64_t n, const int32_t* gt_id,
                    int64_t cells, const int32_t* match, int32_t S, const float bounds[16], int32_t* cal, double* sums, pasco_stream_t s);
 
+/* ---- dense forms: the volumes the reference's Net.evaluate_all is given (net_panoptic_sparse.py:650-695), cell i of
+ *      an [X, Y, Z] volume is row i; no cell array is read ------------------------------------------------------------
+ * panoptic_quality.py:359: out fp32 [cells] = gt_id as float (pasco_eval_gt's ids, 0 at unknown cells), the
+ * gt_panoptic_seg volume evaluate_all returns.                                                                      */
+int pasco_eval_gt_volume(const int32_t* gt_id, int64_t cells, float* out, pasco_stream_t s);
+/* pasco_eval_pairs over a dense id volume panoptic int32 [cells]: pred_area[0] = cells with an id outside [0, S].    */
+int pasco_eval_pairs_dense(const int32_t* panoptic, const int32_t* gt_id, const uint8_t* label, int64_t cells, int32_t G,
+                           int32_t S, int32_t* pairs, int32_t* pred_area, pasco_stream_t s);
+/* net_panoptic_sparse.py:682-694 + metrics.py:480-547 over class planes prob fp32 [K][cells] (channel-major): pred int64
+ * [cells] = first argmax over K as torch.argmax (a NaN wins, the first NaN); confmat int32 [K x K] at known cells; with
+ * confidence fp32 [cells] (NULL: no calibration, cal / sums untouched, sums may be NULL) cal int32 [2][2][16] and sums
+ * double [34] as pasco_eval_ssc's, the NLL of the label's own plane.  bad = known cells with a label >= K, or with a
+ * confidence outside [0, 1] (NaN included).  1 <= K <= 64.                                                          */
+int pasco_eval_ssc_planes(const float* prob, int32_t K, int64_t cells, const uint8_t* label, const float* confidence,
+                          const float bounds[16], int64_t* pred, int32_t* confmat, int32_t* cal, int32_t* bad,
+                          double* sums, pasco_stream_t s);
+/* pasco_eval_vox over dense volumes panoptic int32 / confidence fp32 [cells]; bad = counted cells (gt id != 0,
+ * confidence != 0) whose confidence lies outside [0, 1], left out of cal and sums.                                  */
+int pasco_eval_vox_dense(const int32_t* panoptic, const float* confidence, const int32_t* gt_id, int64_t cells,
+                         const int32_t* match, int32_t S, const float bounds[16], int32_t* cal, int32_t* bad,
+                         double* sums, pasco_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -81,6 +81,10 @@ PROTOTYPES = {
     "pasco_eval_pairs": (C.c_int, [_p, _p, _i64, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
     "pasco_eval_ssc": (C.c_int, [_p, _p, _p, _i64, _p, _i64, _i32, _p, _i32, _p, _p, _p, _p, _p, _p, _p]),
     "pasco_eval_vox": (C.c_int, [_p, _p, _p, _i64, _p, _i64, _p, _i32, _p, _p, _p, _p]),
+    "pasco_eval_gt_volume": (C.c_int, [_p, _i64, _p, _p]),
+    "pasco_eval_pairs_dense": (C.c_int, [_p, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
+    "pasco_eval_ssc_planes": (C.c_int, [_p, _i32, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "pasco_eval_vox_dense": (C.c_int, [_p, _p, _p, _i64, _p, _i32, _p, _p, _p, _p, _p]),
 }
 
 _lib: Optional[C.CDLL] = None

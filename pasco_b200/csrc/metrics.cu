@@ -1,9 +1,11 @@
 // Evaluation of PascoNet.predict's outputs against a scene's ground truth (sm_90a): the counting passes behind the
 // reference's Net.evaluate_all (net_panoptic_sparse.py:650-765) — panoptic quality (panoptic_quality.py:175-261),
 // completion and semantic IoU and their calibration (metrics.py:450-691), and the voxel calibration of
-// UncertaintyMetrics.compute_ece_panop (metrics.py:98-165).  The passes read the predictions' sparse rows; no dense
-// prediction volume is written.  They produce small tables (integer histograms, 16-slot calibration bins) that the host
-// finishes in pasco_b200/metrics.py.
+// UncertaintyMetrics.compute_ece_panop (metrics.py:98-165).  The row-form passes read PascoNet.predict's sparse rows
+// (pasco_b200/metrics.py); the dense forms read the volumes the unmodified reference hands its evaluate_all
+// (pasco_b200/hooks.py): channel-major class planes and [X, Y, Z] id / confidence volumes, row i = cell i.  They produce
+// small tables (integer histograms, 16-slot calibration bins) that the host finishes; the dense forms also write the
+// two volumes evaluate_all returns (its argmax and the ground-truth ids).
 //
 // Counts are integer atomics, exact in any order.  Floating-point sums are accumulated in double by one thread per
 // row position of a CTA, added over the CTA's threads in thread order and over the CTAs in CTA order (k_part_reduce):
@@ -293,6 +295,171 @@ Bounds to_bounds(const float b[kSlots]) {
   return B;
 }
 
+// ------------------------------------------------------------------------------------------------
+// dense forms: the volumes the reference's evaluate_all is given (net_panoptic_sparse.py:650-695), row i = cell i
+// ------------------------------------------------------------------------------------------------
+
+// the gt_panoptic_seg volume convert_mask_label_to_panoptic_output returns (float32, torch.zeros(masks.shape[1:])),
+// zeroed at unknown cells: k_eval_gt's ids as floats
+__global__ void __launch_bounds__(kBlock) k_eval_gt_volume(const int32_t* __restrict__ gt_id, int64_t cells,
+                                                            float* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < cells; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = (float)__ldg(gt_id + i);
+}
+
+// k_eval_pairs over a dense id volume: no cell array, every id outside [0, S1) counts in pred_area[0]
+template <bool SHARED>
+__global__ void __launch_bounds__(kBlock) k_eval_pairs_dense(const int32_t* __restrict__ pan,
+                                                              const int32_t* __restrict__ gt_id,
+                                                              const uint8_t* __restrict__ label, int64_t cells, int G1,
+                                                              int S1, int32_t* __restrict__ pairs,
+                                                              int32_t* __restrict__ pred_area) {
+  extern __shared__ int s_pairs[];
+  const int tot = G1 * S1 + S1;
+  int* tab = SHARED ? s_pairs : pairs;
+  int* area = SHARED ? s_pairs + G1 * S1 : pred_area;
+  if (SHARED) {
+    for (int i = threadIdx.x; i < tot; i += blockDim.x) s_pairs[i] = 0;
+    __syncthreads();
+  }
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < cells; r += (int64_t)gridDim.x * blockDim.x) {
+    const int p = __ldg(pan + r);
+    if (p == 0) continue;
+    if (__ldg(label + r) == 255) continue;                     // pred_panoptic_seg[unknown_mask] = 0
+    if (p < 0 || p >= S1) {
+      atomicAdd(area, 1);
+      continue;
+    }
+    atomicAdd(tab + (int64_t)__ldg(gt_id + r) * S1 + p, 1);
+    atomicAdd(area + p, 1);
+  }
+  if (SHARED) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < tot; i += blockDim.x) {
+      const int v = s_pairs[i];
+      if (v) atomicAdd(i < G1 * S1 ? pairs + i : pred_area + (i - G1 * S1), v);
+    }
+  }
+}
+
+// SSC over channel-major class planes prob [K][cells] (evaluate_all's argmax, add_batch, add_batch_ece): per cell the
+// first-max argmax over K as torch.argmax takes it (a NaN wins, the first NaN), written as int64 pred; at known cells
+// the K x K confusion counts; with ECE, for the given confidence, the 2 x 2 x 16 calibration counts, the 2 x 16
+// confidence sums and per partition Σ −log(prob[label] + 1e-12) (float columns as k_eval_ssc's).  bad counts the known
+// cells with a label >= K and, with ECE, those whose confidence lies outside [0, 1] (torchmetrics would take sigmoids).
+struct SscPlaneParams {
+  const float* prob;
+  const float* conf;
+  const uint8_t* label;
+  int64_t n, chunk;        // n = cells
+  int K;
+  Bounds B;
+  int64_t* pred;
+  int32_t* confmat;
+  int32_t* cal;
+  int32_t* bad;
+  double* part;
+};
+
+template <bool ECE>
+__global__ void __launch_bounds__(kBlock) k_eval_ssc_planes(const __grid_constant__ SscPlaneParams p) {
+  extern __shared__ double s_acc[];                            // ECE: [kSscCols][kBlock]
+  int* s_conf = reinterpret_cast<int*>(s_acc + (ECE ? kSscCols * kBlock : 0));   // [K * K]
+  int* s_cal = s_conf + p.K * p.K;                             // [64]
+  __shared__ int s_bad;
+  if (ECE)
+    for (int i = threadIdx.x; i < kSscCols * kBlock; i += blockDim.x) s_acc[i] = 0.0;
+  for (int i = threadIdx.x; i < p.K * p.K + 4 * kSlots; i += blockDim.x) s_conf[i] = 0;
+  if (threadIdx.x == 0) s_bad = 0;
+  __syncthreads();
+  const int64_t r0 = blockIdx.x * p.chunk, r1 = min(p.n, r0 + p.chunk);
+  double* my = s_acc + threadIdx.x;
+  for (int64_t i = r0 + threadIdx.x; i < r1; i += kBlock) {
+    float best = __ldg(p.prob + i);
+    int arg = 0;
+#pragma unroll 4
+    for (int k = 1; k < p.K; ++k) {
+      const float v = __ldg(p.prob + (int64_t)k * p.n + i);
+      if (!isnan(best) && (isnan(v) || v > best)) {
+        best = v;
+        arg = k;
+      }
+    }
+    p.pred[i] = arg;
+    const int lab = __ldg(p.label + i);
+    if (lab == 255) continue;                                  // keep = target != 255
+    if (lab >= p.K) {
+      atomicAdd(&s_bad, 1);
+      continue;
+    }
+    atomicAdd(s_conf + lab * p.K + arg, 1);
+    if (ECE) {
+      const float c = __ldg(p.conf + i);
+      if (!(c >= 0.f && c <= 1.f)) {
+        atomicAdd(&s_bad, 1);
+        continue;
+      }
+      const int part = arg != 0, slot = conf_slot(p.B, c);
+      atomicAdd(s_cal + part * 2 * kSlots + slot, 1);
+      if (arg == lab) atomicAdd(s_cal + part * 2 * kSlots + kSlots + slot, 1);
+      my[(part * kSlots + slot) * kBlock] += (double)c;
+      const float pt = __ldg(p.prob + (int64_t)lab * p.n + i);
+      my[(2 * kSlots + part) * kBlock] += (double)(-logf(__fadd_rn(pt, 1e-12f)));
+    }
+  }
+  if (ECE) flush_partials(s_acc, kSscCols, p.part);
+  else __syncthreads();
+  for (int i = threadIdx.x; i < p.K * p.K + 4 * kSlots; i += blockDim.x) {
+    const int v = s_conf[i];
+    if (v) atomicAdd(i < p.K * p.K ? p.confmat + i : p.cal + (i - p.K * p.K), v);
+  }
+  if (threadIdx.x == 0 && s_bad) atomicAdd(p.bad, s_bad);
+}
+
+// k_eval_vox over dense volumes (compute_ece_panop's nonempty_mask = gt id != 0 and confidence != 0); bad counts the
+// confidences of those cells outside [0, 1]
+struct VoxDenseParams {
+  const int32_t* pan;
+  const float* conf;
+  int64_t n, chunk;        // n = cells
+  const int32_t* gt_id;
+  const int32_t* match;    // [S1]
+  int S1;
+  Bounds B;
+  int32_t* cal;
+  int32_t* bad;
+  double* part;            // [grid][16]
+};
+
+__global__ void __launch_bounds__(kBlock) k_eval_vox_dense(const __grid_constant__ VoxDenseParams p) {
+  extern __shared__ double s_acc[];                            // [kSlots][kBlock]
+  __shared__ int s_cal[2 * kSlots + 1];
+  for (int i = threadIdx.x; i < kSlots * kBlock; i += blockDim.x) s_acc[i] = 0.0;
+  if (threadIdx.x <= 2 * kSlots) s_cal[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t r0 = blockIdx.x * p.chunk, r1 = min(p.n, r0 + p.chunk);
+  double* my = s_acc + threadIdx.x;
+  for (int64_t r = r0 + threadIdx.x; r < r1; r += kBlock) {
+    const float c = __ldg(p.conf + r);
+    if (c == 0.f) continue;
+    const int g = __ldg(p.gt_id + r);
+    if (g == 0) continue;
+    if (!(c >= 0.f && c <= 1.f)) {
+      atomicAdd(s_cal + 2 * kSlots, 1);
+      continue;
+    }
+    const int pid = __ldg(p.pan + r);
+    const int mapped = pid > 0 && pid < p.S1 ? __ldg(p.match + pid) : 0;
+    const int slot = conf_slot(p.B, c);
+    atomicAdd(s_cal + slot, 1);
+    if (mapped == g) atomicAdd(s_cal + kSlots + slot, 1);
+    my[slot * kBlock] += (double)c;
+  }
+  flush_partials(s_acc, kSlots, p.part);
+  if (threadIdx.x < 2 * kSlots && s_cal[threadIdx.x]) atomicAdd(p.cal + threadIdx.x, s_cal[threadIdx.x]);
+  if (threadIdx.x == 2 * kSlots && s_cal[threadIdx.x]) atomicAdd(p.bad, s_cal[threadIdx.x]);
+}
+
 }  // namespace
 
 extern "C" int pasco_eval_gt(const uint8_t* masks, int32_t n_masks, const int32_t* seg_of_mask, const uint8_t* label,
@@ -373,4 +540,72 @@ extern "C" int pasco_eval_vox(const int64_t* lin, const int32_t* panoptic, const
   p.B = to_bounds(bounds);
   p.cal = cal;
   return cal_launch("pasco_eval_vox", k_eval_vox, p, kSlots, 0, sums, (cudaStream_t)s);
+}
+
+extern "C" int pasco_eval_gt_volume(const int32_t* gt_id, int64_t cells, float* out, pasco_stream_t s) {
+  PASCO_CHECK_ARG(cells > 0, "pasco_eval_gt_volume: empty grid");
+  k_eval_gt_volume<<<grid_for(cells, kBlock, 4), kBlock, 0, (cudaStream_t)s>>>(gt_id, cells, out);
+  PASCO_CHECK_LAUNCH("pasco_eval_gt_volume");
+  return 0;
+}
+
+extern "C" int pasco_eval_pairs_dense(const int32_t* panoptic, const int32_t* gt_id, const uint8_t* label,
+                                      int64_t cells, int32_t G, int32_t S, int32_t* pairs, int32_t* pred_area,
+                                      pasco_stream_t s) {
+  PASCO_CHECK_ARG(G >= 0 && S >= 0 && cells > 0, "pasco_eval_pairs_dense: bad segment or cell counts");
+  const int G1 = G + 1, S1 = S + 1;
+  const size_t smem = sizeof(int) * ((size_t)G1 * S1 + S1);
+  const int grid = grid_for(cells, kBlock, 2);
+  if (smem <= kSmemCap) {
+    cudaFuncSetAttribute(k_eval_pairs_dense<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap);
+    k_eval_pairs_dense<true><<<grid, kBlock, smem, (cudaStream_t)s>>>(panoptic, gt_id, label, cells, G1, S1, pairs,
+                                                                      pred_area);
+  } else {
+    k_eval_pairs_dense<false><<<grid, kBlock, 0, (cudaStream_t)s>>>(panoptic, gt_id, label, cells, G1, S1, pairs,
+                                                                    pred_area);
+  }
+  PASCO_CHECK_LAUNCH("pasco_eval_pairs_dense");
+  return 0;
+}
+
+extern "C" int pasco_eval_ssc_planes(const float* prob, int32_t K, int64_t cells, const uint8_t* label,
+                                     const float* confidence, const float bounds[16], int64_t* pred, int32_t* confmat,
+                                     int32_t* cal, int32_t* bad, double* sums, pasco_stream_t s) {
+  PASCO_CHECK_ARG(K >= 1 && K <= 64, "pasco_eval_ssc_planes: 1 <= K <= 64 classes (got %d)", K);
+  PASCO_CHECK_ARG(cells > 0, "pasco_eval_ssc_planes: empty grid");
+  SscPlaneParams p = {};
+  p.prob = prob;
+  p.conf = confidence;
+  p.label = label;
+  p.n = cells;
+  p.K = K;
+  p.B = to_bounds(bounds);
+  p.pred = pred;
+  p.confmat = confmat;
+  p.cal = cal;
+  p.bad = bad;
+  const size_t counters = sizeof(int) * ((size_t)K * K + 4 * kSlots);
+  if (confidence != nullptr)
+    return cal_launch("pasco_eval_ssc_planes", k_eval_ssc_planes<true>, p, kSscCols, counters, sums, (cudaStream_t)s);
+  const int G = eval_grid(cells, &p.chunk);
+  k_eval_ssc_planes<false><<<G, kBlock, counters, (cudaStream_t)s>>>(p);
+  PASCO_CHECK_LAUNCH("pasco_eval_ssc_planes");
+  return 0;
+}
+
+extern "C" int pasco_eval_vox_dense(const int32_t* panoptic, const float* confidence, const int32_t* gt_id,
+                                    int64_t cells, const int32_t* match, int32_t S, const float bounds[16],
+                                    int32_t* cal, int32_t* bad, double* sums, pasco_stream_t s) {
+  PASCO_CHECK_ARG(S >= 0 && cells > 0, "pasco_eval_vox_dense: bad segment or cell count");
+  VoxDenseParams p = {};
+  p.pan = panoptic;
+  p.conf = confidence;
+  p.n = cells;
+  p.gt_id = gt_id;
+  p.match = match;
+  p.S1 = S + 1;
+  p.B = to_bounds(bounds);
+  p.cal = cal;
+  p.bad = bad;
+  return cal_launch("pasco_eval_vox_dense", k_eval_vox_dense, p, kSlots, 0, sums, (cudaStream_t)s);
 }

@@ -27,21 +27,33 @@ it by name.  They return the reference's structures, computed on the sparse rows
 emits of csrc/panoptic.cu; inputs outside what the kernels cover (CPU tensors, batch size != 1, more than 8 subnets or 64
 classes, rows outside the requested box) go to the saved originals (`_pasco_b200_orig_*`).
 
+The evaluation hook (install(evaluate=True)) replaces `Net.evaluate_all` (net_panoptic_sparse.py:650-765, and the
+KITTI-360 Net's) — run in every training and validation step and for every test entry — whose host work copies the
+dense volumes with .cpu().numpy(), takes np.unique over 2.1 M uint64 keys and loops in Python per matched segment.  It
+runs the dense evaluation passes of csrc/metrics.cu over the volumes it is given (class planes, panoptic ids, voxel
+confidences) and finishes the tables with metrics.py's host code into the reference's own PQStat, SSCMetrics and
+UncertaintyMetrics objects, with their value types; the ECE is torchmetrics 1.4's binary_calibration_error.  At most
+EVAL_SYNCS host synchronisations per call.  CPU tensors, more than 64 classes or one panoptic item, uncertainty
+thresholds other than [0.5], volumes whose shapes disagree and labels or predictions outside [0, K) other than 255 go
+to the saved original.
+
     import pasco_b200.hooks; pasco_b200.hooks.install()        # after `pasco` is importable, before building Net
     pasco_b200.hooks.install(postprocess=True)                 # the attention and the post-processing
+    pasco_b200.hooks.install(postprocess=True, evaluate=True)  # ... and the evaluation
     PASCO_B200_HOOKS=1 python scripts/train.py ...              # compat/MinkowskiEngine calls install() lazily
-    PASCO_B200_HOOKS=attention,postprocess python scripts/eval.py ...
+    PASCO_B200_HOOKS=attention,postprocess,evaluate python scripts/eval.py ...
 """
 from __future__ import annotations
 
 import importlib
 import time
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
 from . import me as ME
-from . import ops, predict
+from . import metrics, ops, predict
 
 
 def _transformer_forward(self, xs, sem_logits, min_Cs, max_Cs, keep_pad):
@@ -230,9 +242,240 @@ def _panoptic_inference(voxel_output, query_output, overlap_threshold, object_ma
 
 
 # ------------------------------------------------------------------------------------------------
+# evaluation: Net.evaluate_all (net_panoptic_sparse.py:650-765) on the dense forms of csrc/metrics.cu, finished by
+# metrics.py's host code into the reference's own metric objects
+# ------------------------------------------------------------------------------------------------
+_EVAL_USERS = (("pasco.models.net_panoptic_sparse", "Net"), ("pasco.models.net_panoptic_sparse_kitti360", "Net_kitti360"))
+EVAL_SYNCS = 3          # host synchronisations of a hooked evaluate_all call, at most (see _evaluate)
+
+
+def _ref_iou(inter: int, union: int):
+    """The reference's pair IoU: np.int64 intersection / a 0-d torch area, i.e. Tensor.__rdiv__ = reciprocal() * other,
+    in float32."""
+    return (np.float32(1.0) / np.float32(union)) * np.float32(inter)
+
+
+class _SeededCats(dict):
+    """metrics.finish_pq's category mapping over a PQStat: a category first touched starts from the PQStat's current
+    fields (device iou sums as their host values), so the float32 sums continue in the reference's order."""
+
+    def __init__(self, pq_stat, prev):
+        super().__init__()
+        self.pq, self.prev = pq_stat, prev
+
+    def __missing__(self, c):
+        cat = metrics._Cat()
+        old = self.pq.pq_per_cat.get(c)
+        if old is not None:
+            cat.all_n, cat.tp, cat.fp, cat.fn = old.all_n, old.tp, old.fp, old.fn
+            cat.all_iou = self.prev.get((c, "all_iou"), old.all_iou)
+            cat.iou = self.prev.get((c, "iou"), old.iou)
+        self[c] = cat
+        return cat
+
+
+def _host_copy(t: torch.Tensor) -> torch.Tensor:
+    """A pinned host copy, enqueued on the stream: complete at the call's next synchronisation."""
+    h = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
+    h.copy_(t, non_blocking=True)
+    return h
+
+
+def _evaluate(net, ssc_confidence, i_infer, sem_prob, panop_out, semantic_label, mask_labels, ssc_metrics, pq_stat,
+              compute_uncertainty, inference_time):
+    """evaluate_all on the device, or None where the saved original decides (the caller then runs it; nothing has been
+    updated).  Host synchronisations: one to read mask_labels["labels"] when it is a device tensor, one for every
+    counting table and the returned volumes, and with compute_uncertainty one for the voxel calibration table — at most
+    EVAL_SYNCS, whatever the query, segment or cell counts."""
+    pan_all = panop_out["panoptic_seg_denses"]
+    if not (torch.is_tensor(sem_prob) and sem_prob.is_cuda and sem_prob.dtype == torch.float32 and sem_prob.dim() == 4
+            and torch.is_tensor(pan_all) and len(pan_all) == 1 and torch.is_tensor(semantic_label)):
+        return None
+    dev, K, size = sem_prob.device, sem_prob.shape[0], tuple(sem_prob.shape[1:])
+    cells = sem_prob[0].numel()
+    ml = mask_labels[0]
+    masks = ml["masks"]
+    thresholds = list(getattr(net, "uncertainty_thresholds", [0.5]))
+    pan = pan_all[0]
+    if (K > 64 or K != ssc_metrics.n_classes or min(size) < 2 or tuple(semantic_label.shape) != (1,) + size
+            or semantic_label.device != dev or semantic_label.dtype.is_floating_point or semantic_label.dtype == torch.bool
+            or pan.device != dev or pan.dtype != torch.int32 or tuple(pan.shape) != size
+            or not (torch.is_tensor(masks) and masks.device == dev and masks.dim() == 4 and tuple(masks.shape[1:]) == size)
+            or not hasattr(pq_stat, "pq_per_cat")):
+        return None
+    if compute_uncertainty:
+        vconf = panop_out["vox_confidence_denses"][0]
+        if (thresholds != [0.5] or not torch.is_tensor(ssc_confidence) or ssc_confidence.device != dev
+                or ssc_confidence.dtype != torch.float32 or ssc_confidence.numel() != cells
+                or not torch.is_tensor(vconf) or vconf.device != dev or vconf.dtype != torch.float32
+                or tuple(vconf.shape) != size):
+            return None
+    # the PQStat's float32 iou sums so far: device tensors are read with the tables below
+    prev_t = []
+    for c, s in pq_stat.pq_per_cat.items():
+        for f in ("all_iou", "iou"):
+            v = getattr(s, f)
+            if torch.is_tensor(v):
+                if not (v.device == dev and v.dtype == torch.float32 and v.numel() == 1):
+                    return None
+                prev_t.append(((c, f), v.reshape(1)))
+
+    # ground truth (convert_mask_label_to_panoptic_output's walk on the host, the mask stack on the device)
+    labels = ml["labels"]
+    labels = labels.reshape(-1).tolist() if torch.is_tensor(labels) else list(labels)      # sync 1 for device labels
+    if any(int(v) != v or not (0 <= v < K or v == 255) for v in labels) or len(labels) != masks.shape[0]:
+        return None
+    labels = [int(v) for v in labels]
+    seg_of, segs = metrics.gt_walk(labels, net.thing_ids)
+    n, G = len(labels), len(segs)
+    label = semantic_label.reshape(-1)
+    if label.dtype != torch.uint8:                     # anything outside [0, K) other than 255 reads as K: the fallback
+        label = torch.where(((label >= 0) & (label < K)) | (label == 255), label, K).to(torch.uint8)
+    label = label.contiguous()
+    m8 = masks.reshape(n, cells)
+    m8 = m8.contiguous().view(torch.uint8) if m8.dtype == torch.bool else (m8 != 0).contiguous().view(torch.uint8)
+    seg = torch.tensor(seg_of, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    gt_id, counts = ops.eval_gt(m8, seg, label, G, K)
+    gt_host = _host_copy(ops.eval_gt_volume(gt_id))
+
+    # the entry: (gt id, pred id) pairs, and the SSC pass over the class planes
+    seg_infos = panop_out["segments_infos"][0]
+    ids = [int(s["id"]) for s in seg_infos]
+    S = max(ids + [0])
+    t_pairs = (G + 1) * (S + 1) + S + 1
+    o_ssc = t_pairs + t_pairs % 2
+    o_sum = K * K + 65 + (K * K + 65) % 2
+    tab = torch.zeros(o_ssc + o_sum + 68, dtype=torch.int32, device=dev)
+    ops.eval_pairs_dense(pan.contiguous(), gt_id, label, G, S, tab[:t_pairs])
+    pred = ops.eval_ssc_planes(sem_prob.reshape(K, cells).contiguous(), label,
+                               ssc_confidence.reshape(-1).contiguous() if compute_uncertainty else None, tab[o_ssc:])
+    pred_host = _host_copy(pred)
+    parts = [tab, counts] + ([torch.cat([v for _, v in prev_t]).view(torch.int32)] if prev_t else [])
+    host = torch.cat(parts).cpu()                                                            # sync 2
+    h = host.numpy()
+    t, counts_h = h[:tab.numel()], h[tab.numel():tab.numel() + counts.numel()]
+    prev = {k: np.float32(v) for (k, _), v in zip(prev_t, h[tab.numel() + counts.numel():].view(np.float32))}
+    mask_sum, id_area, hist = counts_h[:n], counts_h[n:n + G + 1], counts_h[n + G + 1:]
+    pairs = t[:(G + 1) * (S + 1)].reshape(G + 1, S + 1)
+    pred_area = t[(G + 1) * (S + 1):t_pairs]
+    conf = t[o_ssc:o_ssc + K * K].reshape(K, K).astype(np.int64)
+    cal = t[o_ssc + K * K:o_ssc + K * K + 64].reshape(2, 2, 16).astype(np.float64)
+    bad = int(t[o_ssc + K * K + 64])
+    sums = host[o_ssc + o_sum:o_ssc + o_sum + 68].view(torch.float64).numpy()                # 8-byte aligned
+    present = set(np.nonzero(pred_area)[0].tolist()) - {0}
+    if hist[K] or bad or pred_area[0] or not present <= set(ids):
+        return None                  # labels or confidences outside the covered range, or ids without a segment
+
+    # panoptic quality into the PQStat, in the reference's order and value types
+    gt_area = {sid: int(mask_sum[i]) for sid, _, _, i in segs}
+    gt_segs = [(sid, c) for sid, c, _, _ in segs if id_area[sid] > 0]
+    pred_kept = [s for s in seg_infos if int(s["id"]) in present]
+    pred_segs = [(int(s["id"]), int(s["category_id"])) for s in pred_kept]
+    cats = _SeededCats(pq_stat, prev)
+    _, _, unc = metrics.finish_pq(cats, pairs, pred_area, gt_area, gt_segs, pred_segs, net.thing_ids, iou_of=_ref_iou)
+
+    vox = None
+    if compute_uncertainty:
+        match = np.zeros(S + 1, np.int32)
+        for p, g in unc.items():
+            match[p] = g
+        vt = torch.zeros(66, dtype=torch.int32, device=dev)
+        ops.eval_vox_dense(pan.contiguous(), vconf.contiguous(), gt_id,
+                           torch.from_numpy(match).pin_memory().to(dev, non_blocking=True), vt)
+        vh = vt.cpu()                                                                        # sync 3
+        if int(vh[64]):
+            return None
+        vox = vh[:32].numpy().reshape(2, 16), vh[32:64].view(torch.float64).numpy()
+
+    # ---- nothing has been updated so far; from here on the call writes the reference's objects
+    tensor_fields = [(c, f, getattr(cat, f)) for c, cat in cats.items() for f in ("all_iou", "iou")
+                     if isinstance(getattr(cat, f), np.float32)]
+    vals = torch.tensor([float(v) for _, _, v in tensor_fields], dtype=torch.float32).pin_memory().to(
+        dev, non_blocking=True)
+    j = {(c, f): i for i, (c, f, _) in enumerate(tensor_fields)}
+    for c, cat in cats.items():
+        st = pq_stat[c]
+        st.tp, st.fp, st.fn, st.all_n = cat.tp, cat.fp, cat.fn, cat.all_n
+        for f in ("all_iou", "iou"):
+            if (c, f) in j:
+                setattr(st, f, vals[j[c, f]])
+    for s in pred_kept:                                # pq_compute_single_core records each kept segment's area
+        s["area"] = np.int64(pred_area[int(s["id"])])
+
+    tp, fp, fn = int(conf[1:, 1:].sum()), int(conf[0, 1:].sum()), int(conf[1:, 0].sum())
+    diag = np.diag(conf)
+    ssc_metrics.completion_tp += tp
+    ssc_metrics.completion_fp += fp
+    ssc_metrics.completion_fn += fn
+    ssc_metrics.tps += diag
+    ssc_metrics.fps += conf.sum(0) - diag
+    ssc_metrics.fns += conf.sum(1) - diag
+
+    if compute_uncertainty:
+        ssc_metrics.empty_nll += float(sums[32])
+        ssc_metrics.nonempty_nll += float(sums[33])
+        ssc_metrics.n_empty_voxels += int(cal[0, 0].sum())
+        ssc_metrics.n_nonempty_voxels += int(cal[1, 0].sum())
+        ssc_metrics.empty_ece += metrics.ece_from_bins(cal[0, 0], sums[:16], cal[0, 1])
+        ssc_metrics.nonempty_ece += metrics.ece_from_bins(cal[1, 0], sums[16:32], cal[1, 1])
+        ssc_metrics.ece_count += 1
+        ssc_metrics.inference_time += inference_time
+
+        um = net.uncertainty_metrics_by_thresholds[0.5][i_infer]
+        gcat = dict(gt_segs)
+        for s in pred_kept:                            # compute_ece_panop (metrics.py:98-165)
+            g = unc.get(int(s["id"]))
+            um.ins_confs.append(s["confidence"])
+            um.ins_all_class_probs.append(s["all_class_probs"])
+            um.ins_sem_labels.append(net.n_classes if g is None else gcat[g])
+            um.ins_correct.append(g is not None and gcat[g] == s["category_id"])
+        vc, vs = vox
+        um.mask_ece += metrics.ece_from_bins(vc[0], vs, vc[1]) if vc[0].sum() else 0
+        um.mask_auprc += 0
+        um.mask_auroc += 0
+        um.mask_fpr95 += 0
+        um.count += 1
+
+    areas = counts[:n].to(torch.int64)
+    gt_segments_info = [{"id": sid, "isthing": isthing, "category_id": c, "area": areas[i]}
+                        for sid, c, isthing, i in segs if id_area[sid] > 0]
+    return gt_host.numpy().reshape(size), gt_segments_info, pred_host.numpy().reshape((1,) + size)
+
+
+def _evaluate_all(self, ssc_confidence, i_infer, sem_prob, panop_out, semantic_label, mask_labels, ssc_metrics,
+                  pq_stat, uncertainty_metrics, compute_uncertainty=False, inference_time=0.0):
+    """net_panoptic_sparse.py:650-695 on the dense evaluation passes: the reference's metric objects updated in place,
+    its (gt_panoptic_seg, gt_segments_info, ssc_pred) returned."""
+    with torch.no_grad():
+        out = _evaluate(self, ssc_confidence, i_infer, sem_prob, panop_out, semantic_label, mask_labels, ssc_metrics,
+                        pq_stat, compute_uncertainty, inference_time)
+    if out is None:
+        return self._pasco_b200_orig_evaluate_all(
+            ssc_confidence=ssc_confidence, i_infer=i_infer, sem_prob=sem_prob, panop_out=panop_out,
+            semantic_label=semantic_label, mask_labels=mask_labels, ssc_metrics=ssc_metrics, pq_stat=pq_stat,
+            uncertainty_metrics=uncertainty_metrics, compute_uncertainty=compute_uncertainty,
+            inference_time=inference_time)
+    return out
+
+
+def _evaluate_all_kitti360(self, ssc_confidence, i_infer, sem_prob, panop_out, semantic_label, mask_labels,
+                           ssc_metrics, pq_stat, uncertainty_metrics, compute_uncertainty=False):
+    """net_panoptic_sparse_kitti360.py:485-518: the same, without inference_time."""
+    with torch.no_grad():
+        out = _evaluate(self, ssc_confidence, i_infer, sem_prob, panop_out, semantic_label, mask_labels, ssc_metrics,
+                        pq_stat, compute_uncertainty, 0.0)
+    if out is None:
+        return self._pasco_b200_orig_evaluate_all(
+            ssc_confidence=ssc_confidence, i_infer=i_infer, sem_prob=sem_prob, panop_out=panop_out,
+            semantic_label=semantic_label, mask_labels=mask_labels, ssc_metrics=ssc_metrics, pq_stat=pq_stat,
+            uncertainty_metrics=uncertainty_metrics, compute_uncertainty=compute_uncertainty)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # install / uninstall
 # ------------------------------------------------------------------------------------------------
-_installed = set()     # "attention", "postprocess"
+_installed = set()     # "attention", "postprocess", "evaluate"
 
 
 def _install_attention() -> bool:
@@ -278,12 +521,37 @@ def _install_postprocess() -> bool:
     return True
 
 
-def install(attention: bool = True, postprocess: bool = False) -> bool:
+def _eval_nets():
+    """(Net class, its evaluate_all replacement) of both Net modules; the KITTI-360 one when importable."""
+    out = []
+    for (name, cls), fn in zip(_EVAL_USERS, (_evaluate_all, _evaluate_all_kitti360)):
+        try:
+            out.append((getattr(importlib.import_module(name), cls), fn))
+        except Exception:
+            if name != _EVAL_USERS[-1][0]:
+                raise
+    return out
+
+
+def _install_evaluate() -> bool:
+    try:
+        nets = _eval_nets()
+    except Exception:
+        return False
+    for net, fn in nets:
+        net._pasco_b200_orig_evaluate_all = net.evaluate_all
+        net.evaluate_all = fn
+    return True
+
+
+def install(attention: bool = True, postprocess: bool = False, evaluate: bool = False) -> bool:
     """Patch the reference (idempotent per group).  attention: TransformerPredictorV2.forward with its masks as
     bit rows, and the cross-attention layer that takes them; postprocess: the
-    Ensembler and panoptic_inference.  Returns False when a requested group's `pasco` modules are not importable."""
+    Ensembler and panoptic_inference; evaluate: Net.evaluate_all of both Net modules.  Returns False when a requested
+    group's `pasco` modules are not importable."""
     for name, wanted, fn in (("attention", attention, _install_attention),
-                             ("postprocess", postprocess, _install_postprocess)):
+                             ("postprocess", postprocess, _install_postprocess),
+                             ("evaluate", evaluate, _install_evaluate)):
         if wanted and name not in _installed:
             if not fn():
                 return False
@@ -304,4 +572,7 @@ def uninstall() -> None:
         Ensembler.ensemble_panop = Ensembler._pasco_b200_orig_ensemble_panop
         for mod in _users():
             mod.panoptic_inference = mod._pasco_b200_orig_panoptic_inference
+    if "evaluate" in _installed:
+        for net, _ in _eval_nets():
+            net.evaluate_all = net._pasco_b200_orig_evaluate_all
     _installed.clear()

@@ -236,32 +236,36 @@ class TensorField:
 
 
 def _hook_groups(value: str) -> frozenset:
-    """PASCO_B200_HOOKS: "0" / unset = none, "1" = the attention hooks, else a comma list of "attention", "postprocess"."""
+    """PASCO_B200_HOOKS: "0" / unset = none, "1" = the attention hooks, else a comma list of "attention", "postprocess",
+    "evaluate"."""
     if value in ("", "0"):
         return frozenset()
     if value == "1":
         return frozenset({"attention"})
     groups = frozenset(v.strip() for v in value.split(",") if v.strip())
-    if not groups <= {"attention", "postprocess"}:
-        raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of attention, postprocess")
+    if not groups <= {"attention", "postprocess", "evaluate"}:
+        raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of attention, postprocess, evaluate")
     return groups
 
 
 _HOOK_GROUPS = _hook_groups(os.environ.get("PASCO_B200_HOOKS", "0"))
 _HOOKS_PENDING = bool(_HOOK_GROUPS)
 _HOOK_MODULES = {"attention": ("pasco.models.transformer.transformer_predictor_v2",),
-                 "postprocess": ("pasco.models.ensembler", "pasco.models.helper")}     # either Net module imports both
+                 "postprocess": ("pasco.models.ensembler", "pasco.models.helper"),    # either Net module imports both
+                 "evaluate": ("pasco.models.metrics",)}                               # ... and this one
 
 
 def _maybe_install_hooks() -> None:
     """PASCO_B200_HOOKS: once the reference modules of the requested hook groups have been imported, route the
-    cross-attention and attention-mask construction ("attention") and the Ensembler and panoptic_inference
-    ("postprocess") onto the engine (pasco_b200/hooks.py).  Checked when a SparseTensor is built."""
+    cross-attention and attention-mask construction ("attention"), the Ensembler and panoptic_inference
+    ("postprocess") and Net.evaluate_all ("evaluate") onto the engine (pasco_b200/hooks.py).  Checked when a
+    SparseTensor is built."""
     global _HOOKS_PENDING
     if _HOOKS_PENDING and all(m in sys.modules for g in _HOOK_GROUPS for m in _HOOK_MODULES[g]):
         _HOOKS_PENDING = False
         from .. import hooks
-        hooks.install(attention="attention" in _HOOK_GROUPS, postprocess="postprocess" in _HOOK_GROUPS)
+        hooks.install(attention="attention" in _HOOK_GROUPS, postprocess="postprocess" in _HOOK_GROUPS,
+                      evaluate="evaluate" in _HOOK_GROUPS)
 
 
 class _LazyRows:

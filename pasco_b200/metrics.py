@@ -142,12 +142,17 @@ def gt_walk(labels: Sequence[int], thing_ids):
     return seg_of, segs
 
 
-def finish_pq(cats, pairs, pred_area, gt_area, gt_segs, pred_segs, thing_ids):
+def _iou_div(inter: int, union: int):
+    return _f32(inter) / _f32(union)
+
+
+def finish_pq(cats, pairs, pred_area, gt_area, gt_segs, pred_segs, thing_ids, iou_of=_iou_div):
     """pq_compute_single_core (panoptic_quality.py:175-261) and find_matched_segment at threshold 0.5 (:96-164) from
     the device tables.  pairs int [(G+1), (S+1)], pred_area [S+1] after zeroing, gt_area {id: own mask sum};
     gt_segs / pred_segs = [(id, category)] of the segments present after zeroing, in the reference's order.
-    Accumulates into cats (a defaultdict of _Cat, touched in the reference's order) and returns (this scene's
-    per-category fields, PQ matched pairs, uncertainty matches {pred id: gt id})."""
+    Accumulates into cats (a mapping of _Cat that creates a category when first touched, in the reference's order)
+    and returns (this scene's per-category fields, PQ matched pairs, uncertainty matches {pred id: gt id}).
+    iou_of(intersection, union) gives the float32 IoU of a pair."""
     gcat, pcat = dict(gt_segs), dict(pred_segs)
     scene = defaultdict(_Cat)
     gt_matched, pred_matched, pq_pairs, unc = set(), set(), set(), {}
@@ -156,7 +161,7 @@ def finish_pq(cats, pairs, pred_area, gt_area, gt_segs, pred_segs, thing_ids):
         if g not in gcat or p not in pcat:
             continue
         inter = int(pairs[g, p])
-        iou = _f32(inter) / _f32(int(pred_area[p]) + int(gt_area[g]) - inter)
+        iou = iou_of(inter, int(pred_area[p]) + int(gt_area[g]) - inter)
         if iou > MATCH_IOU:
             unc[p] = g
         if gcat[g] != pcat[p]:

@@ -1266,3 +1266,51 @@ def eval_vox(lin: torch.Tensor, pan: torch.Tensor, conf: torch.Tensor, gt_id: to
     call("pasco_eval_vox", ptr(lin), ptr(pan), ptr(conf), lin.shape[0], ptr(gt_id), gt_id.numel(), ptr(match),
          match.shape[0] - 1,
          _bounds(), ptr(out[:32]), ptr(out[32:].view(torch.float64)))
+
+
+# dense forms (the volumes the reference's evaluate_all is given: row i = cell i)
+def eval_gt_volume(gt_id: torch.Tensor) -> torch.Tensor:
+    """gt_id int32 [cells] (eval_gt's) → fp32 [cells]: the gt_panoptic_seg volume evaluate_all returns."""
+    out = torch.empty(gt_id.numel(), dtype=torch.float32, device=gt_id.device)
+    call("pasco_eval_gt_volume", ptr(gt_id), gt_id.numel(), ptr(out))
+    return out
+
+
+def eval_pairs_dense(pan: torch.Tensor, gt_id: torch.Tensor, label: torch.Tensor, G: int, S: int,
+                     out: torch.Tensor) -> None:
+    """eval_pairs over a dense id volume pan int32 [cells]; out as eval_pairs'."""
+    if not (pan.dtype == torch.int32 and pan.numel() == label.numel() and pan.device == label.device):
+        raise ValueError(f"eval_pairs_dense: the id volume must be int32 of {label.numel()} cells on {label.device}, got "
+                         f"{pan.dtype} {tuple(pan.shape)}")
+    t = (G + 1) * (S + 1)
+    call("pasco_eval_pairs_dense", ptr(pan), ptr(gt_id), ptr(label), label.numel(), G, S, ptr(out[:t]), ptr(out[t:]))
+
+
+def eval_ssc_planes(prob: torch.Tensor, label: torch.Tensor, conf: Optional[torch.Tensor], out: torch.Tensor) -> torch.Tensor:
+    """prob fp32 [K, cells] channel-major, label uint8 [cells], conf fp32 [cells] or None → the first-argmax volume int64
+    [cells].  out int32 [K*K + 64 + 1 + pad + 68], zeroed, in eval_ssc's layout (confusion counts, calibration counts,
+    bad-cell count, the 34 double sums); without conf only the confusion counts and the bad count are written."""
+    K, cells = prob.shape[0], label.numel()
+    if not (prob.dtype == torch.float32 and prob.dim() == 2 and prob.shape[1] == cells and prob.device == label.device):
+        raise ValueError(f"eval_ssc_planes: class planes must be fp32 [K, {cells}] on {label.device}, got {prob.dtype} "
+                         f"{tuple(prob.shape)}")
+    if conf is not None and not (conf.dtype == torch.float32 and conf.numel() == cells and conf.device == label.device):
+        raise ValueError(f"eval_ssc_planes: confidences must be fp32 [{cells}] on {label.device}, got {conf.dtype} "
+                         f"{tuple(conf.shape)}")
+    o = K * K + 65 + (K * K + 65) % 2
+    pred = torch.empty(cells, dtype=torch.int64, device=label.device)
+    call("pasco_eval_ssc_planes", ptr(prob), K, cells, ptr(label), ptr(conf), _bounds(), ptr(pred), ptr(out[:K * K]),
+         ptr(out[K * K:K * K + 64]), ptr(out[K * K + 64:K * K + 65]), ptr(out[o:o + 68].view(torch.float64)))
+    return pred
+
+
+def eval_vox_dense(pan: torch.Tensor, conf: torch.Tensor, gt_id: torch.Tensor, match: torch.Tensor,
+                   out: torch.Tensor) -> None:
+    """eval_vox over dense volumes pan int32 / conf fp32 [cells]; out int32 [66], zeroed: [2][16] (count, correct) per
+    slot, the 16 double confidence sums, then the count of counted cells with a confidence outside [0, 1]."""
+    cells = gt_id.numel()
+    if not (pan.dtype == torch.int32 and conf.dtype == torch.float32 and pan.numel() == conf.numel() == cells):
+        raise ValueError(f"eval_vox_dense: the volumes must be int32 / fp32 of {cells} cells, got {pan.dtype} "
+                         f"{tuple(pan.shape)} and {conf.dtype} {tuple(conf.shape)}")
+    call("pasco_eval_vox_dense", ptr(pan), ptr(conf), ptr(gt_id), cells, ptr(match), match.shape[0] - 1, _bounds(),
+         ptr(out[:32]), ptr(out[64:65]), ptr(out[32:64].view(torch.float64)))
