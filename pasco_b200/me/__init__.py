@@ -269,13 +269,13 @@ def _maybe_install_hooks() -> None:
 
 
 class _LazyRows:
-    """Deferred act(BatchNorm(x)) over rows — what MinkowskiBatchNorm (+ a following MinkowskiReLU / LeakyReLU) returns in
-    training mode, and in eval mode without gradients.  If the consumer is a stride-1 k>1 MinkowskiConvolution the three
-    run as ONE fused node whose BatchNorm apply pass writes the bf16 planes the convolution gathers (ops.BNActConv; in eval
-    mode one split pass with the running statistics, ops.bn_act_conv); any other consumer reading `.F`
-    materialises it through the fused row kernels (ops.batchnorm_rows).  Results are identical either way; this only
-    removes one full read+write of the activations per BatchNorm → convolution pair of the UNMODIFIED reference model
-    (pre-activation residual blocks, pasco/maskpls/mink.py:618-658)."""
+    """Deferred act(BatchNorm(x)) over rows — what MinkowskiBatchNorm (+ a following MinkowskiReLU / LeakyReLU) returns for
+    fp32 CUDA rows.  If the consumer is a stride-1 k>1 MinkowskiConvolution the three run through ops.bn_act_conv: in
+    training ONE fused node whose BatchNorm apply pass writes the bf16 planes the convolution gathers (ops.BNActConv), in
+    eval mode without gradients one split pass with the running statistics; any other consumer reading `.F` materialises
+    it through the fused row kernels (ops.batchnorm_rows), activation included.  Results are identical either way; this
+    only removes one full read+write of the activations per BatchNorm → convolution pair (pre-activation residual blocks,
+    pasco/maskpls/mink.py:618-658), in the unmodified reference model and in net3d.PascoNet alike."""
     ndim = 2
 
     def __init__(self, bn, x: torch.Tensor, act: int, group):
@@ -544,12 +544,11 @@ class MinkowskiBatchNorm(MinkowskiModuleBase):
 
     def forward(self, x):
         # training-mode statistics + apply run in the fused row kernels (ops.BatchNormAct; the convolution that produced
-        # x already left its column sums); same parameters, buffers and running-statistics update as nn.BatchNorm1d.  In
-        # eval mode without gradients the deferred form lets a following stride-1 convolution take bn_act_conv's
-        # split fusion (the running-statistics affine + activation written straight into its planes)
+        # x already left its column sums); same parameters, buffers and running-statistics update as nn.BatchNorm1d.  The
+        # deferred form lets a following activation fold into the apply pass and a following stride-1 convolution take
+        # bn_act_conv's fusion in every mode (ops.bn_act_conv_route picks it)
         xf = x.F
-        if (self.bn.running_mean is not None and xf.is_cuda and xf.dtype == torch.float32
-                and (self.bn.training or ops.inference_fusion_active(self.bn))):
+        if self.bn.running_mean is not None and xf.is_cuda and xf.dtype == torch.float32:
             return _like(x, _LazyRows(self.bn, xf, ops.ACT_NONE, self._group()))      # see _LazyRows
         return _like(x, ops.batchnorm_rows(self.bn, xf, ops.ACT_NONE, self._group()))
 
@@ -578,7 +577,7 @@ class MinkowskiSyncBatchNorm(MinkowskiBatchNorm):
                 new.bn.weight, new.bn.bias = module.bn.weight, module.bn.bias
             new.bn.running_mean, new.bn.running_var = module.bn.running_mean, module.bn.running_var
             new.bn.num_batches_tracked = module.bn.num_batches_tracked
-            return new
+            return new.train(module.training)
         for name, child in module.named_children():
             module.add_module(name, cls.convert_sync_batchnorm(child, process_group))
         return module

@@ -200,15 +200,11 @@ def sync_bn_statistics(stats: torch.Tensor, count: float, group=None):
 
 
 def enable_sync_batchnorm(model: torch.nn.Module, group=None) -> int:
-    """Give every fused BatchNorm holder of pasco_b200.net3d the process group (ME.MinkowskiSyncBatchNorm
-    .convert_sync_batchnorm equivalent for the engine-native model).  Returns the number of layers switched."""
-    from .net3d import BNorm
-    n = 0
-    g = group if group is not None else dist.group.WORLD
-    for m in model.modules():
-        if isinstance(m, BNorm):
-            m.group = g
-            n += 1
+    """Switch every MinkowskiBatchNorm of the model to MinkowskiSyncBatchNorm over `group` (None: the default group), in
+    place and with the same parameters and buffers.  Returns the number of layers switched."""
+    from .me import MinkowskiBatchNorm, MinkowskiSyncBatchNorm
+    n = sum(type(m) is MinkowskiBatchNorm for m in model.modules())
+    MinkowskiSyncBatchNorm.convert_sync_batchnorm(model, group)
     return n
 
 

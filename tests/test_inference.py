@@ -34,7 +34,8 @@ class _NoSplitLib:
 
 def test_routing_predicates(monkeypatch):
     """bn_act_conv: training → the fused BNActConv, eval + gradients → the differentiable row path (unchanged), eval
-    without gradients → the split fusion; ResBlock.infer_ok / the drop-in's deferred BatchNorm follow the same predicate."""
+    without gradients → the split fusion; ResBlock.infer_ok follows the same predicate, and a deferred MinkowskiBatchNorm
+    reaches its convolution through this route."""
     from pasco_b200 import ops
     monkeypatch.setattr(ops, "load", lambda: _NoSplitLib)
     bn = torch.nn.BatchNorm1d(64)
