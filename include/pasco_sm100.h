@@ -410,6 +410,51 @@ int pasco_eval_vox_dense(const int32_t* panoptic, const float* confidence, const
                          const int32_t* match, int32_t S, const float bounds[16], int32_t* cal, int32_t* bad,
                          double* sums, pasco_stream_t s);
 
+/* ---- training criterion of the reference's SetCriterion (criterion_sparse.py, matcher_sparse.py, helper.py:7-37,
+ *      lovasz.py:186-219) on one output level's rows; fp32, float sums in a fixed order ------------------------------
+ * Samples the T mask volumes masks uint8 [T][X·Y·Z], unknown uint8 [X·Y·Z] and (label != NULL) the class volume at
+ * the rows (b, x, y, z) of xyz int32 [n][4] with b = 0, at (x, y, z) − min_c (int32 [3], device); rows with b != 0 get
+ * no bit, flag or label and are not counted.  bits uint32 [n][max(1, ceil(T/32))], flags uint8 [n] (1: not
+ * unknown, 2: also at least one target bit), lab int32 [n] (−1 for 255).  stats int32 [T + 5], zeroed by the caller:
+ * per-target bit counts over the valid rows, the valid-row count, rows outside the volume or with a label outside
+ * [0, K) other than 255, two words of present-class bits, the known-row count.  1 <= K <= 64.                      */
+int pasco_setloss_sample(const int32_t* xyz, int64_t n, const int32_t* min_c, const uint8_t* masks, int32_t T,
+                         const uint8_t* unknown, const uint8_t* label, int32_t X, int32_t Y, int32_t Z, int32_t K,
+                         uint32_t* bits, uint8_t* flags, int32_t* lab, int32_t* stats, pasco_stream_t s);
+/* matcher_sparse.py:96-157: C fp32 [Q][T] from F fp32 [n][Q] read once over the valid rows, query_logits fp32 [Q][K1],
+ * target class ids int32 [T] and class_weight fp32 [K1]; the focal part is 0 without valid rows.                    */
+int pasco_setloss_match_cost(const float* F, int64_t n, int32_t Q, const uint32_t* bits, int32_t T,
+                             const uint8_t* flags, const int32_t* stats, const float* query_logits, int32_t K1,
+                             const int32_t* ids, const float* class_weight, float cost_mask, float cost_class,
+                             float cost_dice, float* C, pasco_stream_t s);
+/* criterion_sparse.py:83-112 over the known rows, per matched pair (query qi[k], target tj[k]): sums fp32 [P][4] =
+ * Σ focal(F, t), Σ σ(F)·t, Σ σ(F), Σ t.  The backward writes dL/dF of the pairs' columns from g fp32 [P][4] (the
+ * gradient of those sums) into gF fp32 [n][Q]; other columns are left as they are.                                 */
+int pasco_setloss_pair_sums(const float* F, int64_t n, int32_t Q, const uint32_t* bits, int32_t T,
+                            const uint8_t* flags, const int32_t* qi, const int32_t* tj, int32_t P, float* sums,
+                            pasco_stream_t s);
+int pasco_setloss_pair_backward(const float* F, int64_t n, int32_t Q, const uint32_t* bits, int32_t T,
+                                const uint8_t* flags, const int32_t* qi, const int32_t* tj, int32_t P, const float* g,
+                                float* gF, pasco_stream_t s);
+/* helper.py:7-37: out fp32 [n][K] = Σ_j a_nj · L[j], a_nj = (σ(F[n, keep[j]]) + 1e-8) normalised over the kq kept
+ * queries, L fp32 [kq][K].  The backward writes gF's kept columns and gL fp32 [kq][K] from g fp32 [n][K].
+ * 1 <= kq <= 128, 1 <= K <= 64.                                                                                    */
+int pasco_setloss_ssc_forward(const float* F, int64_t n, int32_t Q, const int32_t* keep, int32_t kq, const float* L,
+                              int32_t K, float* out, pasco_stream_t s);
+int pasco_setloss_ssc_backward(const float* F, int64_t n, int32_t Q, const int32_t* keep, int32_t kq, const float* L,
+                               int32_t K, const float* out, const float* g, float* gF, float* gL, pasco_stream_t s);
+/* lovasz.py:186-219 for every class at once.  labels int32 [P]: −1 leaves the row out, c in [0, C) is class c, >= C
+ * is background of every class.  errors: probs fp32 [P][C] = softmax, err fp32 [C][P] = |fg − p| (−1 for a row left
+ * out); the caller sorts each class's row descending (perm int64 [C][P]).  grad: lovasz_grad at every sorted
+ * position into grad fp32 [C][P] and loss fp32 [C] = Σ err·grad per class.  backward: dx fp32 [P][C] from g fp32 [C]
+ * = dL/dloss.  1 <= C <= 64.                                                                                       */
+int pasco_lovasz_errors(const float* logits, int64_t P, int32_t C, const int32_t* labels, float* probs, float* err,
+                        pasco_stream_t s);
+int pasco_lovasz_grad(const float* err_sorted, const int64_t* perm, const int32_t* labels, int64_t P, int32_t C,
+                      float* grad, float* loss, pasco_stream_t s);
+int pasco_lovasz_backward(const float* probs, const int32_t* labels, const int64_t* perm, const float* grad,
+                          const float* g, int64_t P, int32_t C, float* dx, pasco_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -85,6 +85,16 @@ PROTOTYPES = {
     "pasco_eval_pairs_dense": (C.c_int, [_p, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
     "pasco_eval_ssc_planes": (C.c_int, [_p, _i32, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "pasco_eval_vox_dense": (C.c_int, [_p, _p, _p, _i64, _p, _i32, _p, _p, _p, _p, _p]),
+    "pasco_setloss_sample": (C.c_int, [_p, _i64, _p, _p, _i32, _p, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
+    "pasco_setloss_match_cost": (C.c_int, [_p, _i64, _i32, _p, _i32, _p, _p, _p, _i32, _p, _p, C.c_float, C.c_float,
+                                           C.c_float, _p, _p]),
+    "pasco_setloss_pair_sums": (C.c_int, [_p, _i64, _i32, _p, _i32, _p, _p, _p, _i32, _p, _p]),
+    "pasco_setloss_pair_backward": (C.c_int, [_p, _i64, _i32, _p, _i32, _p, _p, _p, _i32, _p, _p, _p]),
+    "pasco_setloss_ssc_forward": (C.c_int, [_p, _i64, _i32, _p, _i32, _p, _i32, _p, _p]),
+    "pasco_setloss_ssc_backward": (C.c_int, [_p, _i64, _i32, _p, _i32, _p, _i32, _p, _p, _p, _p, _p]),
+    "pasco_lovasz_errors": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p]),
+    "pasco_lovasz_grad": (C.c_int, [_p, _p, _p, _i64, _i32, _p, _p, _p]),
+    "pasco_lovasz_backward": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i32, _p, _p]),
 }
 
 _lib: Optional[C.CDLL] = None

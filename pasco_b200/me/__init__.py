@@ -237,14 +237,15 @@ class TensorField:
 
 def _hook_groups(value: str) -> frozenset:
     """PASCO_B200_HOOKS: "0" / unset = none, "1" = the attention hooks, else a comma list of "attention", "postprocess",
-    "evaluate"."""
+    "evaluate", "criterion"."""
     if value in ("", "0"):
         return frozenset()
     if value == "1":
         return frozenset({"attention"})
     groups = frozenset(v.strip() for v in value.split(",") if v.strip())
-    if not groups <= {"attention", "postprocess", "evaluate"}:
-        raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of attention, postprocess, evaluate")
+    if not groups <= {"attention", "postprocess", "evaluate", "criterion"}:
+        raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of attention, postprocess, evaluate, "
+                         "criterion")
     return groups
 
 
@@ -252,7 +253,8 @@ _HOOK_GROUPS = _hook_groups(os.environ.get("PASCO_B200_HOOKS", "0"))
 _HOOKS_PENDING = bool(_HOOK_GROUPS)
 _HOOK_MODULES = {"attention": ("pasco.models.transformer.transformer_predictor_v2",),
                  "postprocess": ("pasco.models.ensembler", "pasco.models.helper"),    # either Net module imports both
-                 "evaluate": ("pasco.models.metrics",)}                               # ... and this one
+                 "evaluate": ("pasco.models.metrics",),                               # ... and this one
+                 "criterion": ("pasco.loss.criterion_sparse", "pasco.loss.losses")}   # ... and these
 
 
 def _maybe_install_hooks() -> None:
@@ -265,7 +267,7 @@ def _maybe_install_hooks() -> None:
         _HOOKS_PENDING = False
         from .. import hooks
         hooks.install(attention="attention" in _HOOK_GROUPS, postprocess="postprocess" in _HOOK_GROUPS,
-                      evaluate="evaluate" in _HOOK_GROUPS)
+                      evaluate="evaluate" in _HOOK_GROUPS, criterion="criterion" in _HOOK_GROUPS)
 
 
 class _LazyRows:

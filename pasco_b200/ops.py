@@ -1314,3 +1314,119 @@ def eval_vox_dense(pan: torch.Tensor, conf: torch.Tensor, gt_id: torch.Tensor, m
                          f"{tuple(pan.shape)} and {conf.dtype} {tuple(conf.shape)}")
     call("pasco_eval_vox_dense", ptr(pan), ptr(conf), ptr(gt_id), cells, ptr(match), match.shape[0] - 1, _bounds(),
          ptr(out[:32]), ptr(out[64:65]), ptr(out[32:64].view(torch.float64)))
+
+
+# ------------------------------------------------------------------------------------------------
+# training criterion of the reference's SetCriterion (csrc/setloss.cu)
+# ------------------------------------------------------------------------------------------------
+def setloss_sample(xyz: torch.Tensor, min_c: torch.Tensor, masks: torch.Tensor, unknown: torch.Tensor,
+                   label: Optional[torch.Tensor], K: int):
+    """xyz int32 [N, 4] (batch, x, y, z; rows of batch items other than 0 are left out), min_c int32 [3] (device), masks bool / uint8 [T, X, Y, Z], unknown bool [X, Y, Z], label
+    uint8 [X, Y, Z] or None → (bits int32 [N, max(1, ⌈T/32⌉)], flags uint8 [N], lab int32 [N] or None, stats int32
+    [T + 5]) in pasco_setloss_sample's layout."""
+    T, size = masks.shape[0], tuple(unknown.shape)
+    dev, N = xyz.device, xyz.shape[0]
+    W = max(1, (T + 31) // 32)
+    u8 = lambda t: (t.contiguous().view(torch.uint8) if t.dtype == torch.bool else t.to(torch.uint8).contiguous())  # noqa: E731
+    m8 = u8(masks.reshape(T, -1)) if T else torch.zeros(1, dtype=torch.uint8, device=dev)
+    bits = torch.empty(N, W, dtype=torch.int32, device=dev)
+    flags = torch.empty(N, dtype=torch.uint8, device=dev)
+    lab = torch.empty(N, dtype=torch.int32, device=dev) if label is not None else None
+    stats = torch.zeros(T + 5, dtype=torch.int32, device=dev)
+    call("pasco_setloss_sample", ptr(xyz), N, ptr(min_c), ptr(m8), T, ptr(u8(unknown)),
+         ptr(u8(label) if label is not None else None), *size, K, ptr(bits), ptr(flags), ptr(lab), ptr(stats))
+    return bits, flags, lab, stats
+
+
+def match_cost(F: torch.Tensor, bits: torch.Tensor, T: int, flags: torch.Tensor, stats: torch.Tensor,
+               query_logits: torch.Tensor, ids: torch.Tensor, class_weight: torch.Tensor, cost_mask: float,
+               cost_class: float, cost_dice: float) -> torch.Tensor:
+    """matcher_sparse.py:96-157 → C fp32 [Q, T].  F fp32 [N, Q]; query_logits fp32 [Q, K+1]; ids int32 [T]."""
+    Q = F.shape[1]
+    C_ = torch.empty(Q, T, dtype=torch.float32, device=F.device)
+    call("pasco_setloss_match_cost", ptr(F), F.shape[0], Q, ptr(bits), T, ptr(flags), ptr(stats),
+         ptr(query_logits), query_logits.shape[1], ptr(ids), ptr(class_weight), float(cost_mask), float(cost_class),
+         float(cost_dice), ptr(C_))
+    return C_
+
+
+class PairSums(torch.autograd.Function):
+    """criterion_sparse.py:83-112's sums over the known rows per matched pair (qi, tj int32 [P]) → fp32 [P, 4]:
+    Σ focal, Σ σ·t, Σ σ, Σ t.  Differentiable in F [N, Q]; only the pairs' columns get a gradient."""
+
+    @staticmethod
+    def forward(ctx, F, bits, T, flags, qi, tj):
+        F = F.detach().contiguous()
+        P = qi.shape[0]
+        out = torch.empty(P, 4, dtype=torch.float32, device=F.device)
+        call("pasco_setloss_pair_sums", ptr(F), F.shape[0], F.shape[1], ptr(bits), T, ptr(flags), ptr(qi), ptr(tj), P,
+             ptr(out))
+        ctx.save_for_backward(F, bits, flags, qi, tj)
+        ctx.T = T
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        F, bits, flags, qi, tj = ctx.saved_tensors
+        gF = torch.zeros_like(F)
+        call("pasco_setloss_pair_backward", ptr(F), F.shape[0], F.shape[1], ptr(bits), ctx.T, ptr(flags), ptr(qi),
+             ptr(tj), qi.shape[0], ptr(g.contiguous()), ptr(gF))
+        return gF, None, None, None, None, None
+
+
+class SscLogits(torch.autograd.Function):
+    """helper.py:7-37's voxel class logits: out [N, K] = normalised (σ(F[:, keep]) + 1e-8) @ L, L = query_logits[keep,
+    :-1] [kq, K].  Differentiable in F (kept columns) and L."""
+
+    @staticmethod
+    def forward(ctx, F, L, keep):
+        F, L = F.detach().contiguous(), L.detach().contiguous()
+        out = torch.empty(F.shape[0], L.shape[1], dtype=torch.float32, device=F.device)
+        call("pasco_setloss_ssc_forward", ptr(F), F.shape[0], F.shape[1], ptr(keep), keep.shape[0], ptr(L), L.shape[1],
+             ptr(out))
+        ctx.save_for_backward(F, L, keep, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        F, L, keep, out = ctx.saved_tensors
+        gF = torch.zeros_like(F)
+        gL = torch.empty_like(L)
+        call("pasco_setloss_ssc_backward", ptr(F), F.shape[0], F.shape[1], ptr(keep), keep.shape[0], ptr(L), L.shape[1],
+             ptr(out), ptr(g.contiguous()), ptr(gF), ptr(gL))
+        return gF, gL, None
+
+
+class LovaszClasses(torch.autograd.Function):
+    """lovasz.py:186-219's per-class term Σ err·lovasz_grad for every class at once → fp32 [C].  logits [P, C];
+    labels int32 [P] (−1: row left out, >= C: background of every class).  One batched sort of the [C, P] errors."""
+
+    @staticmethod
+    def forward(ctx, logits, labels):
+        x = logits.detach().contiguous()
+        P, C_ = x.shape
+        probs = torch.empty_like(x)
+        err = torch.empty(C_, P, dtype=torch.float32, device=x.device)
+        call("pasco_lovasz_errors", ptr(x), P, C_, ptr(labels), ptr(probs), ptr(err))
+        err_sorted, perm = torch.sort(err, dim=1, descending=True)
+        grad = torch.empty_like(err)
+        loss = torch.empty(C_, dtype=torch.float32, device=x.device)
+        call("pasco_lovasz_grad", ptr(err_sorted), ptr(perm), ptr(labels), P, C_, ptr(grad), ptr(loss))
+        ctx.save_for_backward(probs, labels, perm, grad)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        probs, labels, perm, grad = ctx.saved_tensors
+        dx = torch.empty_like(probs)
+        call("pasco_lovasz_backward", ptr(probs), ptr(labels), ptr(perm), ptr(grad), ptr(g.contiguous().float()),
+             probs.shape[0], probs.shape[1], ptr(dx))
+        return dx, None
+
+
+def lovasz_softmax(logits: torch.Tensor, labels: torch.Tensor, present: torch.Tensor) -> torch.Tensor:
+    """lovasz.py:186-219 with classes="present": the mean of LovaszClasses over the classes flagged in `present`
+    (bool [C], device; the present, non-ignored classes — at least one)."""
+    per = LovaszClasses.apply(logits.float(), labels)
+    w = present.to(per.dtype)
+    return (per * w).sum() / w.sum()
