@@ -455,6 +455,33 @@ int pasco_lovasz_grad(const float* err_sorted, const int64_t* perm, const int32_
 int pasco_lovasz_backward(const float* probs, const int32_t* labels, const int64_t* perm, const float* grad,
                           const float* g, int64_t P, int32_t C, float* dx, pasco_stream_t s);
 
+/* ---- point voxeliser grouping and the MIMO merge (csrc/voxel.cu); keys pack as the hash table's ---------------------
+ * voxel_group: torch.unique(rows, dim=0, return_inverse=True) for rows [n][4] (int32, or int64 when is_i64)
+ * (unet3d_sparse_v2.py:72-75).  Pass 1 inserts every row's key into table_keys (capacity, power of two >= 2n, filled
+ * with 0xFF bytes) and writes the U unique keys, unordered, to ukeys [n]; stats int32 [2], zeroed by the caller: U and
+ * an error flag (a component outside [-32768, 32767]; the other outputs are then undefined and _order must not run).
+ * _order sorts the keys, writes unique_rows [U][4] (the input's integer type) in ascending lexicographic order of the
+ * signed rows and inverse int64 [n]; table_vals int32 [capacity] is scratch.                                       */
+int pasco_voxel_group(const void* rows, int32_t is_i64, int64_t n, uint64_t* table_keys, int64_t capacity,
+                      uint64_t* ukeys, int32_t* stats, pasco_stream_t s);
+int pasco_voxel_group_order(const void* rows, int32_t is_i64, int64_t n, const uint64_t* table_keys,
+                            int32_t* table_vals, int64_t capacity, const uint64_t* ukeys, int64_t U, void* unique_rows,
+                            int64_t* inverse, pasco_stream_t s);
+/* Augmenter.merge (augmenter.py:13-27) without the dense volume.  coords int32 [n][4] (t, x, y, z) with t the subnet,
+ * F fp32 [n][f].  _cells inserts the (x, y, z) cells (table_vals int32 [capacity] zeroed by the caller) and writes the
+ * U cells that have a feature other than ±0 to ukeys [n], unordered; stats int32 [3], zeroed by the caller: U, the
+ * largest t, an error flag (t < 0 or x, y, z outside [-32768, 32767]; _forward must not run).  _forward writes
+ * out_coords int32 [U][4] = (0, x, y, z) in ascending (x, y, z) order, out_F fp32 [U][M·f] (subnet t's channels at
+ * t·f, 0 where t has no row; t < M) and row_of int32 [n] (the output row of each input row, −1 for a dropped cell).
+ * _backward: gin fp32 [n][f] = g [U][M·f] at the row's output row and channels, 0 for a dropped cell.            */
+int pasco_mimo_merge_cells(const int32_t* coords, const float* F, int64_t n, int32_t f, uint64_t* table_keys,
+                           int32_t* table_vals, int64_t capacity, uint64_t* ukeys, int32_t* stats, pasco_stream_t s);
+int pasco_mimo_merge_forward(const int32_t* coords, const float* F, int64_t n, int32_t f, int32_t M,
+                             const uint64_t* table_keys, int32_t* table_vals, int64_t capacity, const uint64_t* ukeys,
+                             int64_t U, int32_t* out_coords, float* out_F, int32_t* row_of, pasco_stream_t s);
+int pasco_mimo_merge_backward(const int32_t* coords, const int32_t* row_of, int64_t n, int32_t f, int32_t M,
+                              const float* g, float* gin, pasco_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

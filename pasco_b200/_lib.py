@@ -95,6 +95,11 @@ PROTOTYPES = {
     "pasco_lovasz_errors": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p]),
     "pasco_lovasz_grad": (C.c_int, [_p, _p, _p, _i64, _i32, _p, _p, _p]),
     "pasco_lovasz_backward": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i32, _p, _p]),
+    "pasco_voxel_group": (C.c_int, [_p, _i32, _i64, _p, _i64, _p, _p, _p]),
+    "pasco_voxel_group_order": (C.c_int, [_p, _i32, _i64, _p, _p, _i64, _p, _i64, _p, _p, _p]),
+    "pasco_mimo_merge_cells": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i64, _p, _p, _p]),
+    "pasco_mimo_merge_forward": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _i64, _p, _i64, _p, _p, _p, _p]),
+    "pasco_mimo_merge_backward": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _p]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -54,6 +54,18 @@ classes, labels beyond the volume, a pair without a present class and (KITTI-360
     PASCO_B200_HOOKS=1 python scripts/train.py ...              # compat/MinkowskiEngine calls install() lazily
     PASCO_B200_HOOKS=attention,postprocess,evaluate python scripts/eval.py ...
     PASCO_B200_HOOKS=attention,postprocess,evaluate,criterion python scripts/train.py ...
+    PASCO_B200_HOOKS=attention,postprocess,evaluate,criterion,trunk python scripts/train.py ...
+
+The trunk hook (install(trunk=True)) replaces three pieces of the reference's own trunk that run on every training step
+and test scene: `CylinderFeat.forward` (unet3d_sparse_v2.py:53-86: torch.unique(dim=0) over all points, a lexicographic
+row sort) groups the points with ops.voxel_group (a hash dedup, then a sort of the unique keys only); `Augmenter.merge`
+(augmenter.py:13-27: a dense fp32 [M, f, X, Y, Z] volume, copied by torch.cat and scanned by ME.to_sparse, forward and
+backward) runs as ops.mimo_merge on the rows; `UNet3DV2.dense_bottleneck` (unet3d_sparse_v2.py:182-214: 11 cuDNN Conv3d
++ BatchNorm3d) runs the reference's SPCDense3Dv2 as box-kernel sparse convolutions over the full stride-8 grid, the
+same implementation PascoNet.dense_bottleneck uses (net3d.bottleneck_on_grid).  Grouping and merge are exact; the
+bottleneck matches cuDNN's fp32 result within the convolutions' tolerance.  At most TRUNK_SYNCS host synchronisations
+per hooked call.  fea_compre, more than 8 subnets, batch size != 1, a dense3d other than (SPCDense3Dv2, Dropout3d), a
+Dropout3d with p > 0 in training, coordinates outside [-32768, 32767] and CPU tensors go to the saved originals.
 """
 from __future__ import annotations
 
@@ -662,9 +674,76 @@ _orig_compl = [None, None]      # the losses module's compute_sem_compl_loss / c
 
 
 # ------------------------------------------------------------------------------------------------
+# trunk: CylinderFeat.forward (unet3d_sparse_v2.py:53-86), Augmenter.merge (augmenter.py:13-27) and
+# UNet3DV2.dense_bottleneck (unet3d_sparse_v2.py:182-214) on csrc/voxel.cu and net3d's grid bottleneck
+# ------------------------------------------------------------------------------------------------
+TRUNK_SYNCS = 4     # host synchronisations of one hooked trunk call, at most (see each function)
+
+
+def _cylinder_forward(self, pt_fea, xy_ind):
+    """unet3d_sparse_v2.py:53-86 with torch.unique(dim=0) as ops.voxel_group and the scatter-max on
+    ops.scatter_max; the point MLP is the reference's own PPmodel.  The randperm is drawn but not applied: the CUDA
+    generator ends where the original leaves it, and the max does not depend on the point order (only the rounding of
+    the BatchNorm1d batch statistics does).  One host synchronisation (the voxel count)."""
+    if self.fea_compre is not None or not (pt_fea[0].is_cuda and xy_ind[0].is_cuda):
+        return self._pasco_b200_orig_forward(pt_fea, xy_ind)
+    cat_pt_ind = torch.cat([F.pad(xy_ind[b], (1, 0), "constant", value=b) for b in range(len(xy_ind))], dim=0)
+    if cat_pt_ind.dtype not in (torch.int32, torch.int64):
+        return self._pasco_b200_orig_forward(pt_fea, xy_ind)
+    grouped = ops.voxel_group(cat_pt_ind)
+    if grouped is None:                                # a coordinate the packed keys cannot hold
+        return self._pasco_b200_orig_forward(pt_fea, xy_ind)
+    torch.randperm(cat_pt_ind.shape[0], device=pt_fea[0].get_device())
+    unq, inv = grouped
+    processed = self.PPmodel(torch.cat(pt_fea, dim=0))
+    pooled = ops.scatter_max(processed, inv, dim=0, dim_size=unq.shape[0])[0]
+    return unq.to(torch.int64), pooled
+
+
+def _augmenter_merge(self, in_feat):
+    """augmenter.py:13-27 on ops.mimo_merge: no dense [M, f, X, Y, Z] volume and no host synchronisation for the
+    minimum coordinate; the same features, coordinates and input gradient bit for bit.  One host synchronisation
+    (the merged row count)."""
+    F_ = in_feat.F
+    if not F_.is_cuda:
+        return self._pasco_b200_orig_merge(in_feat)
+    merged = ops.mimo_merge(F_, in_feat.C)
+    if merged is None:                                 # more than 8 subnets, or coordinates the keys cannot hold
+        return self._pasco_b200_orig_merge(in_feat)
+    feats, coords = merged
+    cm = ME.CoordinateManager()                        # unique rows: register the map without the dedup pass
+    return ME.SparseTensor(feats, coordinate_map_key=cm._register(coords, 1), coordinate_manager=cm)
+
+
+def _dense_bottleneck(self, deepest_features, bs, global_min_coords, global_max_coords):
+    """unet3d_sparse_v2.py:182-214 on net3d's grid bottleneck: the stride-8 rows densified by rows, the reference's
+    SPCDense3Dv2 (dense3d[0]) as box-kernel sparse convolutions on the split-K path, the all-zero rows dropped as
+    ME.to_sparse drops them; a SparseTensor on deepest_features' coordinate manager in to_sparse's order.  Four host
+    synchronisations, whatever the row count: the grid origin and size, the grid offset's copy from pageable memory,
+    and the compaction's row count and error check (plus the kernel maps' construction on the first call at a grid
+    size, which net3d.bottleneck_grid caches)."""
+    from pasco.models.layers import SPCDense3Dv2
+    from pasco.models.unet3d_sparse_v2 import compute_scene_size
+    from .net3d import bottleneck_on_grid
+    d = self.dense3d
+    F_ = deepest_features.F
+    if (bs != 1 or not F_.is_cuda or len(d) != 2 or type(d[0]) is not SPCDense3Dv2
+            or type(d[1]) is not torch.nn.Dropout3d or (d[1].training and d[1].p > 0)):
+        return self._pasco_b200_orig_dense_bottleneck(deepest_features, bs, global_min_coords, global_max_coords)
+    scale = deepest_features.tensor_stride[0]
+    C_ = deepest_features.C
+    gmin = torch.as_tensor(global_min_coords).to(C_.device)
+    gmax = torch.max(torch.as_tensor(global_max_coords).to(C_.device), C_[:, 1:].max(dim=0)[0].int())
+    scene_size = compute_scene_size(gmin, gmax, scale) // scale
+    host = torch.cat([gmin.reshape(3).long(), scene_size.reshape(3).long()]).tolist()       # sync 1
+    y, coords = bottleneck_on_grid(d[0], self, F_, C_, scale, host[:3], host[3:])          # syncs 2, 3
+    return ME.SparseTensor(y, coords, tensor_stride=scale, coordinate_manager=deepest_features.coordinate_manager)
+
+
+# ------------------------------------------------------------------------------------------------
 # install / uninstall
 # ------------------------------------------------------------------------------------------------
-_installed = set()     # "attention", "postprocess", "evaluate", "criterion"
+_installed = set()     # "attention", "postprocess", "evaluate", "criterion", "trunk"
 
 
 def _install_attention() -> bool:
@@ -762,16 +841,34 @@ def _install_criterion() -> bool:
     return True
 
 
-def install(attention: bool = True, postprocess: bool = False, evaluate: bool = False, criterion: bool = False) -> bool:
+def _install_trunk() -> bool:
+    try:
+        from pasco.models.augmenter import Augmenter
+        from pasco.models.unet3d_sparse_v2 import CylinderFeat, UNet3DV2
+    except Exception:
+        return False
+    CylinderFeat._pasco_b200_orig_forward = CylinderFeat.forward
+    CylinderFeat.forward = _cylinder_forward
+    Augmenter._pasco_b200_orig_merge = Augmenter.merge
+    Augmenter.merge = _augmenter_merge
+    UNet3DV2._pasco_b200_orig_dense_bottleneck = UNet3DV2.dense_bottleneck
+    UNet3DV2.dense_bottleneck = _dense_bottleneck
+    return True
+
+
+def install(attention: bool = True, postprocess: bool = False, evaluate: bool = False, criterion: bool = False,
+            trunk: bool = False) -> bool:
     """Patch the reference (idempotent per group).  attention: TransformerPredictorV2.forward with its masks as
     bit rows, and the cross-attention layer that takes them; postprocess: the
     Ensembler and panoptic_inference; evaluate: Net.evaluate_all of both Net modules; criterion:
-    SetCriterion.compute_losses and the completion losses both Net modules import.  Returns False when a requested
-    group's `pasco` modules are not importable."""
+    SetCriterion.compute_losses and the completion losses both Net modules import; trunk: CylinderFeat.forward,
+    Augmenter.merge and UNet3DV2.dense_bottleneck.  Returns False when a requested group's `pasco` modules are not
+    importable."""
     for name, wanted, fn in (("attention", attention, _install_attention),
                              ("postprocess", postprocess, _install_postprocess),
                              ("evaluate", evaluate, _install_evaluate),
-                             ("criterion", criterion, _install_criterion)):
+                             ("criterion", criterion, _install_criterion),
+                             ("trunk", trunk, _install_trunk)):
         if wanted and name not in _installed:
             if not fn():
                 return False
@@ -800,4 +897,10 @@ def uninstall() -> None:
         SetCriterion.compute_losses = SetCriterion._pasco_b200_orig_compute_losses
         for mod, name in _crit_users():
             setattr(mod, name, getattr(mod, "_pasco_b200_orig_" + name))
+    if "trunk" in _installed:
+        from pasco.models.augmenter import Augmenter
+        from pasco.models.unet3d_sparse_v2 import CylinderFeat, UNet3DV2
+        CylinderFeat.forward = CylinderFeat._pasco_b200_orig_forward
+        Augmenter.merge = Augmenter._pasco_b200_orig_merge
+        UNet3DV2.dense_bottleneck = UNet3DV2._pasco_b200_orig_dense_bottleneck
     _installed.clear()

@@ -637,6 +637,88 @@ def scatter_max(src: torch.Tensor, index: torch.Tensor, dim: int = 0, out=None, 
 
 
 # ----------------------------------------------------------------------------------------------
+# point voxeliser grouping and the MIMO merge (csrc/voxel.cu)
+# ----------------------------------------------------------------------------------------------
+def voxel_group(rows: torch.Tensor) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
+    """torch.unique(rows, dim=0, return_inverse=True) for int32 / int64 (b, x, y, z) rows [P, 4], bit for bit: (unique
+    rows [U, 4] of rows' dtype in ascending lexicographic order, int64 inverse [P]).  None when a component lies
+    outside [-32768, 32767] (the packed keys cannot hold it).  One host synchronisation (U and the range flag)."""
+    if rows.dtype not in (torch.int32, torch.int64) or rows.ndim != 2 or rows.shape[1] != 4:
+        raise ValueError("voxel_group takes int32 or int64 [P, 4] rows")
+    rows = rows.contiguous()
+    n, dev, is64 = rows.shape[0], rows.device, int(rows.dtype == torch.int64)
+    if n == 0:
+        return rows.new_zeros(0, 4), torch.zeros(0, dtype=torch.int64, device=dev)
+    cap = _capacity(n)
+    keys = torch.full((cap,), -1, dtype=torch.int64, device=dev)
+    ukeys = torch.empty(n, dtype=torch.int64, device=dev)
+    stats = torch.zeros(2, dtype=torch.int32, device=dev)
+    call("pasco_voxel_group", ptr(rows), is64, n, ptr(keys), cap, ptr(ukeys), ptr(stats))
+    U, bad = stats.tolist()
+    if bad:
+        return None
+    vals = torch.empty(cap, dtype=torch.int32, device=dev)
+    unq = torch.empty(U, 4, dtype=rows.dtype, device=dev)
+    inv = torch.empty(n, dtype=torch.int64, device=dev)
+    call("pasco_voxel_group_order", ptr(rows), is64, n, ptr(keys), ptr(vals), cap, ptr(ukeys), U, ptr(unq), ptr(inv))
+    return unq, inv
+
+
+class MimoMerge(torch.autograd.Function):
+    """Augmenter.merge on the cells of pasco_mimo_merge_cells: (features [U, M·f], coordinates [U, 4]); the backward
+    gathers the features' gradient back to the input rows."""
+
+    @staticmethod
+    def forward(ctx, F, coords, M, cells):
+        keys, vals, cap, ukeys, U = cells
+        n, f = F.shape
+        out_c = torch.empty(U, 4, dtype=torch.int32, device=F.device)
+        out = torch.empty(U, M * f, dtype=torch.float32, device=F.device)
+        row_of = torch.empty(n, dtype=torch.int32, device=F.device)
+        call("pasco_mimo_merge_forward", ptr(coords), ptr(F), n, f, M, ptr(keys), ptr(vals), cap, ptr(ukeys), U,
+             ptr(out_c), ptr(out), ptr(row_of))
+        ctx.save_for_backward(coords, row_of)
+        ctx.M = M
+        ctx.mark_non_differentiable(out_c)
+        return out, out_c
+
+    @staticmethod
+    def backward(ctx, g, _):
+        coords, row_of = ctx.saved_tensors
+        n = coords.shape[0]
+        f = g.shape[1] // ctx.M
+        gin = torch.empty(n, f, dtype=torch.float32, device=g.device)
+        call("pasco_mimo_merge_backward", ptr(coords), ptr(row_of), n, f, ctx.M, ptr(g.contiguous().float()), ptr(gin))
+        return gin, None, None, None
+
+
+def mimo_merge(F: torch.Tensor, coords: torch.Tensor, max_subnets: int = 8):
+    """Augmenter.merge (augmenter.py:13-27) on the rows, without the dense volume: F fp32 [n, f], coords int [n, 4] with
+    the subnet index t in the batch column → (features [U, M·f] with subnet t's channels at t·f, int32 coordinates
+    [U, 4] = (0, x, y, z)), M = largest t + 1, the cells in ascending (x, y, z) order, cells whose M·f features are all
+    ±0 dropped as ME.to_sparse drops them.  Bit-identical to the dense path, forward and backward.  None for more than
+    `max_subnets` subnets, a negative t or a coordinate outside [-32768, 32767].  One host synchronisation (U, M and
+    the range flag); none for the minimum coordinate."""
+    coords = _i32(coords).contiguous()
+    n, f, dev = F.shape[0], F.shape[1], F.device
+    if n == 0:
+        return None
+    Fc = F.contiguous().float()
+    cap = _capacity(n)
+    keys = torch.full((cap,), -1, dtype=torch.int64, device=dev)
+    vals = torch.zeros(cap, dtype=torch.int32, device=dev)
+    ukeys = torch.empty(n, dtype=torch.int64, device=dev)
+    stats = torch.zeros(3, dtype=torch.int32, device=dev)
+    call("pasco_mimo_merge_cells", ptr(coords), ptr(Fc.detach()), n, f, ptr(keys), ptr(vals), cap, ptr(ukeys),
+         ptr(stats))
+    U, top, bad = stats.tolist()
+    M = top + 1
+    if bad or M > max_subnets:
+        return None
+    return MimoMerge.apply(Fc, coords, M, (keys, vals, cap, ukeys, U))
+
+
+# ----------------------------------------------------------------------------------------------
 # fused BatchNorm (+ activation) over rows
 # ----------------------------------------------------------------------------------------------
 def column_stats(x: torch.Tensor) -> torch.Tensor:
