@@ -482,6 +482,30 @@ int pasco_mimo_merge_forward(const int32_t* coords, const float* F, int64_t n, i
 int pasco_mimo_merge_backward(const int32_t* coords, const int32_t* row_of, int64_t n, int32_t f, int32_t M,
                               const float* g, float* gin, pasco_stream_t s);
 
+/* ---- the reference decoder's glue (csrc/decoder.cu; decoder_v3.py) -------------------------------------------------
+ * completion_rows: probs = host array of M (<= 8) device pointers to fp32 softmax rows [n][K] (K <= 64).  Writes
+ * cls int32 [M][n] (torch's max(-1) index: the first maximal value, a NaN at its first index), keep uint8 [M][n] =
+ * cls != 0, votes int32 [n] = sum over m of keep, and with w fp32 [K] (may be null) weight fp32 [M][n] = p_max * w[cls]
+ * as one fp32 multiply.  counts int32 [3M + 1], zeroed by the caller: kept rows per subnet, labelled cells per subnet
+ * ((label != 0) & (label != 255) over labels = host array of M device volumes of n_label signed integers of
+ * label_bytes bytes; may be null), rows whose weight is not a finite value >= 0 per subnet, rows with a vote.
+ * topk_mask: keep uint8 [n] = the k largest w / q (IEEE fp32 division, w / q >= 0, not NaN), ties at the k-th value
+ * taken by lowest row: torch.multinomial(w, k, replacement=False)'s set when q is its Exp(1) draw.
+ * panop_crop: mask uint8 [n] = argmax(logits row) != 0 AND min <= (x, y, z) <= max with box int32 [6] = (min, max);
+ * counts int32 [2], zeroed by the caller: rows with argmax != 0, rows kept.  With no argmax != 0, the first 1000 rows
+ * inside the box are kept (decoder_v3.py:415-417).
+ * mimo_batch: feats / coords = host arrays of M device pointers to fp32 [len_m][C] / int32 [len_m][4], len_m <= L.
+ * out_F fp32 [M][L][C] and out_C int32 [M][L][4] zero-padded; keep_pad uint8 [M][L] (may be null) = any feature or
+ * coordinate of the padded row != 0.                                                                             */
+int pasco_completion_rows(const float* const* probs, int32_t M, int64_t n, int32_t K, const float* w,
+                          const void* const* labels, int64_t n_label, int32_t label_bytes, int32_t* cls, uint8_t* keep,
+                          float* weight, int32_t* votes, int32_t* counts, pasco_stream_t s);
+int pasco_topk_mask(const float* w, const float* q, int64_t n, int64_t k, uint8_t* keep, pasco_stream_t s);
+int pasco_panop_crop(const float* logits, int64_t n, int32_t K, const int32_t* coords, const int32_t* box,
+                     uint8_t* mask, int32_t* counts, pasco_stream_t s);
+int pasco_mimo_batch(const float* const* feats, const int32_t* const* coords, const int64_t* lengths, int32_t M,
+                     int64_t L, int32_t C, float* out_F, int32_t* out_C, uint8_t* keep_pad, pasco_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -100,6 +100,10 @@ PROTOTYPES = {
     "pasco_mimo_merge_cells": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i64, _p, _p, _p]),
     "pasco_mimo_merge_forward": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _i64, _p, _i64, _p, _p, _p, _p]),
     "pasco_mimo_merge_backward": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _p]),
+    "pasco_completion_rows": (C.c_int, [_p, _i32, _i64, _i32, _p, _p, _i64, _i32, _p, _p, _p, _p, _p, _p]),
+    "pasco_topk_mask": (C.c_int, [_p, _p, _i64, _i64, _p, _p]),
+    "pasco_panop_crop": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p]),
+    "pasco_mimo_batch": (C.c_int, [_p, _p, _p, _i32, _i64, _i32, _p, _p, _p, _p]),
 }
 
 _lib: Optional[C.CDLL] = None

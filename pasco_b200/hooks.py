@@ -66,9 +66,24 @@ same implementation PascoNet.dense_bottleneck uses (net3d.bottleneck_on_grid).  
 bottleneck matches cuDNN's fp32 result within the convolutions' tolerance.  At most TRUNK_SYNCS host synchronisations
 per hooked call.  fea_compre, more than 8 subnets, batch size != 1, a dense3d other than (SPCDense3Dv2, Dropout3d), a
 Dropout3d with p > 0 in training, coordinates outside [-32768, 32767] and CPU tensors go to the saved originals.
+
+The decoder hook (install(decoder=True)) replaces the glue between the decoder's convolutions, run at every scale and for
+every subnet: `DecoderBlock.forward` (decoder_v3.py:148-172) runs `resize` through net3d.resize_rows, the function
+PascoNet's decoder stages call (no (C+3)-channel concatenation, the C feature channels on the tensor-core GEMM);
+`predict_completion_sem_logit` (:319-394) makes one pasco_completion_rows pass for the argmax, keep masks, cap weights and
+counts, read on the host once, and its training cap draws torch.multinomial's Exp(1) variates itself and keeps the k
+largest w / q with pasco_topk_mask instead of a full sort (the same rows unless the threshold value occurs twice, the
+same generator state); `forward` (:453-511) prunes x and the M logits once per scale; `predict_panop` (:396-451) crops
+every subnet and scale with one pasco_panop_crop mask and one compaction, and builds the padded batches and keep_pad
+with pasco_mimo_batch on the device, then calls the reference's own transformer_predictor with the original's inputs.
+The log lines keep their text.  At most DECODER_SYNCS host synchronisations of the hooks' own per call.  CPU tensors,
+more than 8 subnets or 64 classes, logits other than fp32, a resize other than (BatchNorm(C+3), 1x1 convolution), C not
+a multiple of 64 in training, a process with an active dropout, bounds that are not 3 integers and logits on another
+coordinate map than x go to the saved originals.
 """
 from __future__ import annotations
 
+import collections
 import importlib
 import time
 
@@ -741,9 +756,238 @@ def _dense_bottleneck(self, deepest_features, bs, global_min_coords, global_max_
 
 
 # ------------------------------------------------------------------------------------------------
+# decoder: DecoderBlock.forward (decoder_v3.py:148-172) and DecoderGenerativeSepConvV2's predict_completion_sem_logit
+# (:319-394), predict_panop (:396-451) and forward (:453-511) on csrc/decoder.cu and net3d.resize_rows
+# ------------------------------------------------------------------------------------------------
+DECODER_SYNCS = 3   # host synchronisations of the hooks' own code in one hooked call, at most (see each function); the
+                    # reference submodules a hook runs (upsample, process, completion heads, voxel_feats, the
+                    # transformer) make their own
+
+
+def _as_printed(v: int, dev) -> str:
+    """How print() shows the reference's 0-dim int64 count on `dev`: its log lines keep their text."""
+    return f"tensor({int(v)}, device='{dev}')"
+
+
+def _resize_channels(resize):
+    """C when resize == (MinkowskiBatchNorm(C+3), MinkowskiConvolution(C+3, C, kernel_size=1)), the pair resize_rows
+    takes; else None."""
+    if not (isinstance(resize, torch.nn.Sequential) and len(resize) == 2):
+        return None
+    bn, conv = resize[0], resize[1]
+    if not (type(conv) is ME.MinkowskiConvolution and conv.use_mm and isinstance(bn, ME.MinkowskiBatchNorm)):
+        return None
+    C = conv.out_channels
+    ok = (bn.bn.num_features == C + 3 and bn.bn.affine and bn.bn.running_mean is not None and conv.in_channels == C + 3)
+    return C if ok else None
+
+
+def _dropout_active(module) -> bool:
+    return any(isinstance(m, torch.nn.modules.dropout._DropoutNd) and m.training and m.p > 0
+               for m in module.modules())
+
+
+def _decoder_block_forward(self, x, shortcut, global_min_coords, global_max_coords):
+    """decoder_v3.py:148-172 with `resize` as net3d.resize_rows, the function PascoNet's decoder stages call: the split
+    BatchNorm, the C feature channels on ops.linear's tensor-core GEMM and the 3 coordinate channels as a rank-3
+    update, without concat_coords' (C+3)-channel copy and its new coordinate map.  Host synchronisations of its own:
+    the box prune's row count and the shortcut union's."""
+    from .net3d import resize_rows
+    C = _resize_channels(self.resize)
+    if (not x.F.is_cuda or C is None or _dropout_active(self.process)
+            or (self.resize[0].bn.training and C % 64 != 0)):
+        return self._pasco_b200_orig_forward(x, shortcut, global_min_coords, global_max_coords)
+    dec = self.upsample(x)
+    c = dec.C
+    keep = ((c[:, 1] >= global_min_coords[0]) & (c[:, 1] <= global_max_coords[0])
+            & (c[:, 2] >= global_min_coords[1]) & (c[:, 2] <= global_max_coords[1])
+            & (c[:, 3] >= global_min_coords[2]) & (c[:, 3] <= global_max_coords[2]))
+    dec = self.pruning(dec, keep)
+    coords = dec.C[:, 1:].float() / dec.tensor_stride[0]
+    y = resize_rows(self.resize[0], self.resize[1], dec.F, coords)
+    dec = ME.SparseTensor(y, coordinate_map_key=dec.coordinate_map_key, coordinate_manager=dec.coordinate_manager)
+    x = self.process(dec + shortcut)
+    return x, [self.completion_heads[str(i)](x) for i in range(self.n_heads)]
+
+
+def _label_weights(class_frequencies, scale, dev) -> torch.Tensor:
+    """decoder_v3.py:353-362: the cap's class weights, float64 on the host, rounded to fp32 as type_as does, moved
+    through pinned memory."""
+    fr = class_frequencies["1_{}".format(scale)]
+    w = fr / np.sum(fr)
+    w = np.power(np.amax(w) / w, 1 / 3.0)
+    return _on(torch.from_numpy(np.asarray(w)).float(), dev)
+
+
+_LABEL_DTYPES = (torch.bool, torch.uint8, torch.int16, torch.int32, torch.int64)
+
+
+def _completion_keep(self, scale, sem_logits, class_frequencies, sem_labels, test):
+    """predict_completion_sem_logit on pasco_completion_rows and pasco_topk_mask → the keep mask, or None where the saved
+    original decides.  One host synchronisation (every subnet's kept and labelled counts and the rows with a vote),
+    and a second one only when a subnet was capped and M >= 3 (the kept union's size)."""
+    M = self.n_infers
+    if sem_labels is None or not 1 <= M <= 8 or len(sem_logits) < M:
+        return None
+    Fs = [sem_logits[m].F for m in range(M)]
+    n, K = Fs[0].shape
+    dev = Fs[0].device
+    if not (all(f.is_cuda and f.dtype == torch.float32 and f.shape == Fs[0].shape for f in Fs) and 1 <= K <= 64):
+        return None
+    try:
+        labels = [sem_labels["1_{}".format(scale)][m] for m in range(M)]
+        w = None if test else _label_weights(class_frequencies, scale, dev)
+    except Exception:
+        return None                                   # the original raises where it reads them
+    if not all(torch.is_tensor(t) and t.device == dev and t.dtype == labels[0].dtype and t.numel() == labels[0].numel()
+               for t in labels) or labels[0].dtype not in _LABEL_DTYPES:
+        return None
+    probs = [F.softmax(f, dim=-1) for f in Fs]
+    _, keep, weight, votes, counts = ops.completion_rows(probs, w, [t.view(torch.uint8) if t.dtype == torch.bool
+                                                                   else t for t in labels])
+    h = counts.tolist()                                                                      # sync 1
+    kept, labelled, bad, n_voted = h[:M], h[M:2 * M], h[2 * M:3 * M], h[3 * M]
+    capped = False
+    for m in range(M):
+        n_m = kept[m]
+        if not test and n_m > self.occ_thres[scale] and ((self.training and M <= 2) or M > 3 or n_m > 500000):
+            k = int(self.occ_thres[scale])
+            if bad[m]:                                # a NaN, inf or negative weight: torch.multinomial's own error
+                torch.multinomial(weight[m], k, replacement=False)
+            q = torch.empty_like(weight[m]).exponential_(1)       # the draw torch.multinomial makes, same generator
+            ops.topk_mask(weight[m], q, k, out=keep[m])
+            print("Scale {}, infer {}: ".format(scale, m), _as_printed(n_m, dev), _as_printed(k, dev),
+                  _as_printed(labelled[m], dev))
+            capped = True
+    if capped:
+        votes = keep.sum(0)
+    out = votes > 0
+    thres = self.agg_occ_thres[scale]
+    if M >= 3 and not test:
+        n_keep = int(out.sum()) if capped else n_voted                                       # sync 2 when capped
+        if n_keep <= 2 or n_keep > thres:
+            top = torch.topk(votes.long(), k=thres, dim=0)[1]      # massive ties: torch's own tie order, as the original
+            out = torch.zeros_like(out).index_fill_(0, top, True)     # `keep[top] = True` without its host copy
+            print("Overall keep", _as_printed(n_keep, dev), "after", _as_printed(top.numel(), dev))
+    return out
+
+
+def _predict_completion_sem_logit(self, x, scale, sem_logits, scene_size, min_Cs, max_Cs, class_frequencies,
+                                  sem_labels=None, test=False):
+    """decoder_v3.py:319-394 without its host reads per subnet, its sorted top-k of the cap and its log lines' device
+    tensors: the same keep mask and the same printed lines."""
+    keep = _completion_keep(self, scale, sem_logits, class_frequencies, sem_labels, test)
+    if keep is None:
+        return self._pasco_b200_orig_predict_completion_sem_logit(x, scale, sem_logits, scene_size, min_Cs, max_Cs,
+                                                                  class_frequencies, sem_labels=sem_labels, test=test)
+    return keep
+
+
+def _box_on(lo, hi, dev) -> torch.Tensor:
+    """int32 [6] = (min_C, max_C) on `dev` without a blocking copy, or None for bounds that are not 3 integers."""
+    lo, hi = torch.as_tensor(lo), torch.as_tensor(hi)
+    if lo.numel() != 3 or hi.numel() != 3 or lo.dtype.is_floating_point or hi.dtype.is_floating_point:
+        return None
+    return torch.cat([_on(lo, dev).reshape(3), _on(hi, dev).reshape(3)]).to(torch.int32)
+
+
+def _predict_panop(self, xs, sem_logits_at_scales, Ts, min_Cs, max_Cs, sem_labels):
+    """decoder_v3.py:396-451: every (subnet, scale) crop as one pasco_panop_crop mask and one compaction that serves the
+    features and the scale-1 logits, the reference's voxel_feats, pasco_mimo_batch for the padded batches and keep_pad,
+    then the reference's transformer_predictor with the original's inputs.  One host synchronisation of its own: all
+    crops' counts at once."""
+    M = self.n_infers
+    args = (xs, sem_logits_at_scales, Ts, min_Cs, max_Cs, sem_labels)
+    if sem_labels is None or not 1 <= M <= 8 or 1 not in xs:
+        return self._pasco_b200_orig_predict_panop(*args)
+    try:
+        for m in range(M):
+            for s in xs:
+                sem_labels["1_{}".format(s)][m]
+    except Exception:
+        return self._pasco_b200_orig_predict_panop(*args)
+    dev = xs[1].F.device
+    boxes = [_box_on(min_Cs[m], max_Cs[m], dev) for m in range(M)] if dev.type == "cuda" else [None]
+    ok = all(b is not None for b in boxes)
+    for s, x in xs.items():
+        for m in range(M):
+            lg = sem_logits_at_scales[s][m]
+            ok = ok and (x.F.is_cuda and x.F.device == dev and lg.F.dtype == torch.float32 and lg.F.device == dev
+                         and 1 <= lg.F.shape[1] <= 64 and lg.F.shape[0] == x.F.shape[0]
+                         and lg.coordinate_map_key == x.coordinate_map_key)
+    if not ok:
+        return self._pasco_b200_orig_predict_panop(*args)
+    scales = list(xs)
+    counts = torch.zeros(M, len(scales), 2, dtype=torch.int32, device=dev)
+    masks = {(m, s): ops.panop_crop(sem_logits_at_scales[s][m].F, xs[s].C, boxes[m], counts[m, j])
+             for m in range(M) for j, s in enumerate(scales)}
+    h = counts.tolist()                                                                      # the one sync
+    xs_infers = collections.defaultdict(list)
+    sem_logits_pruneds = []
+    for m in range(M):
+        for j, s in enumerate(scales):
+            n_cls, n_keep = h[m][j]
+            if n_cls == 0:
+                print("line 367: keep.sum() == 0")
+            x = xs[s]
+            cm = x.coordinate_manager
+            kept, _, _ = ops.compact(masks[m, s], n_keep)
+            key = cm._register(ops.gather_coords(x.C, kept), x.coordinate_map_key.tensor_stride)
+            if s == 1:
+                sem_logits_pruneds.append(ME.SparseTensor(ops.GatherRows.apply(sem_logits_at_scales[s][m].F.float(), kept),
+                                                          coordinate_map_key=key, coordinate_manager=cm))
+            pruned = ME.SparseTensor(ops.GatherRows.apply(x.F.float(), kept), coordinate_map_key=key,
+                                     coordinate_manager=cm)
+            xs_infers[s].append(self.voxel_feats["scale{}_infer{}".format(s, m)](pruned))
+    for s in xs_infers:
+        xs_infers[s] = ops.mimo_batch([t.F for t in xs_infers[s]], [t.C for t in xs_infers[s]])[:2]
+    batch_F, batch_C, keep_pad = ops.mimo_batch([t.F for t in sem_logits_pruneds], [t.C for t in sem_logits_pruneds],
+                                                keep_pad=True)
+    panop_predictions = self.transformer_predictor(xs_infers, (batch_F, batch_C), min_Cs, max_Cs, keep_pad)
+    return panop_predictions, sem_logits_pruneds
+
+
+def _decoder_forward(self, x, features, global_min_coords, global_max_coords, min_Cs, max_Cs, class_frequencies, Ts,
+                     is_predict_panop=True, sem_labels=None, test=False):
+    """decoder_v3.py:453-511 with lines 496-497 as one prune of x and the M logits (net3d.prune_many: one compaction,
+    one host synchronisation and one coordinate map per scale where the original makes M + 1).  The pruned tensors
+    share that map; their coordinates are identical anyway."""
+    from pasco.models import decoder_v3
+    from .net3d import prune_many
+    if not x.F.is_cuda:
+        return self._pasco_b200_orig_forward(x, features, global_min_coords, global_max_coords, min_Cs, max_Cs,
+                                             class_frequencies, Ts, is_predict_panop=is_predict_panop,
+                                             sem_labels=sem_labels, test=test)
+    features = features[::-1]
+    sem_logits_at_scales, xs = {}, {}
+    for i in range(len(self.dec_blocks)):
+        scale = 2 ** (len(self.dec_blocks) - 1 - i)
+        x, sem_logits = self.dec_blocks[i](x, features[i], global_min_coords, global_max_coords)
+        if scale in [4, 2, 1]:
+            scene_size = decoder_v3.compute_scene_size(global_min_coords, global_max_coords)
+            keep = self.predict_completion_sem_logit(x, scale, sem_logits, scene_size, min_Cs, max_Cs,
+                                                     class_frequencies=class_frequencies, sem_labels=sem_labels,
+                                                     test=test)
+            if all(c.coordinate_map_key == x.coordinate_map_key and c.F.shape[0] == x.F.shape[0] for c in sem_logits):
+                x, sem_logits = prune_many([x] + list(sem_logits), keep)                     # one sync
+            else:
+                x = self.pruning(x, keep)
+                sem_logits = [self.pruning(c, keep) for c in sem_logits]
+            xs[scale] = x
+            sem_logits_at_scales[scale] = sem_logits
+    ret = {"sem_logits_at_scales": sem_logits_at_scales}
+    if is_predict_panop:
+        panop_predictions, sem_logits_pruneds = self.predict_panop(xs, sem_logits_at_scales, Ts, min_Cs, max_Cs,
+                                                                   sem_labels)
+        ret["panop_predictions"] = panop_predictions
+        ret["sem_logits_pruneds"] = sem_logits_pruneds
+    return ret
+
+
+# ------------------------------------------------------------------------------------------------
 # install / uninstall
 # ------------------------------------------------------------------------------------------------
-_installed = set()     # "attention", "postprocess", "evaluate", "criterion", "trunk"
+_installed = set()     # "attention", "postprocess", "evaluate", "criterion", "trunk", "decoder"
 
 
 def _install_attention() -> bool:
@@ -856,19 +1100,39 @@ def _install_trunk() -> bool:
     return True
 
 
+_DECODER_PATCHES = (("DecoderBlock", "forward", _decoder_block_forward),
+                    ("DecoderGenerativeSepConvV2", "predict_completion_sem_logit", _predict_completion_sem_logit),
+                    ("DecoderGenerativeSepConvV2", "predict_panop", _predict_panop),
+                    ("DecoderGenerativeSepConvV2", "forward", _decoder_forward))
+
+
+def _install_decoder() -> bool:
+    try:
+        from pasco.models import decoder_v3
+    except Exception:
+        return False
+    for cls, name, fn in _DECODER_PATCHES:
+        c = getattr(decoder_v3, cls)
+        setattr(c, "_pasco_b200_orig_" + name, getattr(c, name))
+        setattr(c, name, fn)
+    return True
+
+
 def install(attention: bool = True, postprocess: bool = False, evaluate: bool = False, criterion: bool = False,
-            trunk: bool = False) -> bool:
+            trunk: bool = False, decoder: bool = False) -> bool:
     """Patch the reference (idempotent per group).  attention: TransformerPredictorV2.forward with its masks as
     bit rows, and the cross-attention layer that takes them; postprocess: the
     Ensembler and panoptic_inference; evaluate: Net.evaluate_all of both Net modules; criterion:
     SetCriterion.compute_losses and the completion losses both Net modules import; trunk: CylinderFeat.forward,
-    Augmenter.merge and UNet3DV2.dense_bottleneck.  Returns False when a requested group's `pasco` modules are not
-    importable."""
+    Augmenter.merge and UNet3DV2.dense_bottleneck; decoder: DecoderBlock.forward and DecoderGenerativeSepConvV2's
+    forward, predict_completion_sem_logit and predict_panop.  Returns False when a requested group's `pasco` modules
+    are not importable."""
     for name, wanted, fn in (("attention", attention, _install_attention),
                              ("postprocess", postprocess, _install_postprocess),
                              ("evaluate", evaluate, _install_evaluate),
                              ("criterion", criterion, _install_criterion),
-                             ("trunk", trunk, _install_trunk)):
+                             ("trunk", trunk, _install_trunk),
+                             ("decoder", decoder, _install_decoder)):
         if wanted and name not in _installed:
             if not fn():
                 return False
@@ -903,4 +1167,9 @@ def uninstall() -> None:
         CylinderFeat.forward = CylinderFeat._pasco_b200_orig_forward
         Augmenter.merge = Augmenter._pasco_b200_orig_merge
         UNet3DV2.dense_bottleneck = UNet3DV2._pasco_b200_orig_dense_bottleneck
+    if "decoder" in _installed:
+        from pasco.models import decoder_v3
+        for cls, name, _ in _DECODER_PATCHES:
+            c = getattr(decoder_v3, cls)
+            setattr(c, name, getattr(c, "_pasco_b200_orig_" + name))
     _installed.clear()

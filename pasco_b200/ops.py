@@ -172,8 +172,9 @@ def kernel_map_down(child_coords: torch.Tensor, parent_table: HashTable, n_paren
 # ----------------------------------------------------------------------------------------------
 # order-preserving compaction
 # ----------------------------------------------------------------------------------------------
-def compact(mask: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, int]:
-    """mask bool/uint8 [N] → (kept_rows[int32 N'], new_row[int32 N], N').  One host sync (N')."""
+def compact(mask: torch.Tensor, total: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, int]:
+    """mask bool/uint8 [N] → (kept_rows[int32 N'], new_row[int32 N], N').  One host sync (N'), none when the caller
+    already knows N' and passes it as `total`."""
     n = mask.shape[0]
     dev = mask.device
     m8 = mask.to(torch.uint8) if mask.dtype != torch.uint8 else mask
@@ -186,9 +187,10 @@ def compact(mask: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, int]:
     call("pasco_mask_block_counts", ptr(m8), n, ptr(counts))
     incl = torch.cumsum(counts, 0, dtype=torch.int32)       # ≤ ~1k elements: plumbing
     offsets = (incl - counts).contiguous()
-    total = int(incl[-1].item())
-    if _ERR:
-        raise_pending_errors(dev)
+    if total is None:
+        total = int(incl[-1].item())
+        if _ERR:
+            raise_pending_errors(dev)
     new_row = torch.empty(n, dtype=torch.int32, device=dev)
     kept = torch.empty(total, dtype=torch.int32, device=dev)
     call("pasco_mask_compact", ptr(m8), n, ptr(offsets), ptr(new_row), ptr(kept))
@@ -716,6 +718,84 @@ def mimo_merge(F: torch.Tensor, coords: torch.Tensor, max_subnets: int = 8):
     if bad or M > max_subnets:
         return None
     return MimoMerge.apply(Fc, coords, M, (keys, vals, cap, ukeys, U))
+
+
+# ----------------------------------------------------------------------------------------------
+# the reference decoder's glue (csrc/decoder.cu)
+# ----------------------------------------------------------------------------------------------
+def _ptrs(ts) -> C.Array:
+    return (C.c_void_p * len(ts))(*[ptr(t) for t in ts])
+
+
+def completion_rows(probs: List[torch.Tensor], w: Optional[torch.Tensor] = None,
+                    labels: Optional[List[torch.Tensor]] = None):
+    """predict_completion_sem_logit's per-row pass (decoder_v3.py:333-345) over the M subnets' softmax rows [N, K]
+    (M <= 8, K <= 64): (cls int32 [M, N], keep bool [M, N], weight fp32 [M, N] = p_max · w[cls] or None without w,
+    votes int32 [N], counts int32 [3M + 1] = kept rows per subnet, labelled cells per subnet, rows per subnet whose
+    weight is not a finite value >= 0, rows with a vote).  labels: M device volumes of one integer dtype."""
+    M, (n, K) = len(probs), probs[0].shape
+    dev = probs[0].device
+    probs = [p.contiguous() for p in probs]
+    cls = torch.empty(M, n, dtype=torch.int32, device=dev)
+    keep = torch.empty(M, n, dtype=torch.bool, device=dev)
+    weight = torch.empty(M, n, dtype=torch.float32, device=dev) if w is not None else None
+    votes = torch.empty(n, dtype=torch.int32, device=dev)
+    counts = torch.zeros(3 * M + 1, dtype=torch.int32, device=dev)
+    labels = None if labels is None else [t.contiguous() for t in labels]
+    call("pasco_completion_rows", _ptrs(probs), M, n, K, ptr(w), _ptrs(labels) if labels else None,
+         labels[0].numel() if labels else 0, labels[0].element_size() if labels else 1, ptr(cls), ptr(keep),
+         ptr(weight), ptr(votes), ptr(counts))
+    return cls, keep, weight, votes, counts
+
+
+def topk_mask(w: torch.Tensor, q: torch.Tensor, k: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """bool [N]: the k largest w / q (fp32, IEEE division), ties at the k-th value taken by lowest row.  With q drawn as
+    torch.multinomial draws it (torch.empty_like(w).exponential_(1) on the same generator), the row set of
+    torch.multinomial(w, k, replacement=False), without its sort.  w >= 0 and finite; 1 <= k <= N."""
+    keep = torch.empty(w.shape[0], dtype=torch.bool, device=w.device) if out is None else out
+    call("pasco_topk_mask", ptr(w.contiguous()), ptr(q.contiguous()), w.shape[0], int(k), ptr(keep))
+    return keep
+
+
+def panop_crop(logits: torch.Tensor, coords: torch.Tensor, box: torch.Tensor, counts: torch.Tensor) -> torch.Tensor:
+    """predict_panop's prunes of one subnet and scale as one mask (decoder_v3.py:409-434): bool [N] = argmax != 0 and
+    box[:3] <= (x, y, z) <= box[3:], or the first 1000 rows inside the box when no argmax is != 0.  counts int32 [2]
+    (zeroed): rows with argmax != 0, rows kept.  No host synchronisation."""
+    mask = torch.empty(logits.shape[0], dtype=torch.bool, device=logits.device)
+    call("pasco_panop_crop", ptr(logits.contiguous()), logits.shape[0], logits.shape[1], ptr(_i32(coords).contiguous()),
+         ptr(box), ptr(mask), ptr(counts))
+    return mask
+
+
+class MimoBatch(torch.autograd.Function):
+    """batch_sparse_tensor (utils.py:659-670) of M subnets: (features [M, L, C], int32 coordinates [M, L, 4], keep_pad
+    bool [M, L] or an empty tensor); the backward hands every subnet its rows of the gradient."""
+
+    @staticmethod
+    def forward(ctx, want_keep, coords, *feats):
+        M, L, C_ = len(feats), max(f.shape[0] for f in feats), feats[0].shape[1]
+        dev = feats[0].device
+        feats = [f.contiguous() for f in feats]
+        out = torch.empty(M, L, C_, dtype=torch.float32, device=dev)
+        out_c = torch.empty(M, L, 4, dtype=torch.int32, device=dev)
+        keep = torch.empty(M, L, dtype=torch.bool, device=dev) if want_keep else torch.empty(0, device=dev)
+        call("pasco_mimo_batch", _ptrs(feats), _ptrs(coords), (C.c_int64 * M)(*[f.shape[0] for f in feats]), M, L, C_,
+             ptr(out), ptr(out_c), ptr(keep) if want_keep else None)
+        ctx.lens = [f.shape[0] for f in feats]
+        ctx.mark_non_differentiable(out_c, keep)
+        return out, out_c, keep
+
+    @staticmethod
+    def backward(ctx, g, _c, _k):
+        return (None, None) + tuple(g[m, :n] for m, n in enumerate(ctx.lens))
+
+
+def mimo_batch(feats: List[torch.Tensor], coords: List[torch.Tensor], keep_pad: bool = False):
+    """The M (<= 8) subnets' fp32 rows [L_m, C] and int32 coordinates [L_m, 4] zero-padded to L = max L_m in one launch:
+    (features [M, L, C], coordinates [M, L, 4], keep_pad bool [M, L] or None) with keep_pad = any feature or coordinate
+    != 0, the reference's rule (decoder_v3.py:443-446), not "row < L_m"."""
+    out, out_c, keep = MimoBatch.apply(keep_pad, tuple(_i32(c).contiguous() for c in coords), *[f.float() for f in feats])
+    return out, out_c, keep if keep_pad else None
 
 
 # ----------------------------------------------------------------------------------------------
