@@ -506,6 +506,16 @@ int pasco_panop_crop(const float* logits, int64_t n, int32_t K, const int32_t* c
 int pasco_mimo_batch(const float* const* feats, const int32_t* const* coords, const int64_t* lengths, int32_t M,
                      int64_t L, int32_t C, float* out_F, int32_t* out_C, uint8_t* keep_pad, pasco_stream_t s);
 
+/* ---- the reference transformer's sine position encoding (csrc/posenc.cu; transformer/position_encoding.py) ----------
+ * sine_pos: PositionEmbeddingSineSparse(n, normalize=True) of P coordinate rows.  coords points at row 0's x; rows are
+ * coord_pitch integers apart (int32, or int64 when is_i64), x, y, z adjacent.  table fp32 [rows][n] = the per-axis
+ * encoding of coordinates lo .. lo + rows - 1; a coordinate beyond either end reads that end's row, so the table must
+ * span every coordinate whose encoding differs from its ends' (|x| < 32 for the reference's eps and scale).  Writes
+ * out fp32 [P][3n] (x, y, z blocks of n), rows out_pitch floats apart: out = pe (add = 0) or out += pe (add = 1).
+ * n even, 2 <= n <= 256.                                                                                           */
+int pasco_sine_pos(const void* coords, int32_t is_i64, int64_t P, int64_t coord_pitch, const float* table, int32_t lo,
+                   int32_t rows, int32_t n, float* out, int64_t out_pitch, int32_t add, pasco_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -104,6 +104,7 @@ PROTOTYPES = {
     "pasco_topk_mask": (C.c_int, [_p, _p, _i64, _i64, _p, _p]),
     "pasco_panop_crop": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p]),
     "pasco_mimo_batch": (C.c_int, [_p, _p, _p, _i32, _i64, _i32, _p, _p, _p, _p]),
+    "pasco_sine_pos": (C.c_int, [_p, _i32, _i64, _i64, _p, _i32, _i32, _i32, _p, _i64, _i32, _p]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -80,11 +80,21 @@ The log lines keep their text.  At most DECODER_SYNCS host synchronisations of t
 more than 8 subnets or 64 classes, logits other than fp32, a resize other than (BatchNorm(C+3), 1x1 convolution), C not
 a multiple of 64 in training, a process with an active dropout, bounds that are not 3 integers and logits on another
 coordinate map than x go to the saved originals.
+
+The transformer hook (install(transformer=True)) replaces the transformer's dense glue: `PositionEmbeddingSineSparse.forward`
+(position_encoding.py:90-135) runs on ops.sine_pos (csrc/posenc.cu, bit for bit) and `TransformerPredictorV2.pred_heads`
+(transformer_predictor_v2.py:291-303) on net3d.mask_head (the einsum on ops.linear), both functions PascoNet's
+MaskTransformer calls.  With the attention hook, the forward builds voxel_feat and every level's key / value input with
+net3d.proj_plus_pos (no [B, P_s, hidden] position tensor; the cross-attention gets pos=None) and each item's outputs
+with one compaction and one gather per level.  At most TRANSFORMER_SYNCS host synchronisations of its own per forward.
+CPU tensors, normalize=False, a scale other than 2π, odd n or n > 256, float coordinates and a hidden size other than
+3n go to the saved originals.
 """
 from __future__ import annotations
 
 import collections
 import importlib
+import math
 import time
 
 import numpy as np
@@ -99,22 +109,33 @@ def _transformer_forward(self, xs, sem_logits, min_Cs, max_Cs, keep_pad):
     """transformer_predictor_v2.py:111-218 with the attention masks built on the device as bit rows
     (ops.attention_mask_bits): the reference's own submodules, outputs and padding semantics — padded rows of a MIMO
     batch take part in attention — without its [B·heads, Q, P] bool mask and the int64 row sum of line 164.
-    xs[scale] = (F [B, P_s, C], C [B, P_s, 4]) with B = n_infers."""
+    xs[scale] = (F [B, P_s, C], C [B, P_s, 4]) with B = n_infers.  With the transformer group installed too (and a
+    pe_layer it covers), the projections add the position encoding into their own rows (net3d.proj_plus_pos: no
+    [B, P_s, hidden] position tensor, pos=None to the cross-attention) and each item's outputs are gathered rows
+    (_item_outputs)."""
     F1, C1 = xs[1]
     if not F1.is_cuda:
         return self._pasco_b200_orig_forward(xs, sem_logits, min_Cs, max_Cs, keep_pad)
     bs = sem_logits[0].shape[0]
     assert self.n_infers == bs, "batch size should be equal to number of inference"
+    glue = _transformer_glue(self, xs)
     output = self.query_feat.weight.reshape(bs, -1, self.hidden_dim)
     query_embed = self.query_embed.weight.reshape(bs, -1, self.hidden_dim)
-    pos = [self.pe_layer(xs[s][1].reshape(-1, 4)[:, 1:]).reshape(bs, -1, self.hidden_dim) for s in self.src_scales]
-    voxel_feat = self.mask_feat_proj(F1) + pos[-1]
+    if glue:
+        pos = [None] * len(self.src_scales)
+        voxel_feat = _proj_plus_pos(self.mask_feat_proj, F1, C1, self.pe_layer.num_pos_feats)
+    else:
+        pos = [self.pe_layer(xs[s][1].reshape(-1, 4)[:, 1:]).reshape(bs, -1, self.hidden_dim) for s in self.src_scales]
+        voxel_feat = self.mask_feat_proj(F1) + pos[-1]
     cls, msk = self.pred_heads(output, voxel_feat)
     classes, masks = [cls], [msk]
     voxels = [_voxel_map(c) for c in C1]
     for i, s in enumerate(self.src_scales):
         src_F, src_C = xs[s]
-        src_F = self.input_projs[i](src_F)
+        if glue:
+            src_F = _proj_plus_pos(self.input_projs[i], src_F, src_C, self.pe_layer.num_pos_feats)
+        else:
+            src_F = self.input_projs[i](src_F)
         bits = torch.stack([_mask_bits(voxels[b], masks[-1][b], src_C[b], s) for b in range(bs)])
         output = self.transformer_cross_attention_layers[i](output, src_F, attn_mask=bits, pos=pos[i],
                                                             query_pos=query_embed)
@@ -124,6 +145,8 @@ def _transformer_forward(self, xs, sem_logits, min_Cs, max_Cs, keep_pad):
         cls, msk = self.pred_heads(output, voxel_feat)
         classes.append(cls)
         masks.append(msk)
+    if glue:
+        return _item_outputs(self, classes, masks, C1, keep_pad)
     preds = []
     for b in range(bs):
         keep = keep_pad[b]
@@ -171,6 +194,82 @@ def _cross_attention_forward(self, q_embed, bb_feat, attn_mask=None, padding_mas
         kv = bb_feat[b] if pos is None else bb_feat[b] + pos[b]
         outs.append(ops.cross_attention(self.multihead_attn, qb, kv, attn_mask[b]))
     return q_embed + self.dropout(torch.stack(outs, 0))
+
+
+# ------------------------------------------------------------------------------------------------
+# transformer glue: PositionEmbeddingSineSparse.forward (position_encoding.py:90-135) on ops.sine_pos,
+# TransformerPredictorV2.pred_heads (transformer_predictor_v2.py:291-303) on net3d.mask_head, and with the attention
+# group the projections and per-item outputs of _transformer_forward
+# ------------------------------------------------------------------------------------------------
+TRANSFORMER_SYNCS = 1   # host synchronisations of the group's own code in one hooked forward, at most: the kept row
+                        # counts of every item (_item_outputs)
+
+
+def _pe_covered(pe) -> bool:
+    """The encodings ops.sine_pos computes: normalize=True with the default scale 2π, n even and at most 256."""
+    n = getattr(pe, "num_pos_feats", None)
+    return (getattr(pe, "normalize", False) is True and getattr(pe, "scale", None) == 2 * math.pi
+            and isinstance(n, int) and n % 2 == 0 and 2 <= n <= 256)
+
+
+def _transformer_glue(self, xs) -> bool:
+    """Whether _transformer_forward runs the group's glue: the transformer and attention groups installed, a pe_layer
+    that _pe_covered covers with hidden_dim = 3n, and integer coordinates at every source scale."""
+    pe = self.pe_layer
+    return ("transformer" in _installed and "attention" in _installed and _pe_covered(pe)
+            and self.hidden_dim == 3 * pe.num_pos_feats
+            and all(xs[s][1].dtype in (torch.int32, torch.int64) for s in self.src_scales))
+
+
+def _pe_forward(self, coords):
+    """position_encoding.py:90-135 on ops.sine_pos, the same values bit for bit.  CPU tensors, float coordinates, rows
+    other than [N, 3] and encodings _pe_covered does not cover go to the saved original."""
+    if not (_pe_covered(self) and torch.is_tensor(coords) and coords.is_cuda and coords.dim() == 2
+            and coords.shape[1] == 3 and coords.dtype in (torch.int32, torch.int64)):
+        return self._pasco_b200_orig_forward(coords)
+    return ops.sine_pos(coords, self.num_pos_feats, temperature=self.temperature)
+
+
+def _pred_heads(self, output, mask_features):
+    """transformer_predictor_v2.py:291-303 as net3d.mask_head: class logits from the module's own layers, the mask
+    einsum on ops.linear.  CPU tensors and inputs other than fp32 [B, Q, d] / [B, P, d] go to the saved original."""
+    from .net3d import mask_head
+    if not (output.is_cuda and mask_features.is_cuda and output.dim() == 3 and mask_features.dim() == 3
+            and output.dtype == torch.float32 and mask_features.dtype == torch.float32
+            and output.shape[0] == mask_features.shape[0] and output.shape[2] == mask_features.shape[2]):
+        return self._pasco_b200_orig_pred_heads(output, mask_features)
+    return mask_head(self, output, mask_features)
+
+
+def _proj_plus_pos(linear, F_: torch.Tensor, C: torch.Tensor, n: int) -> torch.Tensor:
+    """net3d.proj_plus_pos over a padded batch: F [B, P, Cin], C [B, P, 4] → [B, P, 3n]."""
+    from .net3d import proj_plus_pos
+    B, P = F_.shape[0], F_.shape[1]
+    return proj_plus_pos(linear, F_.reshape(B * P, -1), C.reshape(B * P, C.shape[-1]), n).reshape(B, P, -1)
+
+
+def _item_outputs(self, classes, masks, C1, keep_pad):
+    """transformer_predictor_v2.py:190-216 without its boolean indexings, hash inserts and syncs per level: one
+    compaction of keep_pad[b] per item (every item's kept count read in one synchronisation) and, per level, one
+    gather of the logit rows and one of the coordinates, registered on a coordinate manager of the level's own.  Each
+    level's .C is thus a tensor of its own: SetCriterion.compute_losses shifts pred_mask_C by min_C in place.  keep_pad
+    selects one subnet's rows of a coordinate map, which are unique, so the maps are registered without a dedup."""
+    kp = keep_pad if torch.is_tensor(keep_pad) else torch.stack(list(keep_pad))
+    counts = kp.sum(1).tolist()                                                              # the one sync
+    preds = []
+    for b, n_keep in enumerate(counts):
+        kept, _, _ = ops.compact(kp[b], int(n_keep))
+        Cb = C1[b].to(torch.int32).contiguous()
+        item_masks = []
+        for m in masks:
+            mgr = ME.CoordinateManager()
+            key = mgr._register(ops.gather_coords(Cb, kept), 1)
+            item_masks.append(ME.SparseTensor(ops.GatherRows.apply(m[b], kept), coordinate_map_key=key,
+                                              coordinate_manager=mgr))
+        item_classes = [c[b].unsqueeze(0) for c in classes]
+        preds.append({"query_logits": item_classes[-1], "voxel_logits": item_masks[-1],
+                      "aux_outputs": self.set_aux(item_classes, item_masks)})
+    return preds
 
 
 # ------------------------------------------------------------------------------------------------
@@ -987,7 +1086,7 @@ def _decoder_forward(self, x, features, global_min_coords, global_max_coords, mi
 # ------------------------------------------------------------------------------------------------
 # install / uninstall
 # ------------------------------------------------------------------------------------------------
-_installed = set()     # "attention", "postprocess", "evaluate", "criterion", "trunk", "decoder"
+_installed = set()     # "attention", "postprocess", "evaluate", "criterion", "trunk", "decoder", "transformer"
 
 
 def _install_attention() -> bool:
@@ -1118,21 +1217,40 @@ def _install_decoder() -> bool:
     return True
 
 
+_TRANSFORMER_PATCHES = (("pasco.models.transformer.position_encoding", "PositionEmbeddingSineSparse", "forward",
+                         _pe_forward),
+                        ("pasco.models.transformer.transformer_predictor_v2", "TransformerPredictorV2", "pred_heads",
+                         _pred_heads))
+
+
+def _install_transformer() -> bool:
+    try:
+        classes = [getattr(importlib.import_module(mod), cls) for mod, cls, _, _ in _TRANSFORMER_PATCHES]
+    except Exception:
+        return False
+    for c, (_, _, name, fn) in zip(classes, _TRANSFORMER_PATCHES):
+        setattr(c, "_pasco_b200_orig_" + name, getattr(c, name))
+        setattr(c, name, fn)
+    return True
+
+
 def install(attention: bool = True, postprocess: bool = False, evaluate: bool = False, criterion: bool = False,
-            trunk: bool = False, decoder: bool = False) -> bool:
+            trunk: bool = False, decoder: bool = False, transformer: bool = False) -> bool:
     """Patch the reference (idempotent per group).  attention: TransformerPredictorV2.forward with its masks as
     bit rows, and the cross-attention layer that takes them; postprocess: the
     Ensembler and panoptic_inference; evaluate: Net.evaluate_all of both Net modules; criterion:
     SetCriterion.compute_losses and the completion losses both Net modules import; trunk: CylinderFeat.forward,
     Augmenter.merge and UNet3DV2.dense_bottleneck; decoder: DecoderBlock.forward and DecoderGenerativeSepConvV2's
-    forward, predict_completion_sem_logit and predict_panop.  Returns False when a requested group's `pasco` modules
-    are not importable."""
+    forward, predict_completion_sem_logit and predict_panop; transformer: PositionEmbeddingSineSparse.forward and
+    TransformerPredictorV2.pred_heads, and with attention the projections and per-item outputs of the forward.
+    Returns False when a requested group's `pasco` modules are not importable."""
     for name, wanted, fn in (("attention", attention, _install_attention),
                              ("postprocess", postprocess, _install_postprocess),
                              ("evaluate", evaluate, _install_evaluate),
                              ("criterion", criterion, _install_criterion),
                              ("trunk", trunk, _install_trunk),
-                             ("decoder", decoder, _install_decoder)):
+                             ("decoder", decoder, _install_decoder),
+                             ("transformer", transformer, _install_transformer)):
         if wanted and name not in _installed:
             if not fn():
                 return False
@@ -1171,5 +1289,9 @@ def uninstall() -> None:
         from pasco.models import decoder_v3
         for cls, name, _ in _DECODER_PATCHES:
             c = getattr(decoder_v3, cls)
+            setattr(c, name, getattr(c, "_pasco_b200_orig_" + name))
+    if "transformer" in _installed:
+        for mod, cls, name, _ in _TRANSFORMER_PATCHES:
+            c = getattr(importlib.import_module(mod), cls)
             setattr(c, name, getattr(c, "_pasco_b200_orig_" + name))
     _installed.clear()

@@ -237,15 +237,15 @@ class TensorField:
 
 def _hook_groups(value: str) -> frozenset:
     """PASCO_B200_HOOKS: "0" / unset = none, "1" = the attention hooks, else a comma list of "attention", "postprocess",
-    "evaluate", "criterion", "trunk", "decoder"."""
+    "evaluate", "criterion", "trunk", "decoder", "transformer"."""
     if value in ("", "0"):
         return frozenset()
     if value == "1":
         return frozenset({"attention"})
     groups = frozenset(v.strip() for v in value.split(",") if v.strip())
-    if not groups <= {"attention", "postprocess", "evaluate", "criterion", "trunk", "decoder"}:
+    if not groups <= {"attention", "postprocess", "evaluate", "criterion", "trunk", "decoder", "transformer"}:
         raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of attention, postprocess, evaluate, "
-                         "criterion, trunk, decoder")
+                         "criterion, trunk, decoder, transformer")
     return groups
 
 
@@ -256,14 +256,16 @@ _HOOK_MODULES = {"attention": ("pasco.models.transformer.transformer_predictor_v
                  "evaluate": ("pasco.models.metrics",),                               # ... and this one
                  "criterion": ("pasco.loss.criterion_sparse", "pasco.loss.losses"),   # ... and these
                  "trunk": ("pasco.models.augmenter", "pasco.models.unet3d_sparse_v2"),
-                 "decoder": ("pasco.models.decoder_v3",)}
+                 "decoder": ("pasco.models.decoder_v3",),
+                 "transformer": ("pasco.models.transformer.transformer_predictor_v2",)}
 
 
 def _maybe_install_hooks() -> None:
     """PASCO_B200_HOOKS: once the reference modules of the requested hook groups have been imported, route the
     cross-attention and attention-mask construction ("attention"), the Ensembler and panoptic_inference
     ("postprocess"), Net.evaluate_all ("evaluate"), the criterion ("criterion"), the trunk's voxeliser, merge and
-    dense bottleneck ("trunk") and the decoder's pruning, crops and MIMO batch ("decoder") onto the engine
+    dense bottleneck ("trunk"), the decoder's pruning, crops and MIMO batch ("decoder") and the transformer's position
+    encoding, projections and mask heads ("transformer") onto the engine
     (pasco_b200/hooks.py).  Checked when a
     SparseTensor is built."""
     global _HOOKS_PENDING
@@ -272,7 +274,8 @@ def _maybe_install_hooks() -> None:
         from .. import hooks
         hooks.install(attention="attention" in _HOOK_GROUPS, postprocess="postprocess" in _HOOK_GROUPS,
                       evaluate="evaluate" in _HOOK_GROUPS, criterion="criterion" in _HOOK_GROUPS,
-                      trunk="trunk" in _HOOK_GROUPS, decoder="decoder" in _HOOK_GROUPS)
+                      trunk="trunk" in _HOOK_GROUPS, decoder="decoder" in _HOOK_GROUPS,
+                      transformer="transformer" in _HOOK_GROUPS)
 
 
 class _LazyRows:

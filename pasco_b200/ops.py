@@ -6,6 +6,7 @@ current stream and the autograd graph.  Row indices are int32, −1 = no row.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import weakref
 from typing import List, Optional, Sequence, Tuple
 
@@ -1097,6 +1098,71 @@ def cross_attention(mha: torch.nn.MultiheadAttention, q: torch.Tensor, kv: torch
     o = MaskedCrossAttention.apply(torch.nn.functional.linear(q, wq, bq), linear(kv, wk, bk), linear(kv, wv, bv), mask,
                                    mha.num_heads)
     return mha.out_proj(o)
+
+
+# ----------------------------------------------------------------------------------------------
+# the mask transformer's sine position encoding (posenc.cu)
+# ----------------------------------------------------------------------------------------------
+SINE_SPAN = 64          # the encoding table covers coordinates [-SINE_SPAN, SINE_SPAN]; it is constant beyond |x| >= 32
+_SINE_TABLES = {}
+
+
+def sine_table(n: int, temperature, dev) -> torch.Tensor:
+    """One axis of PositionEmbeddingSineSparse(n, temperature, normalize=True) (position_encoding.py:94-131) over the
+    coordinates -SINE_SPAN .. SINE_SPAN, computed by the reference's own torch expression, so every value carries torch's
+    bits: fp32 [2·SINE_SPAN + 1, n].  Cached per (n, temperature, device)."""
+    key = (n, temperature, type(temperature), dev)
+    t = _SINE_TABLES.get(key)
+    if t is None:
+        x = torch.arange(-SINE_SPAN, SINE_SPAN + 1, device=dev).float()
+        x = x / (x + 1e-6) * (2 * math.pi)
+        dim_t = torch.arange(n, dtype=torch.float, device=dev)
+        dim_t = temperature ** (2 * (dim_t // 2) / n)
+        p = x[:, None] / dim_t
+        t = _SINE_TABLES[key] = torch.stack((p[:, 0::2].sin(), p[:, 1::2].cos()), dim=1).flatten(1).contiguous()
+    return t
+
+
+def sine_pos(coords: torch.Tensor, n: int, out: Optional[torch.Tensor] = None, add: bool = False,
+             temperature=10000) -> torch.Tensor:
+    """PositionEmbeddingSineSparse(n, normalize=True) of integer coordinates, bit for bit: coords int32 / int64 [P, 4]
+    (b, x, y, z) or [P, 3] (x, y, z), any row pitch → fp32 [P, 3n].  add=False writes the encoding (into `out` when given,
+    else a new tensor); add=True adds it into `out` in place, one read-modify-write.  `out` may be a column slice: unit
+    column stride, any row pitch.  n even, 2 <= n <= 256."""
+    assert coords.is_cuda and coords.dtype in (torch.int32, torch.int64) and coords.dim() == 2
+    assert coords.shape[1] in (3, 4), "sine_pos: coordinates are [P, 4] (b, x, y, z) or [P, 3]"
+    P = coords.shape[0]
+    if coords.stride(1) != 1 or (P > 1 and coords.stride(0) < coords.shape[1]):
+        coords = coords.contiguous()
+    if out is None:
+        assert not add, "sine_pos: add=True adds into `out`"
+        out = torch.empty(P, 3 * n, dtype=torch.float32, device=coords.device)
+    assert out.dtype == torch.float32 and out.device == coords.device and tuple(out.shape) == (P, 3 * n)
+    assert out.stride(1) == 1 and (P <= 1 or out.stride(0) >= 3 * n), "sine_pos: out needs unit column stride"
+    table = sine_table(n, temperature, coords.device)
+    call("pasco_sine_pos", C.c_void_p(coords.data_ptr() + coords.element_size() * (coords.shape[1] - 3)),
+         int(coords.dtype == torch.int64), P, coords.stride(0) if P > 1 else coords.shape[1], ptr(table), -SINE_SPAN,
+         table.shape[0], n, C.c_void_p(out.data_ptr()), out.stride(0) if P > 1 else 3 * n, int(add))
+    return out
+
+
+class AddSinePos(torch.autograd.Function):
+    """y + sine_pos(coords, n), added into y's rows in place; the gradient with respect to y is the identity."""
+
+    @staticmethod
+    def forward(ctx, y, coords, n):
+        ctx.mark_dirty(y)
+        return sine_pos(coords, n, out=y, add=True)
+
+    @staticmethod
+    def backward(ctx, g):
+        return g, None, None
+
+
+def add_sine_pos(y: torch.Tensor, coords: torch.Tensor, n: int) -> torch.Tensor:
+    """y += PositionEmbeddingSineSparse(n, normalize=True)(coords) in place, autograd-transparent (y must be a tensor no
+    backward pass reads, such as a fresh Linear output).  Returns y."""
+    return AddSinePos.apply(y, coords, n)
 
 
 # ----------------------------------------------------------------------------------------------
