@@ -95,6 +95,8 @@ from __future__ import annotations
 import collections
 import importlib
 import math
+import os
+import sys
 import time
 
 import numpy as np
@@ -276,8 +278,13 @@ def _item_outputs(self, classes, masks, C1, keep_pad):
 # post-processing: Ensembler.ensemble_sem_compl / ensemble_panop (ensembler.py:20-187) and panoptic_inference
 # (helper.py:91-303) on the row-form kernels of csrc/panoptic.cu (predict.py's stages)
 # ------------------------------------------------------------------------------------------------
-_PANOPTIC_USERS = ("pasco.models.helper", "pasco.models.net_panoptic_sparse", "pasco.models.net_panoptic_sparse_kitti360")
-_orig_panoptic_inference = None
+def _saved(module: str, name: str):
+    """The original of `module`'s module-level `name` as install() saved it (`_pasco_b200_orig_<name>` on the module),
+    read when called."""
+    return lambda *args: getattr(importlib.import_module(module), "_pasco_b200_orig_" + name)(*args)
+
+
+_orig_panoptic_inference = _saved("pasco.models.helper", "panoptic_inference")   # the Net modules import the same one
 
 
 def _rows_at(lin: torch.Tensor, size=predict.SCENE) -> torch.Tensor:
@@ -383,7 +390,6 @@ def _panoptic_inference(voxel_output, query_output, overlap_threshold, object_ma
 # evaluation: Net.evaluate_all (net_panoptic_sparse.py:650-765) on the dense forms of csrc/metrics.cu, finished by
 # metrics.py's host code into the reference's own metric objects
 # ------------------------------------------------------------------------------------------------
-_EVAL_USERS = (("pasco.models.net_panoptic_sparse", "Net"), ("pasco.models.net_panoptic_sparse_kitti360", "Net_kitti360"))
 EVAL_SYNCS = 3          # host synchronisations of a hooked evaluate_all call, at most (see _evaluate)
 
 
@@ -614,8 +620,6 @@ def _evaluate_all_kitti360(self, ssc_confidence, i_infer, sem_prob, panop_out, s
 # training criterion: SetCriterion.compute_losses (criterion_sparse.py:239-351) and the completion losses
 # (losses.py:69-179) on csrc/setloss.cu
 # ------------------------------------------------------------------------------------------------
-_CRIT_USERS = (("pasco.models.net_panoptic_sparse", "compute_sem_compl_loss"),
-               ("pasco.models.net_panoptic_sparse_kitti360", "compute_sem_compl_loss_kitti360"))
 CRITERION_SYNCS = 1     # host synchronisations of one hooked compute_losses level or completion-loss call, at most
 
 
@@ -784,7 +788,9 @@ def _compute_sem_compl_loss_kitti360(sem_labels, sem_logits_at_scales, min_Cs, m
     return out
 
 
-_orig_compl = [None, None]      # the losses module's compute_sem_compl_loss / compute_sem_compl_loss_kitti360
+# the Net modules' compute_sem_compl_loss / compute_sem_compl_loss_kitti360 as install() found them
+_orig_compl = [_saved("pasco.models.net_panoptic_sparse", "compute_sem_compl_loss"),
+               _saved("pasco.models.net_panoptic_sparse_kitti360", "compute_sem_compl_loss_kitti360")]
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1086,152 +1092,68 @@ def _decoder_forward(self, x, features, global_min_coords, global_max_coords, mi
 # ------------------------------------------------------------------------------------------------
 # install / uninstall
 # ------------------------------------------------------------------------------------------------
-_installed = set()     # "attention", "postprocess", "evaluate", "criterion", "trunk", "decoder", "transformer"
+_TP = "pasco.models.transformer.transformer_predictor_v2"
+_DEC = "pasco.models.decoder_v3"
+_NET = "pasco.models.net_panoptic_sparse"
+_K360 = "pasco.models.net_panoptic_sparse_kitti360"    # imports pasco.data.kitti360.params, which may not import
+
+# Every hook group in install order: (the trigger modules PASCO_B200_HOOKS waits for, its patch sites).  A site is
+# (module, class or None for a module-level name, attribute, replacement, whether the site may be missing); install()
+# keeps the original as `_pasco_b200_orig_<attribute>` on that class or module.
+_GROUPS = {
+    "attention": ((_TP,), (
+        (_TP, "TransformerPredictorV2", "forward", _transformer_forward, False),
+        ("pasco.models.transformer.blocks", "CrossAttentionLayer", "forward", _cross_attention_forward, False))),
+    "postprocess": (("pasco.models.ensembler", "pasco.models.helper"), (      # either Net module imports both
+        ("pasco.models.ensembler", "Ensembler", "ensemble_sem_compl", _ensemble_sem_compl, False),
+        ("pasco.models.ensembler", "Ensembler", "ensemble_panop", _ensemble_panop, False),
+        ("pasco.models.helper", None, "panoptic_inference", _panoptic_inference, False),
+        (_NET, None, "panoptic_inference", _panoptic_inference, False),        # the Net modules import it by name
+        (_K360, None, "panoptic_inference", _panoptic_inference, True))),
+    "evaluate": (("pasco.models.metrics",), (                                   # ... and this one
+        (_NET, "Net", "evaluate_all", _evaluate_all, False),
+        (_K360, "Net_kitti360", "evaluate_all", _evaluate_all_kitti360, True))),
+    "criterion": (("pasco.loss.criterion_sparse", "pasco.loss.losses"), (      # ... and these
+        ("pasco.loss.criterion_sparse", "SetCriterion", "compute_losses", _compute_losses, False),
+        # the completion losses under the names the Net modules import; pasco.loss.losses keeps its own
+        (_NET, None, "compute_sem_compl_loss", _compute_sem_compl_loss, False),
+        (_K360, None, "compute_sem_compl_loss_kitti360", _compute_sem_compl_loss_kitti360, True))),
+    "trunk": (("pasco.models.augmenter", "pasco.models.unet3d_sparse_v2"), (
+        ("pasco.models.unet3d_sparse_v2", "CylinderFeat", "forward", _cylinder_forward, False),
+        ("pasco.models.augmenter", "Augmenter", "merge", _augmenter_merge, False),
+        ("pasco.models.unet3d_sparse_v2", "UNet3DV2", "dense_bottleneck", _dense_bottleneck, False))),
+    "decoder": ((_DEC,), (
+        (_DEC, "DecoderBlock", "forward", _decoder_block_forward, False),
+        (_DEC, "DecoderGenerativeSepConvV2", "predict_completion_sem_logit", _predict_completion_sem_logit, False),
+        (_DEC, "DecoderGenerativeSepConvV2", "predict_panop", _predict_panop, False),
+        (_DEC, "DecoderGenerativeSepConvV2", "forward", _decoder_forward, False))),
+    "transformer": ((_TP,), (
+        ("pasco.models.transformer.position_encoding", "PositionEmbeddingSineSparse", "forward", _pe_forward, False),
+        (_TP, "TransformerPredictorV2", "pred_heads", _pred_heads, False))),
+}
+_installed = set()     # the names of the installed groups
 
 
-def _install_attention() -> bool:
-    try:
-        from pasco.models.transformer import blocks
-        from pasco.models.transformer.transformer_predictor_v2 import TransformerPredictorV2
-    except Exception:
-        return False
-    TransformerPredictorV2._pasco_b200_orig_forward = TransformerPredictorV2.forward
-    TransformerPredictorV2.forward = _transformer_forward
-    blocks.CrossAttentionLayer._pasco_b200_orig_forward = blocks.CrossAttentionLayer.forward
-    blocks.CrossAttentionLayer.forward = _cross_attention_forward
-    return True
+def _owners(sites) -> list:
+    """The class or module that holds each site's attribute, None for an optional site that is missing.  Raises when
+    any other site's module does not import or lacks the class."""
+    out = []
+    for module, cls, _, _, optional in sites:
+        try:
+            mod = importlib.import_module(module)
+            out.append(mod if cls is None else getattr(mod, cls))
+        except Exception:
+            if not optional:
+                raise
+            out.append(None)
+    return out
 
 
 def _users():
-    """The modules that hold the name panoptic_inference (the Net modules import it by name); kitti360 when importable."""
-    mods = []
-    for name in _PANOPTIC_USERS:
-        try:
-            mods.append(importlib.import_module(name))
-        except Exception:
-            if name != _PANOPTIC_USERS[-1]:
-                raise
-    return mods
-
-
-def _install_postprocess() -> bool:
-    global _orig_panoptic_inference
-    try:
-        from pasco.models.ensembler import Ensembler
-        users = _users()
-    except Exception:
-        return False
-    Ensembler._pasco_b200_orig_ensemble_sem_compl = Ensembler.ensemble_sem_compl
-    Ensembler.ensemble_sem_compl = _ensemble_sem_compl
-    Ensembler._pasco_b200_orig_ensemble_panop = Ensembler.ensemble_panop
-    Ensembler.ensemble_panop = _ensemble_panop
-    _orig_panoptic_inference = users[0].panoptic_inference
-    for mod in users:
-        mod._pasco_b200_orig_panoptic_inference = _orig_panoptic_inference
-        mod.panoptic_inference = _panoptic_inference
-    return True
-
-
-def _eval_nets():
-    """(Net class, its evaluate_all replacement) of both Net modules; the KITTI-360 one when importable."""
-    out = []
-    for (name, cls), fn in zip(_EVAL_USERS, (_evaluate_all, _evaluate_all_kitti360)):
-        try:
-            out.append((getattr(importlib.import_module(name), cls), fn))
-        except Exception:
-            if name != _EVAL_USERS[-1][0]:
-                raise
-    return out
-
-
-def _install_evaluate() -> bool:
-    try:
-        nets = _eval_nets()
-    except Exception:
-        return False
-    for net, fn in nets:
-        net._pasco_b200_orig_evaluate_all = net.evaluate_all
-        net.evaluate_all = fn
-    return True
-
-
-def _crit_users():
-    """(Net module, the completion-loss name it imports) of both Net modules; the KITTI-360 one when importable."""
-    out = []
-    for name, fn in _CRIT_USERS:
-        try:
-            out.append((importlib.import_module(name), fn))
-        except Exception:
-            if name != _CRIT_USERS[-1][0]:
-                raise
-    return out
-
-
-def _install_criterion() -> bool:
-    try:
-        from pasco.loss import losses
-        from pasco.loss.criterion_sparse import SetCriterion
-        users = _crit_users()
-    except Exception:
-        return False
-    SetCriterion._pasco_b200_orig_compute_losses = SetCriterion.compute_losses
-    SetCriterion.compute_losses = _compute_losses
-    _orig_compl[:] = [losses.compute_sem_compl_loss, losses.compute_sem_compl_loss_kitti360]
-    for mod, name in users:
-        setattr(mod, "_pasco_b200_orig_" + name, getattr(mod, name))
-        setattr(mod, name, _compute_sem_compl_loss if name == "compute_sem_compl_loss"
-                else _compute_sem_compl_loss_kitti360)
-    return True
-
-
-def _install_trunk() -> bool:
-    try:
-        from pasco.models.augmenter import Augmenter
-        from pasco.models.unet3d_sparse_v2 import CylinderFeat, UNet3DV2
-    except Exception:
-        return False
-    CylinderFeat._pasco_b200_orig_forward = CylinderFeat.forward
-    CylinderFeat.forward = _cylinder_forward
-    Augmenter._pasco_b200_orig_merge = Augmenter.merge
-    Augmenter.merge = _augmenter_merge
-    UNet3DV2._pasco_b200_orig_dense_bottleneck = UNet3DV2.dense_bottleneck
-    UNet3DV2.dense_bottleneck = _dense_bottleneck
-    return True
-
-
-_DECODER_PATCHES = (("DecoderBlock", "forward", _decoder_block_forward),
-                    ("DecoderGenerativeSepConvV2", "predict_completion_sem_logit", _predict_completion_sem_logit),
-                    ("DecoderGenerativeSepConvV2", "predict_panop", _predict_panop),
-                    ("DecoderGenerativeSepConvV2", "forward", _decoder_forward))
-
-
-def _install_decoder() -> bool:
-    try:
-        from pasco.models import decoder_v3
-    except Exception:
-        return False
-    for cls, name, fn in _DECODER_PATCHES:
-        c = getattr(decoder_v3, cls)
-        setattr(c, "_pasco_b200_orig_" + name, getattr(c, name))
-        setattr(c, name, fn)
-    return True
-
-
-_TRANSFORMER_PATCHES = (("pasco.models.transformer.position_encoding", "PositionEmbeddingSineSparse", "forward",
-                         _pe_forward),
-                        ("pasco.models.transformer.transformer_predictor_v2", "TransformerPredictorV2", "pred_heads",
-                         _pred_heads))
-
-
-def _install_transformer() -> bool:
-    try:
-        classes = [getattr(importlib.import_module(mod), cls) for mod, cls, _, _ in _TRANSFORMER_PATCHES]
-    except Exception:
-        return False
-    for c, (_, _, name, fn) in zip(classes, _TRANSFORMER_PATCHES):
-        setattr(c, "_pasco_b200_orig_" + name, getattr(c, name))
-        setattr(c, name, fn)
-    return True
+    """The modules that hold the name panoptic_inference: helper and the Net modules, which import it by name (the
+    KITTI-360 one when importable)."""
+    sites = [site for _, sites in _GROUPS.values() for site in sites if site[2] == "panoptic_inference"]
+    return [m for m in _owners(sites) if m is not None]
 
 
 def install(attention: bool = True, postprocess: bool = False, evaluate: bool = False, criterion: bool = False,
@@ -1243,55 +1165,53 @@ def install(attention: bool = True, postprocess: bool = False, evaluate: bool = 
     Augmenter.merge and UNet3DV2.dense_bottleneck; decoder: DecoderBlock.forward and DecoderGenerativeSepConvV2's
     forward, predict_completion_sem_logit and predict_panop; transformer: PositionEmbeddingSineSparse.forward and
     TransformerPredictorV2.pred_heads, and with attention the projections and per-item outputs of the forward.
-    Returns False when a requested group's `pasco` modules are not importable."""
-    for name, wanted, fn in (("attention", attention, _install_attention),
-                             ("postprocess", postprocess, _install_postprocess),
-                             ("evaluate", evaluate, _install_evaluate),
-                             ("criterion", criterion, _install_criterion),
-                             ("trunk", trunk, _install_trunk),
-                             ("decoder", decoder, _install_decoder),
-                             ("transformer", transformer, _install_transformer)):
-        if wanted and name not in _installed:
-            if not fn():
-                return False
-            _installed.add(name)
+    Groups install in _GROUPS' order, each only once all its sites have been found.  Returns False at the first
+    requested group whose `pasco` modules are not importable; the groups before it stay installed."""
+    requested = locals()                               # one keyword per group of _GROUPS
+    for group, (_, sites) in _GROUPS.items():
+        if not requested[group] or group in _installed:
+            continue
+        try:
+            owners = _owners(sites)
+        except Exception:
+            return False
+        for owner, (_, _, attr, fn, _) in zip(owners, sites):
+            if owner is not None:
+                setattr(owner, "_pasco_b200_orig_" + attr, getattr(owner, attr))
+                setattr(owner, attr, fn)
+        _installed.add(group)
     return True
 
 
 def uninstall() -> None:
     """Restore every attribute install() patched."""
-    if "attention" in _installed:
-        from pasco.models.transformer import blocks
-        from pasco.models.transformer.transformer_predictor_v2 import TransformerPredictorV2
-        TransformerPredictorV2.forward = TransformerPredictorV2._pasco_b200_orig_forward
-        blocks.CrossAttentionLayer.forward = blocks.CrossAttentionLayer._pasco_b200_orig_forward
-    if "postprocess" in _installed:
-        from pasco.models.ensembler import Ensembler
-        Ensembler.ensemble_sem_compl = Ensembler._pasco_b200_orig_ensemble_sem_compl
-        Ensembler.ensemble_panop = Ensembler._pasco_b200_orig_ensemble_panop
-        for mod in _users():
-            mod.panoptic_inference = mod._pasco_b200_orig_panoptic_inference
-    if "evaluate" in _installed:
-        for net, _ in _eval_nets():
-            net.evaluate_all = net._pasco_b200_orig_evaluate_all
-    if "criterion" in _installed:
-        from pasco.loss.criterion_sparse import SetCriterion
-        SetCriterion.compute_losses = SetCriterion._pasco_b200_orig_compute_losses
-        for mod, name in _crit_users():
-            setattr(mod, name, getattr(mod, "_pasco_b200_orig_" + name))
-    if "trunk" in _installed:
-        from pasco.models.augmenter import Augmenter
-        from pasco.models.unet3d_sparse_v2 import CylinderFeat, UNet3DV2
-        CylinderFeat.forward = CylinderFeat._pasco_b200_orig_forward
-        Augmenter.merge = Augmenter._pasco_b200_orig_merge
-        UNet3DV2.dense_bottleneck = UNet3DV2._pasco_b200_orig_dense_bottleneck
-    if "decoder" in _installed:
-        from pasco.models import decoder_v3
-        for cls, name, _ in _DECODER_PATCHES:
-            c = getattr(decoder_v3, cls)
-            setattr(c, name, getattr(c, "_pasco_b200_orig_" + name))
-    if "transformer" in _installed:
-        for mod, cls, name, _ in _TRANSFORMER_PATCHES:
-            c = getattr(importlib.import_module(mod), cls)
-            setattr(c, name, getattr(c, "_pasco_b200_orig_" + name))
+    for group, (_, sites) in _GROUPS.items():
+        if group in _installed:
+            for owner, (_, _, attr, _, _) in zip(_owners(sites), sites):
+                if owner is not None:
+                    setattr(owner, attr, getattr(owner, "_pasco_b200_orig_" + attr))
     _installed.clear()
+
+
+def _parse_groups(value: str) -> frozenset:
+    """PASCO_B200_HOOKS: "" / "0" = no group, "1" = the attention group, else a comma list of _GROUPS' names."""
+    if value in ("", "0"):
+        return frozenset()
+    if value == "1":
+        return frozenset(list(_GROUPS)[:1])          # the first group: attention
+    groups = frozenset(v.strip() for v in value.split(",") if v.strip())
+    if not groups <= set(_GROUPS):
+        raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of {', '.join(_GROUPS)}")
+    return groups
+
+
+_REQUESTED = _parse_groups(os.environ.get("PASCO_B200_HOOKS", "0"))     # an unknown group raises on import
+
+
+def _install_requested() -> bool:
+    """PASCO_B200_HOOKS: install the requested groups once all their trigger modules have been imported; whether they
+    had been.  pasco_b200.me asks on every SparseTensor construction until then."""
+    if not all(m in sys.modules for g in _REQUESTED for m in _GROUPS[g][0]):
+        return False
+    install(**{g: g in _REQUESTED for g in _GROUPS})
+    return True

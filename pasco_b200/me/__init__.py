@@ -12,7 +12,6 @@ from __future__ import annotations
 import itertools
 import math
 import os
-import sys
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -235,47 +234,14 @@ class TensorField:
     """Referenced only in isinstance checks (pasco/models/dropout.py:23,47)."""
 
 
-def _hook_groups(value: str) -> frozenset:
-    """PASCO_B200_HOOKS: "0" / unset = none, "1" = the attention hooks, else a comma list of "attention", "postprocess",
-    "evaluate", "criterion", "trunk", "decoder", "transformer"."""
-    if value in ("", "0"):
-        return frozenset()
-    if value == "1":
-        return frozenset({"attention"})
-    groups = frozenset(v.strip() for v in value.split(",") if v.strip())
-    if not groups <= {"attention", "postprocess", "evaluate", "criterion", "trunk", "decoder", "transformer"}:
-        raise ValueError(f"PASCO_B200_HOOKS={value!r}: expected 0, 1 or a comma list of attention, postprocess, evaluate, "
-                         "criterion, trunk, decoder, transformer")
-    return groups
-
-
-_HOOK_GROUPS = _hook_groups(os.environ.get("PASCO_B200_HOOKS", "0"))
-_HOOKS_PENDING = bool(_HOOK_GROUPS)
-_HOOK_MODULES = {"attention": ("pasco.models.transformer.transformer_predictor_v2",),
-                 "postprocess": ("pasco.models.ensembler", "pasco.models.helper"),    # either Net module imports both
-                 "evaluate": ("pasco.models.metrics",),                               # ... and this one
-                 "criterion": ("pasco.loss.criterion_sparse", "pasco.loss.losses"),   # ... and these
-                 "trunk": ("pasco.models.augmenter", "pasco.models.unet3d_sparse_v2"),
-                 "decoder": ("pasco.models.decoder_v3",),
-                 "transformer": ("pasco.models.transformer.transformer_predictor_v2",)}
+_HOOKS_PENDING = os.environ.get("PASCO_B200_HOOKS", "0") not in ("", "0")
 
 
 def _maybe_install_hooks() -> None:
-    """PASCO_B200_HOOKS: once the reference modules of the requested hook groups have been imported, route the
-    cross-attention and attention-mask construction ("attention"), the Ensembler and panoptic_inference
-    ("postprocess"), Net.evaluate_all ("evaluate"), the criterion ("criterion"), the trunk's voxeliser, merge and
-    dense bottleneck ("trunk"), the decoder's pruning, crops and MIMO batch ("decoder") and the transformer's position
-    encoding, projections and mask heads ("transformer") onto the engine
-    (pasco_b200/hooks.py).  Checked when a
-    SparseTensor is built."""
+    """PASCO_B200_HOOKS: install the requested hook groups (pasco_b200/hooks.py) once their trigger modules have been
+    imported.  Checked when a SparseTensor is built."""
     global _HOOKS_PENDING
-    if _HOOKS_PENDING and all(m in sys.modules for g in _HOOK_GROUPS for m in _HOOK_MODULES[g]):
-        _HOOKS_PENDING = False
-        from .. import hooks
-        hooks.install(attention="attention" in _HOOK_GROUPS, postprocess="postprocess" in _HOOK_GROUPS,
-                      evaluate="evaluate" in _HOOK_GROUPS, criterion="criterion" in _HOOK_GROUPS,
-                      trunk="trunk" in _HOOK_GROUPS, decoder="decoder" in _HOOK_GROUPS,
-                      transformer="transformer" in _HOOK_GROUPS)
+    _HOOKS_PENDING = not _hooks._install_requested()
 
 
 class _LazyRows:
@@ -747,3 +713,8 @@ class _Utils:
 
 
 utils = _Utils()
+
+
+# last, as hooks imports this module: importing hooks parses PASCO_B200_HOOKS and raises on an unknown group
+if _HOOKS_PENDING:
+    from .. import hooks as _hooks  # noqa: E402

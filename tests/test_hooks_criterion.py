@@ -2,7 +2,7 @@
 SetCriterion.compute_losses and completion losses on csrc/setloss.cu, against the stored outputs of the reference's own
 loss code (tests/golden/loss_m2.npz) and against the saved originals on the same inputs.
 
-  * CPU: the new C-ABI symbols are declared and typed, PASCO_B200_HOOKS parsing, install / uninstall restore all three
+  * CPU: the new C-ABI symbols are declared and typed, install / uninstall restore all three
     replaced names, no local memory in the new kernels;
   * GPU: the fixture (M = 2, 4 levels, overlapping masks, unknown rows, 255 labels, dustbin queries); N = 400 k rows,
     Q = 100, T = 30 against the original (cost matrices, assignments, every term, gradients), and with two target words
@@ -67,16 +67,6 @@ def test_new_kernels_use_no_local_memory():
                 found[n] += 1
                 assert not re.search(r"\b(LDL|STL)\b", f), f"{head}: local-memory traffic"
     assert set(found) == set(names), set(names) - set(found)
-
-
-def test_hook_switch_values():
-    from pasco_b200.me import _hook_groups
-    assert _hook_groups("attention,postprocess,evaluate,criterion") == {"attention", "postprocess", "evaluate",
-                                                                          "criterion"}
-    assert _hook_groups("criterion") == {"criterion"}
-    assert _hook_groups("1") == {"attention"}
-    with pytest.raises(ValueError):
-        _hook_groups("criterion,loss")
 
 
 def _reference_modules():

@@ -2,8 +2,8 @@
 DecoderGenerativeSepConvV2's predict_completion_sem_logit, predict_panop and forward on csrc/decoder.cu and
 net3d.resize_rows, against the saved originals on the same inputs.
 
-  * CPU: the new C-ABI symbols are declared and typed, no local memory in the new kernels, PASCO_B200_HOOKS parsing,
-    install / uninstall restore all four names;
+  * CPU: the new C-ABI symbols are declared and typed, no local memory in the new kernels, install / uninstall restore
+    all four names;
   * GPU: pasco_completion_rows against torch (M = 1..4, K = 19 / 20, tied maxima, NaN rows); the cap against
     torch.multinomial (the exponential-race identity, the keep mask at N = 1 M and k = 400 000, the CUDA generator state
     afterwards); the M >= 3 vote cap; predict_panop bit for bit (the all-empty keep[:1000] case, unequal subnets, the
@@ -68,16 +68,6 @@ def test_new_kernels_use_no_local_memory():
                 found[n] += 1
                 assert not re.search(r"\b(LDL|STL)\b", f), f"{head}: local-memory traffic"
     assert set(found) == set(KERNELS), set(KERNELS) - set(found)
-
-
-def test_hook_switch_values():
-    from pasco_b200.me import _hook_groups
-    assert _hook_groups("attention,postprocess,evaluate,criterion,trunk,decoder") == {
-        "attention", "postprocess", "evaluate", "criterion", "trunk", "decoder"}
-    assert _hook_groups("decoder") == {"decoder"}
-    assert _hook_groups(" decoder , trunk ") == {"decoder", "trunk"}
-    with pytest.raises(ValueError):
-        _hook_groups("decoder,prune")
 
 
 def _decoder_module():

@@ -1,7 +1,7 @@
 """The evaluation hook (pasco_b200/hooks.py install(evaluate=True)): the unmodified reference's Net.evaluate_all on the
 dense passes of csrc/metrics.cu, against the reference's own saved original on the same inputs.
 
-  * CPU: the new C-ABI symbols are declared and typed, PASCO_B200_HOOKS parsing, install / uninstall restore
+  * CPU: the new C-ABI symbols are declared and typed, install / uninstall restore
     evaluate_all on both Net modules, the reference's float32 pair IoU (Tensor.__rdiv__), no local memory in the new
     kernels;
   * GPU: the three eval.npz scenes (make_golden_eval's predictions and ground truth) with all M + 1 entries, with and
@@ -68,15 +68,6 @@ def test_new_kernels_use_no_local_memory():
                 found[n] += 1
                 assert not re.search(r"\b(LDL|STL)\b", f), f"{head}: local-memory traffic"
     assert set(found) == set(names) and found["k_eval_ssc_planes"] == 2 and found["k_eval_pairs_dense"] == 2
-
-
-def test_hook_switch_values():
-    from pasco_b200.me import _hook_groups
-    assert _hook_groups("attention,postprocess,evaluate") == {"attention", "postprocess", "evaluate"}
-    assert _hook_groups("evaluate") == {"evaluate"}
-    assert _hook_groups("1") == {"attention"}
-    with pytest.raises(ValueError):
-        _hook_groups("attention,metrics")
 
 
 def test_reference_pair_iou_is_reciprocal_times_intersection():

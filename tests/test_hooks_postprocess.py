@@ -3,7 +3,7 @@ Ensembler.ensemble_sem_compl / ensemble_panop and panoptic_inference on the pano
 saved originals (`_pasco_b200_orig_*`) on the same inputs.
 
   * CPU: install / uninstall restore every patched attribute (both Net modules' panoptic_inference included), install()
-    without arguments patches the attention alone, PASCO_B200_HOOKS parsing;
+    without arguments patches the attention alone;
   * GPU: panoptic_inference on make_golden_predict.scene_a rows at Q = 24, 100 and 200 (merged stuff, no kept query, one
     kept query, a zero-area query, voxel logits, a training-frame call with negative min_C, a scale-8 scene size and
     unsorted rows), the Ensembler at M = 1, 2, 3 under identity, flip + translation and 7-degree poses, fallbacks, bit-
@@ -78,16 +78,6 @@ def test_install_uninstall_restores_every_attribute():
              blocks.CrossAttentionLayer.forward, TransformerPredictorV2.compute_attn_mask)
     assert all(a is b for a, b in zip(after, before))
     assert all(m.panoptic_inference is before[2] for m in users)
-
-
-def test_hook_switch_values():
-    from pasco_b200.me import _hook_groups
-    assert _hook_groups("0") == frozenset() and _hook_groups("") == frozenset()
-    assert _hook_groups("1") == {"attention"}
-    assert _hook_groups("attention,postprocess") == {"attention", "postprocess"}
-    assert _hook_groups("postprocess") == {"postprocess"}
-    with pytest.raises(ValueError):
-        _hook_groups("attention,dense")
 
 
 # ------------------------------------------------------------------------------------------------

@@ -3,8 +3,8 @@ PositionEmbeddingSineSparse.forward on ops.sine_pos (csrc/posenc.cu), Transforme
 net3d.mask_head and, with the attention group, the projections and per-item outputs of its forward; and PascoNet's
 MaskTransformer on the same shared functions.
 
-  * CPU: the new C-ABI symbol is declared and typed, no local memory in the new kernel, PASCO_B200_HOOKS parsing,
-    install / uninstall restore every patched name, alone and together with the attention group;
+  * CPU: the new C-ABI symbol is declared and typed, no local memory in the new kernel, install / uninstall
+    restore every patched name, alone and together with the attention group;
   * GPU: the encoding against the reference module bit for bit (int32 / int64, [P, 4] / [P, 3], zero, negative and
     ±32767 coordinates, P = 1 / 4095 / 2 M, n = 128 / 32), add mode into a column slice, the mask head, the whole
     hooked forward against the golden fixtures, independent coordinates per level, Net.step + backward with the group
@@ -60,17 +60,6 @@ def test_new_kernel_uses_no_local_memory():
             found += 1
             assert not re.search(r"\b(LDL|STL)\b", f), f"{head}: local-memory traffic"
     assert found == 2                                   # int32 and int64 coordinates
-
-
-def test_hook_switch_values():
-    from pasco_b200.me import _HOOK_MODULES, _hook_groups
-    assert _hook_groups("attention,postprocess,evaluate,criterion,trunk,decoder,transformer") == {
-        "attention", "postprocess", "evaluate", "criterion", "trunk", "decoder", "transformer"}
-    assert _hook_groups("transformer") == {"transformer"}
-    assert _hook_groups(" attention , transformer ") == {"attention", "transformer"}
-    assert "transformer" in _HOOK_MODULES
-    with pytest.raises(ValueError):
-        _hook_groups("transformer,glue")
 
 
 def _classes():

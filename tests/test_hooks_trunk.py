@@ -2,7 +2,7 @@
 Augmenter.merge and UNet3DV2.dense_bottleneck on csrc/voxel.cu and net3d's grid bottleneck, against the saved
 originals on the same inputs.
 
-  * CPU: the new C-ABI symbols are declared and typed, PASCO_B200_HOOKS parsing, install / uninstall restore all three
+  * CPU: the new C-ABI symbols are declared and typed, install / uninstall restore all three
     names, no local memory in the new kernels;
   * GPU: voxel grouping bit-identical to torch.unique(dim=0, return_inverse=True); the merge's features, coordinates
     and input gradient bit-identical to the dense original (M = 1, 2, 3; disjoint and overlapping subnets; all-zero,
@@ -66,17 +66,6 @@ def test_new_kernels_use_no_local_memory():
                 found[n] += 1
                 assert not re.search(r"\b(LDL|STL)\b", f), f"{head}: local-memory traffic"
     assert set(found) == set(KERNELS), set(KERNELS) - set(found)
-
-
-def test_hook_switch_values():
-    from pasco_b200.me import _hook_groups
-    assert _hook_groups("attention,postprocess,evaluate,criterion,trunk") == {"attention", "postprocess", "evaluate",
-                                                                                "criterion", "trunk"}
-    assert _hook_groups("trunk") == {"trunk"}
-    assert _hook_groups(" trunk , criterion ") == {"trunk", "criterion"}
-    assert _hook_groups("1") == {"attention"}
-    with pytest.raises(ValueError):
-        _hook_groups("trunk,voxel")
 
 
 def _reference_modules():
