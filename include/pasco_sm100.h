@@ -455,6 +455,74 @@ int pasco_lovasz_grad(const float* err_sorted, const int64_t* perm, const int32_
 int pasco_lovasz_backward(const float* probs, const int32_t* labels, const int64_t* perm, const float* grad,
                           const float* g, int64_t P, int32_t C, float* dx, pasco_stream_t s);
 
+/* ---- the same criterion over a table of levels: each pass is one launch for every level (up to 24 per launch) -----
+ * A level is one output level of one subnet: its mask logits F fp32 [n][Q], its subnet's sampled bits / flags / stats
+ * (pasco_setloss_sample), its query logits [Q][K1], target class ids [T] and class weights [K1].  Each level keeps the
+ * row chunking and the fixed-order partial sums of the one-level calls above, so a grouped call gives the same bits as
+ * one call per level.  Each pass reads only the fields it names; the others may be zero.                            */
+typedef struct {
+  const float* F;                /* [n][Q] */
+  int64_t n;
+  int32_t Q, T;
+  const uint32_t* bits;
+  const uint8_t* flags;
+  const int32_t* stats;
+  const float* query_logits;     /* [Q][K1] */
+  int32_t K1;
+  const int32_t* ids;            /* [T] */
+  const float* class_weight;     /* [K1] */
+  float* C;                      /* match cost: [Q][T] */
+  const int32_t* qi;             /* pair sums: P matched pairs */
+  const int32_t* tj;
+  int32_t P;
+  float* sums;                   /* [P][4] */
+  const float* g_sums;           /* pair backward: [P][4] */
+  float* gF_pairs;               /* [n][Q], the pairs' columns written */
+  int32_t* keep;                 /* keep: queries whose arg-max is not the last class, ascending, [Q] */
+  int32_t* kept;                 /* keep: their count, [1] */
+  int32_t kq;                    /* ssc: kept queries (0: the level has no ssc term) */
+  const float* L;                /* ssc: row j of the class logits at L + rows[j]·ldL (rows NULL: j), K columns */
+  const int32_t* L_rows;
+  int32_t ldL, K;
+  float* ssc;                    /* [n][K] */
+  const float* g_ssc;            /* ssc backward: [n][K] */
+  float* gF_ssc;                 /* [n][Q], the kept columns written */
+  float* gL;                     /* [kq][K] */
+} pasco_setloss_level;
+
+/* keep: helper.py:20-23's kept queries of every level, built on the device.  1 <= Q <= 4096, 2 <= K1 <= 65.      */
+int pasco_setloss_keep_group(const pasco_setloss_level* lv, int32_t count, pasco_stream_t s);
+/* pasco_setloss_match_cost for every level with T >= 1.                                                             */
+int pasco_setloss_match_cost_group(const pasco_setloss_level* lv, int32_t count, float cost_mask, float cost_class,
+                                   float cost_dice, pasco_stream_t s);
+/* pasco_setloss_pair_sums / _pair_backward for every level with P >= 1.                                             */
+int pasco_setloss_pair_sums_group(const pasco_setloss_level* lv, int32_t count, pasco_stream_t s);
+int pasco_setloss_pair_backward_group(const pasco_setloss_level* lv, int32_t count, pasco_stream_t s);
+/* pasco_setloss_ssc_forward / _ssc_backward for every level with kq >= 1.                                           */
+int pasco_setloss_ssc_forward_group(const pasco_setloss_level* lv, int32_t count, pasco_stream_t s);
+int pasco_setloss_ssc_backward_group(const pasco_setloss_level* lv, int32_t count, pasco_stream_t s);
+
+/* One Lovász-softmax term: the fields of pasco_lovasz_errors / _grad / _backward.  perm holds row indices within the
+ * term, as in the one-term calls.                                                                                   */
+typedef struct {
+  const float* logits;           /* [P][C] */
+  int64_t P;
+  int32_t C;
+  const int32_t* labels;         /* [P] */
+  float* probs;                  /* [P][C] */
+  float* err;                    /* [C][P] */
+  const float* err_sorted;       /* [C][P] */
+  const int64_t* perm;           /* [C][P] */
+  float* grad;                   /* [C][P] */
+  float* loss;                   /* [C] */
+  const float* g;                /* [C] */
+  float* dx;                     /* [P][C] */
+} pasco_lovasz_term;
+
+int pasco_lovasz_errors_group(const pasco_lovasz_term* t, int32_t count, pasco_stream_t s);
+int pasco_lovasz_grad_group(const pasco_lovasz_term* t, int32_t count, pasco_stream_t s);
+int pasco_lovasz_backward_group(const pasco_lovasz_term* t, int32_t count, pasco_stream_t s);
+
 /* ---- point voxeliser grouping and the MIMO merge (csrc/voxel.cu); keys pack as the hash table's ---------------------
  * voxel_group: torch.unique(rows, dim=0, return_inverse=True) for rows [n][4] (int32, or int64 when is_i64)
  * (unet3d_sparse_v2.py:72-75).  Pass 1 inserts every row's key into table_keys (capacity, power of two >= 2n, filled

@@ -95,6 +95,15 @@ PROTOTYPES = {
     "pasco_lovasz_errors": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p]),
     "pasco_lovasz_grad": (C.c_int, [_p, _p, _p, _i64, _i32, _p, _p, _p]),
     "pasco_lovasz_backward": (C.c_int, [_p, _p, _p, _p, _p, _i64, _i32, _p, _p]),
+    "pasco_setloss_keep_group": (C.c_int, [_p, _i32, _p]),
+    "pasco_setloss_match_cost_group": (C.c_int, [_p, _i32, C.c_float, C.c_float, C.c_float, _p]),
+    "pasco_setloss_pair_sums_group": (C.c_int, [_p, _i32, _p]),
+    "pasco_setloss_pair_backward_group": (C.c_int, [_p, _i32, _p]),
+    "pasco_setloss_ssc_forward_group": (C.c_int, [_p, _i32, _p]),
+    "pasco_setloss_ssc_backward_group": (C.c_int, [_p, _i32, _p]),
+    "pasco_lovasz_errors_group": (C.c_int, [_p, _i32, _p]),
+    "pasco_lovasz_grad_group": (C.c_int, [_p, _i32, _p]),
+    "pasco_lovasz_backward_group": (C.c_int, [_p, _i32, _p]),
     "pasco_voxel_group": (C.c_int, [_p, _i32, _i64, _p, _i64, _p, _p, _p]),
     "pasco_voxel_group_order": (C.c_int, [_p, _i32, _i64, _p, _p, _i64, _p, _i64, _p, _p, _p]),
     "pasco_mimo_merge_cells": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _i64, _p, _p, _p]),
@@ -106,6 +115,32 @@ PROTOTYPES = {
     "pasco_mimo_batch": (C.c_int, [_p, _p, _p, _i32, _i64, _i32, _p, _p, _p, _p]),
     "pasco_sine_pos": (C.c_int, [_p, _i32, _i64, _i64, _p, _i32, _i32, _i32, _p, _i64, _i32, _p]),
 }
+
+
+
+class SetlossLevel(C.Structure):
+    """pasco_setloss_level: one output level of the grouped criterion calls."""
+    _fields_ = [("F", _p), ("n", _i64), ("Q", _i32), ("T", _i32), ("bits", _p), ("flags", _p), ("stats", _p),
+                ("query_logits", _p), ("K1", _i32), ("ids", _p), ("class_weight", _p), ("C", _p), ("qi", _p),
+                ("tj", _p), ("P", _i32), ("sums", _p), ("g_sums", _p), ("gF_pairs", _p), ("keep", _p), ("kept", _p),
+                ("kq", _i32), ("L", _p), ("L_rows", _p), ("ldL", _i32), ("K", _i32), ("ssc", _p), ("g_ssc", _p),
+                ("gF_ssc", _p), ("gL", _p)]
+
+
+class LovaszTerm(C.Structure):
+    """pasco_lovasz_term: one Lovász-softmax term of the grouped calls."""
+    _fields_ = [("logits", _p), ("P", _i64), ("C", _i32), ("labels", _p), ("probs", _p), ("err", _p),
+                ("err_sorted", _p), ("perm", _p), ("grad", _p), ("loss", _p), ("g", _p), ("dx", _p)]
+
+
+def table(struct, rows):
+    """A ctypes array of `struct` from dicts of its fields (tensors become device pointers, absent fields zero)."""
+    arr = (struct * max(1, len(rows)))()
+    for a, row in zip(arr, rows):
+        for k, v in row.items():
+            setattr(a, k, ptr(v) if isinstance(v, torch.Tensor) else v)
+    return arr
+
 
 _lib: Optional[C.CDLL] = None
 

@@ -623,25 +623,18 @@ def _evaluate_all_kitti360(self, ssc_confidence, i_infer, sem_prob, panop_out, s
 CRITERION_SYNCS = 1     # host synchronisations of one hooked compute_losses level or completion-loss call, at most
 
 
-def _pinned_to(vals, dtype, dev) -> torch.Tensor:
-    return torch.tensor(vals, dtype=dtype).pin_memory().to(dev, non_blocking=True)
-
-
-def _on(t, dev) -> torch.Tensor:
-    """t on `dev` without a blocking copy: host tensors (the reference keeps its class weights there) go through pinned
-    memory."""
-    t = torch.as_tensor(t)
-    return t if t.device == dev else t.pin_memory().to(dev, non_blocking=True)
+_pinned_to = ops.pinned_to
+_on = ops.on_device
 
 
 def _criterion_level(crit, outputs, targets, semantic_label, unknown_mask_dense, i_infer, min_C):
     """compute_losses for batch size 1 → (loss_label_agg, loss_mask_agg), or None where the saved original decides.
-    One host synchronisation: the cost matrix, the sampling counters and the ssc keep decision in one copy, at the
-    reference's own crossing before linear_sum_assignment.  Host inputs (class weights, labels, min_C) and the
-    assignment move through pinned memory."""
-    from scipy.optimize import linear_sum_assignment
+    The device work is criterion.DeviceCriterion's for one level with its ssc term: one host synchronisation for the
+    cost matrix, the sampling counters and the kept-query count, at the reference's own crossing before
+    linear_sum_assignment.  What stays here is the reference's: its objects, `loss_labels` and `CE_ssc_loss`."""
     from pasco.loss.losses import CE_ssc_loss
     from pasco.loss.matcher_sparse import HungarianMatcher
+    from .criterion import MAX_CLASSES, DeviceCriterion
     vl, ql = outputs["voxel_logits"], outputs["query_logits"]
     if len(targets) != 1 or type(crit.matcher) is not HungarianMatcher or min_C is None:
         return None
@@ -650,59 +643,39 @@ def _criterion_level(crit, outputs, targets, semantic_label, unknown_mask_dense,
     if not (F_.is_cuda and ql.is_cuda and torch.is_tensor(masks) and masks.device == dev and masks.dim() == 4):
         return None
     K1 = ql.shape[-1]
-    K, Q, T, size = K1 - 1, F_.shape[1], masks.shape[0], tuple(masks.shape[1:])
-    if not (1 <= K <= 64 and Q == ql.shape[-2] and tuple(unknown_mask_dense.shape) == (1,) + size
+    K, Q, size = K1 - 1, F_.shape[1], tuple(masks.shape[1:])
+    if not (1 <= K <= MAX_CLASSES and Q == ql.shape[-2] and Q <= 4096 and tuple(unknown_mask_dense.shape) == (1,) + size
             and tuple(semantic_label.shape) == (1,) + size and unknown_mask_dense.device == dev
             and semantic_label.device == dev and F_.dtype == torch.float32):
         return None
-    class_weight = _on(crit.class_weights[i_infer], dev)
     pred_logit = ql[0]
-    Fd = F_.detach().contiguous()
-    bits, flags, lab, stats = ops.setloss_sample(vl.C.to(torch.int32).contiguous(),
-                                                 _on(min_C, dev).reshape(3).to(torch.int32), masks,
-                                                 unknown_mask_dense[0], semantic_label[0], K)
-    labels = _on(labels, dev)
-    ids = labels.to(torch.int32)
-    m = crit.matcher
-    cost = (ops.match_cost(Fd, bits, T, flags, stats, pred_logit.detach().float().contiguous(), ids,
-                           class_weight.float().contiguous(), m.cost_mask, m.cost_class, m.cost_dice)
-            if T else torch.zeros(Q, 0, device=dev))
-    keep = F.softmax(pred_logit.detach(), dim=-1).max(-1)[1] != K                  # helper.py:20-23
-    host = torch.cat([cost.reshape(-1).view(torch.int32), stats, keep.to(torch.int32)]).cpu()   # the one sync
-    st = host[Q * T:Q * T + T + 5].tolist()
-    # the two present-class words are int32 on the host: read them unsigned, so that class 31 does not sign-extend
-    bad, present_bits, known = st[T + 1], (st[T + 2] & 0xFFFFFFFF) | ((st[T + 3] & 0xFFFFFFFF) << 32), st[T + 4]
-    keep_h = np.nonzero(host[Q * T + T + 5:].numpy())[0]
-    if bad or present_bits == 0 or len(keep_h) > 128:
+    dc = DeviceCriterion(dev)
+    dc.add_subnet(vl.C, min_C, masks, unknown_mask_dense[0], semantic_label[0], labels, crit.class_weights[i_infer], K,
+                  [(F_, pred_logit, True)])
+    if not dc.read(crit.matcher):
         return None                 # rows outside the volume, labels outside [0, K), no labelled row, > 128 kept
-    C_host = host[:Q * T].view(torch.float32).reshape(Q, T)
-    i, j = linear_sum_assignment(C_host)
-    qi_d, tj_d = _pinned_to(i, torch.int32, dev), _pinned_to(j, torch.int32, dev)
+    dc.run()
+    lv, sub = dc.levels[0], dc.subnets[0]
+    qi_d, tj_d, class_weight = lv["qi"], lv["tj"], sub["cw"]
 
     loss_label_agg = {"loss_ce": 0}
     loss_mask_agg = {"loss_mask": 0, "loss_dice": 0, "ssc_ce_loss": 0, "ssc_lovasz_loss": 0}
     # loss_labels (criterion_sparse.py:56-81) itself, given the assignment as device indices
-    loss_label = crit.loss_labels({"query_logits": pred_logit}, {"labels": labels}, (qi_d.long(), tj_d.long()),
+    loss_label = crit.loss_labels({"query_logits": pred_logit}, {"labels": sub["labels"]}, (qi_d.long(), tj_d.long()),
                                   class_weight)
     # loss_masks (criterion_sparse.py:83-112) from the per-pair sums over the known rows
-    sums = ops.PairSums.apply(F_, bits, T, flags, qi_d, tj_d) if len(i) else torch.zeros(0, 4, device=dev)
-    tgt_weights = class_weight[ids[tj_d.long()].long()]
-    loss_mask = sums[:, 0] / known * tgt_weights
-    loss_dice = (1 - (2 * sums[:, 1] + 1) / (sums[:, 2] + sums[:, 3] + 1)) * tgt_weights
+    loss_mask, loss_dice = DeviceCriterion.mask_dice(lv, class_weight[sub["ids"][tj_d.long()].long()])
     loss_label_agg["loss_ce"] += (loss_label["loss_ce"] * crit.weight_dict["loss_ce"]).mean()
     loss_mask_agg["loss_mask"] += (loss_mask * crit.weight_dict["loss_mask"]).mean()
     loss_mask_agg["loss_dice"] += (loss_dice * crit.weight_dict["loss_dice"]).mean()
 
     # compute_ssc_sparse_loss (criterion_sparse.py:180-209)
     ssc_ce_loss, ssc_lovasz_loss = 0, 0
-    if len(keep_h):
-        keep_d = _pinned_to(keep_h.tolist(), torch.int64, dev)
-        logits = ops.SscLogits.apply(F_, pred_logit[keep_d, :-1].float(), keep_d.to(torch.int32))
-        ssc_ce_loss += CE_ssc_loss(logits, torch.where(lab < 0, 0, lab).long(), crit.compl_labelweights)
-        present = [c for c in range(K) if present_bits >> c & 1 and c != 0]               # ignores=[0]
-        if present:
-            ssc_lovasz_loss += ops.lovasz_softmax(logits, lab, _pinned_to([c in present for c in range(K)],
-                                                                          torch.bool, dev))
+    if lv["ssc_logits"] is not None:
+        lab = sub["lab"]
+        ssc_ce_loss += CE_ssc_loss(lv["ssc_logits"], torch.where(lab < 0, 0, lab).long(), crit.compl_labelweights)
+        if lv["ssc_lovasz"] is not None:
+            ssc_lovasz_loss += lv["ssc_lovasz"]
     loss_mask_agg["ssc_ce_loss"] += ssc_ce_loss * crit.weight_dict["ssc_ce"]
     loss_mask_agg["ssc_lovasz_loss"] += ssc_lovasz_loss * crit.weight_dict["ssc_lovasz"]
     return loss_label_agg, loss_mask_agg
@@ -721,55 +694,30 @@ def _compute_losses(self, sem_logits_pruned_1_1, outputs, targets, semantic_labe
 
 def _sem_compl_loss(sem_labels, sem_logits_at_scales, min_Cs, max_Cs, class_frequencies, power, skip_empty):
     """losses.py:124-179 (power 1/3, pairs without a row inside the bounds skipped) and :71-121 (power 1/1.5) →
-    (CE, Lovász), or None where the saved original decides.  One host synchronisation for all (scale, subnet) pairs:
-    their in-bounds row counts and present classes; host bounds and the label weights move through pinned memory."""
-    pairs = []
+    (CE, Lovász), or None where the saved original decides.  The device work is criterion.DeviceCriterion's for all
+    (scale, subnet) pairs: one host synchronisation for their in-bounds row counts and present classes."""
+    from .criterion import MAX_CLASSES, DeviceCriterion, label_weights
+    dc = None
     for scale in sem_logits_at_scales:
         sem_logits = sem_logits_at_scales[scale]
         targets = sem_labels["1_{}".format(scale)]
-        fr = class_frequencies["1_{}".format(scale)]
-        w = fr / np.sum(fr)
-        w = np.power(np.amax(w) / w, power)
+        w = label_weights(class_frequencies["1_{}".format(scale)], power).tolist()
         for i_subnet in range(len(targets)):
             sl, target = sem_logits[i_subnet], targets[i_subnet]
             if not (sl.F.is_cuda and torch.is_tensor(target) and target.device == sl.F.device and target.dim() == 3
-                    and sl.F.dtype == torch.float32 and 1 <= sl.F.shape[1] <= 64):
+                    and sl.F.dtype == torch.float32 and 1 <= sl.F.shape[1] <= MAX_CLASSES):
                 return None
-            dev = sl.F.device
-            lo = _on(min_Cs[i_subnet], dev).reshape(1, 3)
-            hi = _on(max_Cs[i_subnet], dev).reshape(1, 3)
-            xyz = sl.C[:, 1:]
-            inside = ((xyz <= hi) & (xyz >= lo)).all(1)
-            cell = (xyz - lo) // scale
-            X, Y, Z = target.shape
-            ok = inside & (cell >= 0).all(1) & (cell[:, 0] < X) & (cell[:, 1] < Y) & (cell[:, 2] < Z)
-            cell = torch.where(ok[:, None], cell, 0).long()
-            t = target[cell[:, 0], cell[:, 1], cell[:, 2]].long()
-            C_ = sl.F.shape[1]
-            cls = torch.where(ok & (t < C_), t, C_)
-            counts = torch.zeros(C_ + 1, dtype=torch.int32, device=dev).scatter_add_(
-                0, cls, torch.ones_like(cls, dtype=torch.int32))
-            stat = torch.stack([inside.sum().to(torch.int32), (inside & ~ok).sum().to(torch.int32)])
-            pairs.append((sl, _pinned_to(w.tolist(), sl.F.dtype, dev), torch.where(ok, t, 255), torch.where(ok, t, -1).to(torch.int32),
-                          torch.cat([stat, (counts[:C_] > 0).to(torch.int32)]), C_))
-    if not pairs:
+            dc = dc or DeviceCriterion(sl.F.device)
+            dc.add_pair(sl, target, min_Cs[i_subnet], max_Cs[i_subnet], scale, w)
+    if dc is None:
         return None
-    host = torch.cat([p[4] for p in pairs]).cpu().tolist()                         # the one sync
-    ce_losses, lovasz_losses, at = [], [], 0
-    for sl, w, t_ce, t_lov, _, C_ in pairs:
-        n_in, bad, present = host[at], host[at + 1], host[at + 2:at + 2 + C_]
-        at += 2 + C_
-        if bad or (n_in and not any(present)) or (n_in == 0 and not skip_empty):
-            return None             # labels beyond the volume, no present class, or an empty pair the original decides
-        if n_in == 0:
-            continue
-        crit = torch.nn.CrossEntropyLoss(weight=w, ignore_index=255, reduction="mean")
-        ce_losses.append(crit(sl.F, t_ce))
-        lovasz_losses.append(ops.lovasz_softmax(sl.F, t_lov, _pinned_to([bool(v) for v in present], torch.bool,
-                                                                          sl.F.device)))
-    if len(ce_losses) == 0:
+    if not dc.read(None, skip_empty):
+        return None             # labels beyond the volume, no present class, or an empty pair the original decides
+    dc.run()
+    live = [pr for pr in dc.pairs if pr["n_in"] > 0]
+    if len(live) == 0:
         return 0.0, 0.0
-    return torch.stack(ce_losses).mean(), torch.stack(lovasz_losses).mean()
+    return torch.stack([pr["ce"] for pr in live]).mean(), torch.stack([pr["lovasz"] for pr in live]).mean()
 
 
 def _compute_sem_compl_loss(sem_labels, sem_logits_at_scales, min_Cs, max_Cs, class_frequencies):

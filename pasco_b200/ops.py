@@ -6,6 +6,7 @@ current stream and the autograd graph.  Row indices are int32, −1 = no row.
 from __future__ import annotations
 
 import ctypes as C
+import itertools
 import math
 import weakref
 from typing import List, Optional, Sequence, Tuple
@@ -1658,3 +1659,194 @@ def lovasz_softmax(logits: torch.Tensor, labels: torch.Tensor, present: torch.Te
     per = LovaszClasses.apply(logits.float(), labels)
     w = present.to(per.dtype)
     return (per * w).sum() / w.sum()
+
+
+# ------------------------------------------------------------------------------------------------
+# the criterion over a table of levels (pasco_setloss_*_group, pasco_lovasz_*_group): one launch per pass for all
+# levels; each level's arithmetic and summation order are those of the one-level calls above
+# ------------------------------------------------------------------------------------------------
+def on_device(t, dev) -> torch.Tensor:
+    """t on `dev` without a blocking copy: host tensors or lists (bounds, class weights, target classes) go through
+    pinned memory."""
+    t = torch.as_tensor(t)
+    return t if t.device == dev else t.pin_memory().to(dev, non_blocking=True)
+
+
+def pinned_to(vals, dtype, dev) -> torch.Tensor:
+    """A small host list on `dev` through pinned memory, without waiting for the device."""
+    return torch.tensor(vals, dtype=dtype).pin_memory().to(dev, non_blocking=True)
+
+
+def _group(name: str, struct, rows, *args):
+    if rows:
+        call(name, _lib.table(struct, rows), len(rows), *args)
+
+
+def setloss_keep_group(query_logits: Sequence[torch.Tensor]):
+    """helper.py:20-23 for every level: query_logits fp32 [Q, K1] each → (keep int32 [L, max Q], kept int32 [L]), the
+    ascending indices of the queries whose arg-max is not the last class and their count, per level."""
+    dev = query_logits[0].device
+    keep = torch.empty(len(query_logits), max(q.shape[0] for q in query_logits), dtype=torch.int32, device=dev)
+    kept = torch.empty(len(query_logits), dtype=torch.int32, device=dev)
+    _group("pasco_setloss_keep_group", _lib.SetlossLevel,
+           [dict(query_logits=q, Q=q.shape[0], K1=q.shape[1], keep=keep[i], kept=kept[i:i + 1])
+            for i, q in enumerate(query_logits)])
+    return keep, kept
+
+
+def match_cost_group(levels: Sequence[dict], cost_mask: float, cost_class: float, cost_dice: float) -> torch.Tensor:
+    """match_cost for every level: dicts of F, bits, T, flags, stats, query_logits, ids, class_weight (match_cost's
+    arguments) → one fp32 buffer holding each level's C [Q, T] in turn."""
+    sizes = [lv["F"].shape[1] * lv["T"] for lv in levels]
+    out = torch.empty(sum(sizes), dtype=torch.float32, device=levels[0]["F"].device)
+    rows, at = [], 0
+    for lv, sz in zip(levels, sizes):
+        F, ql = lv["F"], lv["query_logits"]
+        rows.append(dict(F=F, n=F.shape[0], Q=F.shape[1], T=lv["T"], bits=lv["bits"], flags=lv["flags"],
+                         stats=lv["stats"], query_logits=ql, K1=ql.shape[1], ids=lv["ids"],
+                         class_weight=lv["class_weight"], C=out[at:at + sz] if sz else None))
+        at += sz
+    _group("pasco_setloss_match_cost_group", _lib.SetlossLevel, rows, float(cost_mask), float(cost_class),
+           float(cost_dice))
+    return out
+
+
+class PairSumsGroup(torch.autograd.Function):
+    """PairSums for every level: apply(meta, *F) with meta one (bits, T, flags, qi, tj) per level and F fp32 [N, Q]
+    each → fp32 [ΣP, 4], the levels' pairs in turn."""
+
+    @staticmethod
+    def forward(ctx, meta, *Fs):
+        Fs = [F.detach().contiguous() for F in Fs]
+        P = [m[3].shape[0] for m in meta]
+        out = torch.empty(sum(P), 4, dtype=torch.float32, device=Fs[0].device)
+        ctx.rows = []
+        for F, (bits, T, flags, qi, tj), p in zip(Fs, meta, P):
+            ctx.rows.append(dict(F=F, n=F.shape[0], Q=F.shape[1], T=T, bits=bits, flags=flags, qi=qi, tj=tj, P=p))
+        fwd, at = [], 0
+        for row, p in zip(ctx.rows, P):
+            if p:
+                fwd.append(dict(row, sums=out[at:at + p]))
+            at += p
+        _group("pasco_setloss_pair_sums_group", _lib.SetlossLevel, fwd)
+        ctx.P, ctx.keep_alive = P, (Fs, meta)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        g = g.contiguous()
+        gFs, rows, at = [], [], 0
+        for row, p in zip(ctx.rows, ctx.P):
+            gF = torch.zeros_like(row["F"])
+            gFs.append(gF)
+            if p:
+                rows.append(dict(row, g_sums=g[at:at + p], gF_pairs=gF))
+            at += p
+        _group("pasco_setloss_pair_backward_group", _lib.SetlossLevel, rows)
+        return (None, *gFs)
+
+
+class SscLogitsGroup(torch.autograd.Function):
+    """SscLogits for every level, the class logits read through the kept-query list: apply(meta, *F, *query_logits)
+    with meta one (keep int32 [≥ kq], kq) per level, F fp32 [N, Q], query_logits fp32 [Q, K+1] → one fp32 [N, K] per
+    level, out = normalised (σ(F[:, keep[:kq]]) + 1e-8) @ query_logits[keep[:kq], :K].  Every kq >= 1."""
+
+    @staticmethod
+    def forward(ctx, meta, *tensors):
+        L = len(meta)
+        Fs = [F.detach().contiguous() for F in tensors[:L]]
+        qls = [q.detach().contiguous() for q in tensors[L:]]
+        outs, rows = [], []
+        for F, ql, (keep, kq) in zip(Fs, qls, meta):
+            K = ql.shape[1] - 1
+            out = torch.empty(F.shape[0], K, dtype=torch.float32, device=F.device)
+            outs.append(out)
+            rows.append(dict(F=F, n=F.shape[0], Q=F.shape[1], keep=keep, kq=kq, L=ql, L_rows=keep, ldL=ql.shape[1], K=K,
+                             ssc=out))
+        _group("pasco_setloss_ssc_forward_group", _lib.SetlossLevel, rows)
+        ctx.rows, ctx.meta, ctx.keep_alive = rows, meta, (Fs, qls, outs)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *gs):
+        rows, gFs, gLs = [], [], []
+        for row, g, (keep, kq) in zip(ctx.rows, gs, ctx.meta):
+            gF = torch.zeros_like(row["F"])
+            gL = torch.empty(kq, row["K"], dtype=torch.float32, device=gF.device)
+            gFs.append(gF)
+            gLs.append(gL)
+            rows.append(dict(row, g_ssc=g.contiguous(), gF_ssc=gF, gL=gL))
+        _group("pasco_setloss_ssc_backward_group", _lib.SetlossLevel, rows)
+        gqs = []
+        for row, gL, (keep, kq) in zip(ctx.rows, gLs, ctx.meta):
+            gq = torch.zeros_like(row["L"])
+            gq[keep[:kq].long(), :row["K"]] = gL
+            gqs.append(gq)
+        return (None, *gFs, *gqs)
+
+
+def _segmented_descending(err: torch.Tensor, shapes: Sequence[Tuple[int, int]]):
+    """Sorts each class row of each term's [C, P] errors (the terms laid out in turn in the flat fp32 `err`) descending,
+    in one stable sort of int64 keys (row index << 32 | 0x7FFFFFFF − float bits), built in place: non-negative errors
+    order as their bits, the −1 of rows left out after all of them.  → (sorted errors, each position's row within its
+    term).  Temporaries: the key, the sorted key and the permutation, int64 each, the key freed before the gather."""
+    dev = err.device
+    key = err.view(torch.int32).to(torch.int64).neg_().add_(0x7FFFFFFF)
+    at, row0 = 0, 0
+    for C_, P in shapes:
+        key[at:at + C_ * P].view(C_, P).add_((torch.arange(row0, row0 + C_, device=dev) << 32).view(C_, 1))
+        at, row0 = at + C_ * P, row0 + C_
+    perm = torch.sort(key, stable=True)[1]
+    del key
+    err_sorted = err[perm]
+    at = 0
+    for C_, P in shapes:
+        perm[at:at + C_ * P].view(C_, P).sub_((at + P * torch.arange(C_, device=dev)).view(C_, 1))
+        at += C_ * P
+    return err_sorted, perm
+
+
+class LovaszGroup(torch.autograd.Function):
+    """LovaszClasses for every term: apply(labels, *logits) with labels one int32 [P] per term (LovaszClasses' label
+    convention) and logits fp32 [P, C] → fp32 [ΣC], each term's per-class Σ err·lovasz_grad in turn.  One errors
+    launch, one segmented sort of all terms' [C, P] errors, one grad launch."""
+
+    @staticmethod
+    def forward(ctx, labels, *logits):
+        xs = [x.detach().contiguous() for x in logits]
+        dev = xs[0].device
+        sizes = [x.numel() for x in xs]
+        err = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
+        probs = [torch.empty_like(x) for x in xs]
+        rows, at = [], 0
+        for x, lab, pr, sz in zip(xs, labels, probs, sizes):
+            rows.append(dict(logits=x, P=x.shape[0], C=x.shape[1], labels=lab, probs=pr, err=err[at:at + sz]))
+            at += sz
+        _group("pasco_lovasz_errors_group", _lib.LovaszTerm, rows)
+        err_sorted, perm = _segmented_descending(err, [(x.shape[1], x.shape[0]) for x in xs])
+        grad = torch.empty_like(err)
+        loss = torch.zeros(sum(x.shape[1] for x in xs), dtype=torch.float32, device=dev)     # a term without rows: 0
+        grows, at, c0 = [], 0, 0
+        for x, lab, sz in zip(xs, labels, sizes):
+            C_ = x.shape[1]
+            grows.append(dict(P=x.shape[0], C=C_, labels=lab, err_sorted=err_sorted[at:at + sz], perm=perm[at:at + sz],
+                              grad=grad[at:at + sz], loss=loss[c0:c0 + C_]))
+            at, c0 = at + sz, c0 + C_
+        _group("pasco_lovasz_grad_group", _lib.LovaszTerm, [r for r in grows if r["P"] > 0])
+        ctx.grows, ctx.keep_alive = grows, (probs, labels, perm, grad)
+        ctx.probs = probs
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        g = g.contiguous().float()
+        dxs, rows, c0 = [], [], 0
+        for r, pr in zip(ctx.grows, ctx.probs):
+            dx = torch.zeros_like(pr)
+            dxs.append(dx)
+            if r["P"] > 0:
+                rows.append(dict(probs=pr, labels=r["labels"], perm=r["perm"], grad=r["grad"], g=g[c0:c0 + r["C"]],
+                                 P=r["P"], C=r["C"], dx=dx))
+            c0 += r["C"]
+        _group("pasco_lovasz_backward_group", _lib.LovaszTerm, rows)
+        return (None, *dxs)

@@ -57,3 +57,17 @@ def make_scene(grid: Sequence[int] = (256, 256, 32), occ: float = 0.10, n_infers
     b["mask_boxes"] = boxes
     b["mask_classes"] = torch.randint(1, n_classes, (n_masks,), generator=g)
     return b
+
+
+def training_batch(scene: Dict, device="cuda") -> Dict:
+    """`make_scene`'s output (unchanged) plus the reference's training fields on `device`: sem_labels, semantic_label
+    [M, X, Y, Z] (the scale-1 labels), dense mask_label (one {"labels" uint8 [T], "masks" bool [T, X, Y, Z]} per subnet,
+    the scene's boxes) and geo_labels["1_1"] (occupancy, float).  Inputs stay on the host."""
+    sem = scene["sem_labels"]["1_1"].to(device)
+    grid = tuple(sem.shape[1:])
+    masks = torch.zeros(len(scene["mask_boxes"]), *grid, dtype=torch.bool)
+    for i, (lo, hi) in enumerate(scene["mask_boxes"]):
+        masks[i, lo[0]:hi[0], lo[1]:hi[1], lo[2]:hi[2]] = True
+    label = {"labels": scene["mask_classes"].to(torch.uint8).to(device), "masks": masks.to(device)}
+    return dict(scene, sem_labels={k: v.to(device) for k, v in scene["sem_labels"].items()}, semantic_label=sem,
+                geo_labels={"1_1": (sem > 0).float()}, mask_label=[label] * sem.shape[0])

@@ -32,15 +32,10 @@ from postprocess_bench import batch_of, calibrate, reference_net  # noqa: E402
 
 def train_batch(make_scene, M, seed):
     """A reference-format training batch: the scene of batch_of plus dense labels and instance masks."""
-    sc = make_scene(GRID, OCC, M, IN_CH, N_CLASSES, seed=seed)
+    from pasco_b200.synthetic import training_batch
+    tb = training_batch(make_scene(GRID, OCC, M, IN_CH, N_CLASSES, seed=seed))
     b = batch_of(make_scene, M, seed)
-    sem = sc["sem_labels"]["1_1"].cuda()
-    masks = torch.zeros(len(sc["mask_boxes"]), *GRID, dtype=torch.bool)
-    for i, (lo, hi) in enumerate(sc["mask_boxes"]):
-        masks[i, lo[0]:hi[0], lo[1]:hi[1], lo[2]:hi[2]] = True
-    label = {"labels": sc["mask_classes"].to(torch.uint8).cuda(), "masks": masks.cuda()}
-    b.update(sem_labels={k: v.cuda() for k, v in sc["sem_labels"].items()}, semantic_label=sem,
-             geo_labels={"1_1": (sem > 0).float()}, mask_label=[label] * M)
+    b.update({k: tb[k] for k in ("sem_labels", "semantic_label", "geo_labels", "mask_label")})
     return b
 
 
