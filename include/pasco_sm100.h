@@ -281,6 +281,13 @@ int pasco_pose_lookup(const uint64_t* table_keys, const int32_t* table_vals, int
 int pasco_cell_mask_or(const int32_t* cell_row, int64_t n, uint8_t* mask, pasco_stream_t s);
 /* out[r] = cell_row[lin[r]] */
 int pasco_lookup_rows(const int32_t* cell_row, const int32_t* lin, int64_t n, int32_t* out, pasco_stream_t s);
+/* Net.step's subnet box (net_panoptic_sparse.py:430-459): every row r of coords int32 [n, 4] (b, x, y, z; b ignored)
+ * with lo <= (x, y, z) <= hi sets cell_row[cell] = r at cell (x, y, z) − lo of the X x Y x Z box (cell_row filled with
+ * −1 by the caller; hi − lo below the box size) and cell_mask[cell] = 1 (zeroed by the caller); counts int32 [2]
+ * (zeroed) += the rows outside [lo, hi], the rows at a cell another row already holds (which row holds it is then
+ * unspecified).  Integer atomics only.                                                                             */
+int pasco_box_cells(const int32_t* coords, int64_t n, const int32_t lo[3], const int32_t hi[3], int32_t X, int32_t Y,
+                    int32_t Z, int32_t* cell_row, uint8_t* cell_mask, int32_t* counts, pasco_stream_t s);
 
 /* ensembler.py:40-58 for the masks: out[r, q] = sigmoid(logits[rows[r], q]) fp32 [n, Q]; optionally (hi != NULL) the
  * bf16 planes hi = bf16(out), lo = bf16(out − hi) [n, Qp], Qp % 16 == 0, columns past Q zero; colsum (NULL allowed)

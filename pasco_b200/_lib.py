@@ -65,6 +65,7 @@ PROTOTYPES = {
     "pasco_pose_lookup": (C.c_int, [_p, _p, _i64, _p, _i32, _i32, _i32, _p, _p, _p]),
     "pasco_cell_mask_or": (C.c_int, [_p, _i64, _p, _p]),
     "pasco_lookup_rows": (C.c_int, [_p, _p, _i64, _p, _p]),
+    "pasco_box_cells": (C.c_int, [_p, _i64, _p, _p, _i32, _i32, _i32, _p, _p, _p, _p]),
     "pasco_mask_rows_sigmoid": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _p, _i32, _p, _p, _p]),
     "pasco_mask_merge": (C.c_int, [_p, _p, _i32, _p, _p, _i32, _p, _i64, _p, _p, _i32, _i32, _p, _p, _p, _p, _i32, _p, _p, _p]),
     "pasco_softmax_rows": (C.c_int, [_p, _p, _i64, _i32, _p, _p]),

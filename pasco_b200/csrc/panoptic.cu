@@ -57,6 +57,49 @@ __global__ void k_lookup_rows(const int32_t* __restrict__ cell_row, const int32_
     out[i] = __ldg(cell_row + __ldg(lin + i));
 }
 
+// subnet box (net_panoptic_sparse.py:430-459): a row at (x, y, z) in [lo, hi] (inclusive) takes the cell (x, y, z) − lo of
+// the X x Y x Z box.  A row outside [lo, hi], or at a cell another row already holds, is only counted; the per-warp
+// counts reach counts[] as integer atomics.
+struct BoxBounds {
+  int lo[3], hi[3];
+};
+
+__global__ void k_box_cells(const int32_t* __restrict__ coords, int64_t n, const BoxBounds b, int X, int Y, int Z,
+                            int32_t* __restrict__ cell_row, uint8_t* __restrict__ cell_mask, int32_t* __restrict__ counts) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int lane = threadIdx.x & 31;
+  int outside = 0, taken = 0;
+  // every lane of a warp runs the same trip count, so the whole warp reaches the reductions below
+  for (int64_t base = blockIdx.x * (int64_t)blockDim.x + threadIdx.x - lane; base < n; base += stride) {
+    const int64_t i = base + lane;
+    if (i >= n) continue;
+    int64_t c[3];
+    bool in = true;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      const int v = __ldg(coords + 4 * i + 1 + d);
+      in = in && v >= b.lo[d] && v <= b.hi[d];
+      c[d] = (int64_t)v - b.lo[d];
+    }
+    if (!in) {
+      ++outside;
+      continue;
+    }
+    const int64_t cell = (c[0] * Y + c[1]) * Z + c[2];
+    if (atomicCAS(cell_row + cell, -1, (int32_t)i) != -1) {
+      ++taken;
+      continue;
+    }
+    cell_mask[cell] = 1;
+  }
+  outside = __reduce_add_sync(0xffffffffu, outside);
+  taken = __reduce_add_sync(0xffffffffu, taken);
+  if (lane == 0) {
+    if (outside) atomicAdd(counts, outside);
+    if (taken) atomicAdd(counts + 1, taken);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // mask rows: sigmoid gather (MERGE = false) or matched running average (MERGE = true), with the bf16 hi/lo planes,
 // the per-CTA column partial sums and the non-zero flag of every row.  Block (32, 8): lanes over columns, 8 row lanes;
@@ -522,6 +565,26 @@ extern "C" int pasco_lookup_rows(const int32_t* cell_row, const int32_t* lin, in
   if (n == 0) return 0;
   k_lookup_rows<<<grid_for(n, 256), 256, 0, (cudaStream_t)s>>>(cell_row, lin, n, out);
   PASCO_CHECK_LAUNCH("pasco_lookup_rows");
+  return 0;
+}
+
+extern "C" int pasco_box_cells(const int32_t* coords, int64_t n, const int32_t lo[3], const int32_t hi[3], int32_t X,
+                               int32_t Y, int32_t Z, int32_t* cell_row, uint8_t* cell_mask, int32_t* counts,
+                               pasco_stream_t s) {
+  PASCO_CHECK_ARG(X > 0 && Y > 0 && Z > 0, "pasco_box_cells: empty box");
+  PASCO_CHECK_ARG((int64_t)X * Y * Z <= INT32_MAX, "pasco_box_cells: %d x %d x %d cells exceed the int32 cell maps", X, Y, Z);
+  PASCO_CHECK_ARG(n <= INT32_MAX, "pasco_box_cells: %lld rows exceed the int32 cell map", (long long)n);
+  BoxBounds b;
+  const int32_t size[3] = {X, Y, Z};
+  for (int d = 0; d < 3; ++d) {
+    PASCO_CHECK_ARG((int64_t)hi[d] - lo[d] < size[d], "pasco_box_cells: bounds [%d, %d] exceed the box's %d cells on axis %d",
+                    lo[d], hi[d], size[d], d);
+    b.lo[d] = lo[d];
+    b.hi[d] = hi[d];
+  }
+  if (n == 0) return 0;
+  k_box_cells<<<grid_for(n, 256), 256, 0, (cudaStream_t)s>>>(coords, n, b, X, Y, Z, cell_row, cell_mask, counts);
+  PASCO_CHECK_LAUNCH("pasco_box_cells");
   return 0;
 }
 

@@ -39,6 +39,8 @@ from .predict import THING_IDS
 NLL_EPS = 1e-12                     # SSCMetrics.add_batch_ece
 INS_NLL_EPS = 1e-8                  # UncertaintyMetrics.get_stats
 MATCH_IOU = 0.5                     # the reference's single uncertainty threshold (net_panoptic_sparse.py:198)
+VAL_UPDATE_SYNCS = 3                # host synchronisations of Evaluator(uncertainty=False).update for one entry: the mask
+                                    # labels (when on the device), the ground-truth counts, the entry's tables
 
 
 def calibration_error(conf: torch.Tensor, correct: torch.Tensor) -> torch.Tensor:

@@ -1267,6 +1267,22 @@ def lookup_rows(cell_row: torch.Tensor, lin: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def box_cells(coords: torch.Tensor, lo: Sequence[int], hi: Sequence[int], size: Sequence[int], counts: torch.Tensor):
+    """The rows of coords ([N, 4] (b, x, y, z), b ignored) with lo <= (x, y, z) <= hi at cells (x, y, z) − lo of the box
+    `size` → (cell_row int32 [cells], −1 = none; cell_row >= 0 as uint8).  counts (int32 [2] on the device, zeroed)
+    receives the number of rows outside [lo, hi] and of rows at a cell another row already holds; nothing is read back."""
+    X, Y, Z = (int(s) for s in size)
+    dev = coords.device
+    c = coords if coords.dtype == torch.int32 and coords.is_contiguous() else coords.to(torch.int32).contiguous()
+    if c.dim() != 2 or c.shape[1] != 4:
+        raise ValueError(f"box_cells: coordinates must be [N, 4], got {tuple(coords.shape)}")
+    cell_row = torch.full((X * Y * Z,), -1, dtype=torch.int32, device=dev)
+    mask = torch.zeros(X * Y * Z, dtype=torch.uint8, device=dev)
+    call("pasco_box_cells", ptr(c), c.shape[0], int_array(lo), int_array(hi), X, Y, Z, ptr(cell_row), ptr(mask),
+         ptr(counts))
+    return cell_row, mask
+
+
 def _mask_outputs(n: int, q: int, dev, planes: bool, colsum: bool):
     qp = plane_cols(q)
     out = torch.empty(n, q, dtype=torch.float32, device=dev)

@@ -186,6 +186,102 @@ def mask_rows(masks: Sequence[Dict], qprobs: Sequence[torch.Tensor], gate: torch
     return rows, qprobs + [a_q]
 
 
+# ------------------------------------------------------------------------------------------------
+# Net.step's per-step evaluation (net_panoptic_sparse.py:425-475): one subnet of a training forward, in its own box
+# ------------------------------------------------------------------------------------------------
+STEP_ENTRY_SYNCS = 2    # host synchronisations per subnet of step_entries: the box check, then the segment records
+                        # (one more per call reads min_Cs / max_Cs when they are device tensors)
+
+
+def step_box(min_C, max_C):
+    """(min_C, max_C, size) as host int tuples: size = compute_scene_size(min_C, max_C, scale=8) (misc.py:30), the box
+    of ceil((max − min + 1) / 8)·8 cells per axis from min_C that Net.step evaluates a subnet in."""
+    lo, hi = (torch.as_tensor(v).reshape(-1)[-3:] for v in (min_C, max_C))
+    dev = lo.device if lo.is_cuda else hi.device
+    both = torch.cat([lo.to(dev, torch.int64), hi.to(dev, torch.int64)]).cpu().tolist()
+    lo, hi = both[:3], both[3:]
+    size = tuple(int(np.ceil((h - l + 1) / 8.0)) * 8 for l, h in zip(lo, hi))
+    if min(size) <= 0:
+        raise ValueError(f"step_entries: empty box from min_C {lo} to max_C {hi}")
+    return tuple(lo), tuple(hi), size
+
+
+def _outside_rows_host(C: torch.Tensor, lo, size) -> int:
+    xyz = C[:, -3:].long() - torch.tensor(lo).view(1, 3)
+    return int(((xyz < 0) | (xyz >= torch.tensor(size).view(1, 3))).any(1).sum())
+
+
+def step_entries(out: Dict, batch: Dict, subnets: Sequence[int], *, thing_ids=THING_IDS, overlap_threshold: float = 0.4,
+                 object_mask_threshold: float = 0.7) -> List[Dict]:
+    """One entry per listed subnet i of a training-mode forward output `out` (PascoNet.forward(..., predict_panop=True)),
+    in the format postprocess emits, for metrics.Evaluator(n_entries=1, uncertainty=False): what Net.step evaluates
+    every training step (net_panoptic_sparse.py:430-459), on rows instead of dense volumes.
+
+    The box is min_C = batch["min_Cs"][i] with step_box's size; `lin` and `ssc_lin` are cells (coord − min_C) of it,
+    ascending.  The masks are the sigmoid of panop_predictions[i]["voxel_logits"] with the softmax of its query logits
+    through the panoptic passes; every mask row must lie in the box (PascoNet.predict_panop crops to it), a row outside
+    raises.  The semantics are the softmax of the scale-1 sem_logits_at_scales[1][i] rows inside [min_C, max_C]
+    (prune_outside_coords; other rows are dropped): ssc_pred the argmax, ssc_confidence the max.  The reference densifies zero logits at the box
+    cells without a row, whose softmax is uniform with argmax class 0; Evaluator counts a known cell without a row as
+    prediction 0, so its SSC counts are the reference's without those cells being written.  batch["semantic_label"][i]
+    must have the box's shape.  ValueError on bad subnet indices, a label of another shape, rows outside the box or
+    two rows at one cell, and CPU tensors.  STEP_ENTRY_SYNCS host synchronisations per subnet, whatever Q."""
+    preds = out.get("panop_predictions") or []
+    subnets = list(subnets)
+    bad = [i for i in subnets if not (isinstance(i, (int, np.integer)) and not isinstance(i, bool) and 0 <= i < len(preds))]
+    if bad:
+        raise ValueError(f"step_entries: subnets {bad} are not indices of the {len(preds)} panoptic predictions")
+    entries = []
+    for i in subnets:
+        i = int(i)
+        lo, hi, size = step_box(batch["min_Cs"][i], batch["max_Cs"][i])
+        label = batch["semantic_label"][i]
+        if tuple(label.shape) != size:
+            raise ValueError(f"step_entries: subnet {i}: semantic_label has shape {tuple(label.shape)}, the box from "
+                             f"{list(lo)} is {list(size)}")
+        vl, ql, sl = preds[i]["voxel_logits"], preds[i]["query_logits"], out["sem_logits_at_scales"][1][i]
+        if not all(t.is_cuda for t in (vl.F, vl.C, ql, sl.F, sl.C)):
+            n = _outside_rows_host(vl.C, lo, size)
+            if n:
+                raise ValueError(f"step_entries: subnet {i}: {n} mask rows outside the box {list(size)} at {list(lo)}")
+            raise ValueError("step_entries: the panoptic and semantic passes take CUDA tensors")
+        entries.append(_step_entry(i, vl, ql, sl, lo, hi, size, thing_ids, overlap_threshold, object_mask_threshold))
+    return entries
+
+
+def _step_entry(i, vl, ql, sl, lo, hi, size, thing_ids, overlap_threshold, object_mask_threshold) -> Dict:
+    counts = torch.zeros(4, dtype=torch.int32, device=vl.F.device)
+    m_cell, m_mask = ops.box_cells(vl.C, lo, [l + s - 1 for l, s in zip(lo, size)], size, counts[:2])   # the whole box
+    s_cell, s_mask = ops.box_cells(sl.C, lo, hi, size, counts[2:])                        # prune_outside_coords' bounds
+    m_out, m_dup, s_out, s_dup = counts.cpu().tolist()                                     # the box check
+    if m_out or m_dup or s_dup:
+        raise ValueError(f"step_entries: subnet {i}: {m_out} mask rows outside the box {list(size)} at {list(lo)}; "
+                         f"{m_dup} mask rows and {s_dup} semantic rows at a cell another row holds")
+    lin, _, _ = ops.compact(m_mask, total=vl.F.shape[0])
+    prob = ops.mask_rows_sigmoid(vl.F, ops.lookup_rows(m_cell, lin), planes=False)[0]
+    qp = F.softmax(ql.detach().float(), -1)[0]
+    pan, sem, conf, records = ops.panoptic(prob, qp, overlap_threshold, object_mask_threshold, thing_ids)   # records
+    s_lin, s_new, _ = ops.compact(s_mask, total=sl.F.shape[0] - s_out)           # s_new: cell → row of s_lin's order
+    s_pred, s_conf = ops.sem_ensemble([ops.softmax_rows(sl.F, ops.lookup_rows(s_cell, s_lin))], [s_new], s_lin)
+    return {"lin": lin.long(), "panoptic_seg": pan, "semantic_seg": sem, "vox_confidence": conf,
+            "segments_info": _segments(records, qp), "ssc_lin": s_lin.long(), "ssc_pred": s_pred,
+            "ssc_confidence": s_conf, "query_probs": qp}
+
+
+def evaluate_step(out: Dict, batch: Dict, metrics: Dict, *, thing_ids=THING_IDS, overlap_threshold: float = 0.4,
+                  object_mask_threshold: float = 0.7) -> None:
+    """Net.step's evaluate_all(compute_uncertainty=False) calls (net_panoptic_sparse.py:425-475): metrics = {subnet:
+    metrics.Evaluator(n_entries=1, uncertainty=False)} accumulates step_entries' entry of that subnet against
+    batch["semantic_label"][i] and batch["mask_label"][i] — pq_stat["train"][i] and ssc_metrics["train"][i].  Every
+    entry is built before any Evaluator is touched."""
+    subnets = sorted(metrics)
+    with torch.no_grad():
+        entries = step_entries(out, batch, subnets, thing_ids=thing_ids, overlap_threshold=overlap_threshold,
+                               object_mask_threshold=object_mask_threshold)
+        for i, e in zip(subnets, entries):
+            metrics[i].update([e], batch["semantic_label"][i], batch["mask_label"][i])
+
+
 _DENSE = {"panoptic_seg": ("lin", 0.0), "semantic_seg": ("lin", 0.0), "vox_confidence": ("lin", 0.0),
           "ssc_pred": ("ssc_lin", 0.0), "ssc_confidence": ("ssc_lin", 1.0)}
 
