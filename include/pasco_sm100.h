@@ -591,6 +591,71 @@ int pasco_mimo_batch(const float* const* feats, const int32_t* const* coords, co
 int pasco_sine_pos(const void* coords, int32_t is_i64, int64_t P, int64_t coord_pitch, const float* table, int32_t lo,
                    int32_t rows, int32_t n, float* out, int64_t out_pitch, int32_t add, pasco_stream_t s);
 
+/* ---- SemanticKITTI scene preparation (pasco/data/semantic_kitti/kitti_dataset.py:142-490, collate.py) ----
+ * One item: label volumes sem / inst uint8 [X, Y, Z] (C order), a pose T and its inverse Ti (fp32 row-major 4x4, host
+ * arrays), points fp32 [N, pitch] (x, y, z, then intensity columns).  Cells are transformed as transform_utils.transform
+ * does, in fp32 (c * 0.2 + 0.1 + min_bound, T with fused multiply-adds in k order, (p − min_bound − 0.1) / 0.2,
+ * round half to even); points as load_data_v3 does (numpy floor_divide in fp64, then transform).  stats int32
+ * [PASCO_SCENE_STATS] collects each phase's integer results at the offsets below (pasco_scene_source initialises it);
+ * bounds fp64 [4] are the crop's (new_min x, new_min y, new_max x, new_max y), ±inf without a crop.              */
+enum {
+  PASCO_SCENE_BND = 0,            /* min[3], max[3] of transform(nonzero(sem != 255), T)                   */
+  PASCO_SCENE_N_LABELLED = 6,     /* source cells with sem != 255                                           */
+  PASCO_SCENE_N_INSTANCE = 7,     /* source cells with inst != 0                                            */
+  PASCO_SCENE_SEM_EXT = 8,        /* min[3], max[3] of the semantic rows of the transformed box             */
+  PASCO_SCENE_N_SEM_ROWS = 14,    /* semantic rows of the transformed box                                   */
+  PASCO_SCENE_BOX = 16,           /* min[3], max[3] of the semantic and instance rows the crop keeps        */
+  PASCO_SCENE_N_SEM_KEPT = 22,    /* semantic rows the crop keeps                                           */
+  PASCO_SCENE_N_POINTS = 23,      /* points inside the extent                                               */
+  PASCO_SCENE_N_POINTS_KEPT = 24, /* of those, points the crop keeps                                        */
+  PASCO_SCENE_CLS_ORIGIN = 256,   /* [256] flags: classes of the source semantic volume                     */
+  PASCO_SCENE_INST_ORIGIN = 512,  /* [256] flags: ids of the source instance volume other than 0            */
+  PASCO_SCENE_CLS = 768,          /* [256] flags: classes of the kept semantic rows                         */
+  PASCO_SCENE_INST = 1024,        /* [256] flags: ids of the kept instance rows                             */
+  PASCO_SCENE_STATS = 1280
+};
+/* initialises stats; BND, N_LABELLED, N_INSTANCE and the *_ORIGIN flags.  X, Y, Z >= 2.                              */
+int pasco_scene_source(const uint8_t* sem, const uint8_t* inst, int32_t X, int32_t Y, int32_t Z, const float T[16],
+                       int32_t* stats, pasco_stream_t s);
+/* transform_scene over the box [lo, lo + G) (lo, G host arrays): gs / gi uint8 [G0, G1, G2] = source label + 1 (uint8,
+ * so 255 → 0 = no row) at grid_sample's nearest source cell of Ti · centre, 0 outside; gi only with with_inst (the
+ * source has an instance id other than 0).  SEM_EXT and N_SEM_ROWS.                                                   */
+int pasco_scene_resample(const uint8_t* sem, const uint8_t* inst, int32_t X, int32_t Y, int32_t Z, const float Ti[16],
+                         const int32_t lo[3], const int32_t G[3], int32_t with_inst, uint8_t* gs, uint8_t* gi,
+                         int32_t* stats, pasco_stream_t s);
+/* KittiDataset.crop's bounds from SEM_EXT and draw (np.random.rand(3), host array; NULL without a crop): crop_size =
+ * (max − min) · 0.8 in fp32, new_min = min + (max − min − crop_size) · draw in fp64.  train = 0: ±inf.                 */
+int pasco_scene_crop(const int32_t* stats, const double draw[3], int32_t train, double* bounds, pasco_stream_t s);
+/* BOX, N_SEM_KEPT, CLS and INST over the rows of gs / gi inside the crop                                              */
+int pasco_scene_crop_stats(const uint8_t* gs, const uint8_t* gi, const int32_t lo[3], const int32_t G[3],
+                           int32_t with_inst, const double* bounds, int32_t* stats, pasco_stream_t s);
+/* per point: ext[i] = inside the extent, keep[i] = ext and its transformed voxel inside the crop; N_POINTS and
+ * N_POINTS_KEPT.                                                                                                       */
+int pasco_scene_points(const float* pts, int64_t N, int32_t pitch, const float T[16], const double* bounds, uint8_t* ext,
+                       uint8_t* keep, int32_t* stats, pasco_stream_t s);
+/* keep_rows int32 [n_keep] (ascending point indices): feats fp32 [n_keep, V + pitch − 3 + 1 + E + 6] = (vote fp32 [N, V],
+ * intensity, radius, embedding emb fp32 [E, N] transposed, xyz − voxel centre, xyz) and coords int64 [n_keep, 3];
+ * ext_rows int32 [n_ext]: xyz fp64 [n_ext, 3] = xyz − vox_origin and label_out [n_ext] = label & 0xFFFF.             */
+int pasco_scene_point_rows(const float* pts, int32_t pitch, const float* vote, int32_t V, const float* emb, int32_t E,
+                           int64_t N, const int32_t* keep_rows, int64_t n_keep, const float T[16], float* feats,
+                           int64_t* coords, const int32_t* label, const int32_t* ext_rows, int64_t n_ext, double* xyz,
+                           int32_t* label_out, pasco_stream_t s);
+/* the item's volumes on the box [box_lo, box_lo + size) (host arrays) from the kept rows of gs / gi: sem (255 where no
+ * row), inst (0 where no row) and geo = complete_voxel as uint8 (0 empty, 1 labelled, 255 unknown), all uint8.        */
+int pasco_scene_box(const uint8_t* gs, const uint8_t* gi, const int32_t lo[3], const int32_t G[3], int32_t with_inst,
+                    const double* bounds, const int32_t box_lo[3], const int32_t size[3], uint8_t* sem, uint8_t* inst,
+                    uint8_t* geo, pasco_stream_t s);
+/* sem_labels / geo_labels at scale 2 or 4 (kitti_dataset.py:217-266) of sem uint8 [X, Y, Z] (multiples of the scale):
+ * geo = 255 if the whole block is 255, else whether a cell is labelled 1-254; sem = the first class of 1-19 with the
+ * most cells, and without one 0 if the whole block is 255, else 255.  Outputs uint8 [X/s, Y/s, Z/s].                 */
+int pasco_scene_scale(const uint8_t* sem, int32_t X, int32_t Y, int32_t Z, int32_t scale, uint8_t* sem_out,
+                      uint8_t* geo_out, pasco_stream_t s);
+/* prepare_mask_label of sem / inst uint8 [cells]: slot int32 [512] (device) gives the mask of class c at slot[c] and of
+ * instance id at slot[256 + id], −1 for none.  masks bool [n_masks, cells] (zero-filled here), labels uint8 [n_masks]:
+ * the class of a class mask, sem at the first cell in C order of an instance mask.  cells < 2^31.                     */
+int pasco_scene_masks(const uint8_t* sem, const uint8_t* inst, int64_t cells, const int32_t* slot, int32_t n_masks,
+                      uint8_t* masks, uint8_t* labels, pasco_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

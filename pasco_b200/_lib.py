@@ -115,6 +115,16 @@ PROTOTYPES = {
     "pasco_panop_crop": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p]),
     "pasco_mimo_batch": (C.c_int, [_p, _p, _p, _i32, _i64, _i32, _p, _p, _p, _p]),
     "pasco_sine_pos": (C.c_int, [_p, _i32, _i64, _i64, _p, _i32, _i32, _i32, _p, _i64, _i32, _p]),
+    "pasco_scene_source": (C.c_int, [_p, _p, _i32, _i32, _i32, _p, _p, _p]),
+    "pasco_scene_resample": (C.c_int, [_p, _p, _i32, _i32, _i32, _p, _p, _p, _i32, _p, _p, _p, _p]),
+    "pasco_scene_crop": (C.c_int, [_p, _p, _i32, _p, _p]),
+    "pasco_scene_crop_stats": (C.c_int, [_p, _p, _p, _p, _i32, _p, _p, _p]),
+    "pasco_scene_points": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p, _p]),
+    "pasco_scene_point_rows": (C.c_int, [_p, _i32, _p, _i32, _p, _i32, _i64, _p, _i64, _p, _p, _p, _p, _p, _i64, _p,
+                                         _p, _p]),
+    "pasco_scene_box": (C.c_int, [_p, _p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p]),
+    "pasco_scene_scale": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p, _p]),
+    "pasco_scene_masks": (C.c_int, [_p, _p, _i64, _p, _i32, _p, _p, _p]),
 }
 
 

@@ -450,6 +450,14 @@ class DeviceCriterion:
         return s[:, 0] / lv["sub"]["known"] * tw, (1 - (2 * s[:, 1] + 1) / (s[:, 2] + s[:, 3] + 1)) * tw
 
 
+def _on_device(v) -> bool:
+    """A CUDA tensor, stacked over the subnets or one subnet's, or a list / tuple of per-subnet CUDA tensors (collate_fn
+    keeps per-item volumes as lists: each item has its own box)."""
+    if isinstance(v, (list, tuple)):
+        return len(v) > 0 and all(torch.is_tensor(t) and t.is_cuda for t in v)
+    return torch.is_tensor(v) and v.is_cuda
+
+
 def _covered(out, batch, criterion) -> bool:
     """What can be decided without reading the device: every prediction and label volume is a CUDA tensor, fp32
     logits, at most MAX_CLASSES classes, every level's rows those its subnet samples."""
@@ -459,12 +467,12 @@ def _covered(out, batch, criterion) -> bool:
     if not rows or not all(r.F.is_cuda and r.F.dtype == torch.float32 and 1 <= r.F.shape[1] <= MAX_CLASSES
                            for r in rows):
         return False
-    if not all(torch.is_tensor(v) and v.is_cuda for v in batch["sem_labels"].values()):
+    if not all(_on_device(v) for v in batch["sem_labels"].values()):
         return False
     if not preds:
         return True
     vols = [batch["semantic_label"], batch["geo_labels"]["1_1"]] + [ml["masks"] for ml in batch["mask_label"][:len(preds)]]
-    if not all(torch.is_tensor(v) and v.is_cuda for v in vols):
+    if not all(_on_device(v) for v in vols):
         return False
     for p in preds:
         n = p["voxel_logits"].F.shape[0]
